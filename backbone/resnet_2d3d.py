@@ -2,7 +2,7 @@
 
 Same constructors, parameter / buffer names (conv1, bn1, layerN.i.{conv1..3, bn1..3, downsample.0/1}) and the same
 initialisation (kaiming_normal_(fan_out) convs, BN weight 1 / bias 0; :147-153).  The modules only *hold* parameters:
-`forward` runs on the sm_100a kernels of coclr_b200 (implicit-GEMM convs, BatchNorm + residual add + ReLU fused into
+`forward` runs on the sm_90a kernels of coclr_b200 (implicit-GEMM convs, BatchNorm + residual add + ReLU fused into
 one pass); there is no PyTorch/cuDNN execution path and no CPU path.
 """
 import torch.nn as nn

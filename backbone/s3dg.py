@@ -2,7 +2,7 @@
 
 Same constructor, same parameter / buffer names (incl. the `blockN.i` aliases the reference's
 state_dict carries) and the same initialisation (conv N(0, 0.01), BN weight 1 / bias 0; s3dg.py:20-22,
-51-56).  The modules below only *hold* parameters: the arithmetic of `forward` runs on the sm_100a
+51-56).  The modules below only *hold* parameters: the arithmetic of `forward` runs on the sm_90a
 kernels of coclr_b200 (implicit-GEMM convs with BatchNorm/ReLU folded around them); there is no
 PyTorch/cuDNN execution path and no CPU path.
 """

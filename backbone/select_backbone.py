@@ -4,7 +4,7 @@ from .resnet_2d3d import r2d3d50
 
 
 def select_backbone(network, first_channel=3):
-    """-> (module, {'feature_size': int}). 's3d', 's3dg' (S3D with feature gating) and 'r50' run on the sm_100a engine;
+    """-> (module, {'feature_size': int}). 's3d', 's3dg' (S3D with feature gating) and 'r50' run on the sm_90a engine;
     unknown names raise NotImplementedError as in the reference."""
     param = {'feature_size': 1024}
     if network == 's3d':

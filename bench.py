@@ -56,7 +56,38 @@ def parse():
     ap.add_argument("--breakdown", action="store_true", help="print the per-kernel time table of one step to stderr")
     ap.add_argument("--timeline", action="store_true",
                     help="per-phase CUDA-event timeline of one step (ms since step start, max over ranks) in the JSON line")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (loss, logits, labels, queue, "
+                         "a fixed sample of the updated parameters and of their gradient) as DIR/<name>.npy")
     return ap.parse_args()
+
+
+DUMP_SAMPLE = 1 << 20    # elements of the flat parameter / gradient buffers written by --dump-outputs (seeded choice)
+
+
+def dump_outputs(out_dir, model, loss, logits, labels):
+    """The arrays a caller of the timed train step receives, as float32 / float64 .npy files (< 64 MB in all)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    store = model.encoder_q.store
+    n = store.flat.numel()
+    idx = torch.randperm(n, generator=torch.Generator().manual_seed(12345))[:min(n, DUMP_SAMPLE)].sort().values
+    idx = idx.to(store.flat.device)
+    arrays = {
+        "loss": loss.detach().double().reshape(1),
+        "logits": logits.detach().float(),
+        "labels": labels.detach().double() if labels is not None else None,
+        "queue": model.queue.detach().float(),
+        "params_sample": store.flat[idx].float(),
+        "grad_sample": store.grad[idx].float(),
+        "sample_index": idx.double(),
+    }
+    for name, t in arrays.items():
+        if t is not None:
+            if t.numel() > DUMP_SAMPLE:      # seeded sample: < 64 MB in all
+                t = t.reshape(-1)[torch.randperm(t.numel(), generator=torch.Generator().manual_seed(12345))
+                                  [:DUMP_SAMPLE].sort().values.to(t.device)]
+            np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy())
 
 
 # ------------------------------------------------------------------------------------------------
@@ -144,7 +175,7 @@ def reference_arm(args):
     if rank != 0:
         return
     batch, sample_T = CPU_SAMPLE_BATCH, CPU_SAMPLE_T
-    steps = max(1, min(args.steps, 10))
+    steps = max(1, args.steps)
     val, med = cpu_oracle_clips_per_s(batch, sample_T, CFG["img"], args.moco_k, steps, 1, args.net)
     line = {"impl": "reference", "metric": "clips/sec %s InfoNCE (32x128^2, K=%d)" % (NET_NAME[args.net], args.moco_k), "value": val, "unit": "clips/s",
             "n_gpus": args.gpus, "steps": steps, "warmup": 1, "ms_per_step": med * 1e3, "higher_is_better": True,
@@ -240,7 +271,7 @@ def replicas_identical(model, world, dev):
 
 # ------------------------------------------------------------------------------------------------
 # the same training step in stock PyTorch ops (the oracle's restatement of the reference, cuDNN / cuBLAS) on THIS GPU:
-# what the unmodified reference would reach on a B200 -- "the Blackwell kernels to beat" (SURVEY.md 2a / 8d).
+# what the unmodified reference would reach on this GPU -- the kernels to beat (SURVEY.md 2a / 8d).
 # fp32-strict is the arithmetic the 1e-3 parity bar needs; TF32 is PyTorch's default (misses the bar by ~40x).
 # ------------------------------------------------------------------------------------------------
 def stock_gpu_baseline(batch, seq_len, img, K, net, dev, steps=3):
@@ -390,22 +421,22 @@ def main():
     gen = torch.Generator().manual_seed(1000 + rank)
     nblk = 2 if coclr else 1                               # CoCLR reads two blocks per sample (clip 1 and clip 2, RGB + flow)
     host_blocks = [torch.randn(nblk * B, 2, 3, T, HW, HW, generator=gen).pin_memory() for _ in range(2)]
-    dev_blocks = [hb.to(dev) for hb in host_blocks]       # 2 x 403 MB > 126 MB L2: inputs never L2-resident
+    dev_blocks = [hb.to(dev) for hb in host_blocks]       # 2 x 403 MB > 50 MB L2: inputs never L2-resident
     vname = torch.randint(0, 997, (B,), device=dev)
-    loss_keep = [None, None]
+    loss_keep = [None, None, None]
 
     def train_step(block):
         if coclr:
             import main_coclr
-            logits, mask = model(block[:B], block[B:], vname)
-            loss = main_coclr.multi_nce_loss(logits, mask)
+            logits, labels = model(block[:B], block[B:], vname)   # labels: the positive mask
+            loss = main_coclr.multi_nce_loss(logits, labels)
         else:
             logits, labels = model(block)
             loss = moco.nce_cross_entropy(logits, labels)
         opt.zero_grad()
         loss.backward()
         opt.step()
-        loss_keep[0], loss_keep[1] = loss, logits
+        loss_keep[0], loss_keep[1], loss_keep[2] = loss, logits, labels
         return loss
 
     # ---- parity of this configuration, before anything is timed (all ranks take part; rank 0 runs the oracle) ----
@@ -443,6 +474,8 @@ def main():
     ms = float(t)
     final_loss = float(loss_keep[0].detach())
     value = 2.0 * B * world / (ms * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, loss_keep[0], loss_keep[1], loss_keep[2])
 
     # ---- end to end: pinned host inputs, H2D inside the timed region (prefetched), loss read back every step ----
     e2e = None
@@ -523,26 +556,16 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "fallback 1.4 PFLOP/s sustained (B200_PROFILING.md)"
+    peak_tf = peaks.get("bf16_tflops_sustained", 989.0)
+    peak_src = ("MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else
+                "NVIDIA H100 SXM data sheet: 989 TFLOP/s dense BF16 at up to 700 W (not a measured figure)")
     cv = table.get("coclr_conv_igemm", {"ms": 0.0, "flops": 0.0, "launches": 0})
     wg = table.get("coclr_conv_wgrad", {"ms": 0.0, "flops": 0.0, "launches": 0})
     passes = 3 if args.precision == "parity" else None
-    # DRAM traffic of the heaviest coclr_conv_igemm launch of the step (Conv_2c.conv1 forward) from the committed
-    # `ncu --set full` capture; its algorithmic bytes are one read of the fp16 hi/lo input planes + one fp32 write
-    traffic, traffic_note = None, None
-    try:
-        cap = json.load(open(os.path.join(ROOT, "profiles", "r02_ncu_full_summary.json")))["ncu_r02_tma_conv2c1_fwd.ncu-rep"]
-        traffic = (cap["dram__bytes_read.sum"]["value"] + cap["dram__bytes_write.sum"]["value"]) * 1e6
-        traffic_note = ("bytes of ONE launch of the kernel as benched (TMA-staged): Conv_2c.conv1 forward, M=524288 N=192 "
-                        "K=576, from the committed `ncu --set full` capture (profiles/r02_ncu_full_summary.json); "
-                        "algorithmic = 134.2e6 (input planes, read once) + 402.7e6 (fp32 output) bytes")
-    except Exception:
-        pass
     achieved = cv["flops"] / (cv["ms"] * 1e-3) / 1e12 if cv["ms"] > 0 else 0.0
     roofline = {"bound": "tensor", "kernel": "coclr_conv_igemm (forward + dgrad implicit GEMM)",
                 "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf,
-                "traffic": traffic if args.net == "s3d" else None, "traffic_note": traffic_note, "peak_source": peak_src,
+                "peak_source": peak_src,
                 "launches_per_step": cv["launches"], "ms_per_step_in_kernel": cv["ms"],
                 "mode": "%s (forward %s, backward %s)" % (args.precision,
                                                         "3 MMA passes fp16 hi/lo" if args.precision != "fast" else "1 pass bf16",
@@ -651,7 +674,7 @@ def main():
                                         "enqueue x2, bwd, all-reduce, Adam); 2 of the 4 clips of a sample are counted"
                                         % (NET_NAME[args.net], K, B, T)),
                            "global_batch": B * world, "parallelism": "dp%d" % world, "precision": args.precision,
-                           "l2": "two alternating 403 MB input blocks per rank (> 126 MB L2)",
+                           "l2": "two alternating 403 MB input blocks per rank (> 50 MB L2)",
                            "pairs_per_s": value / 2, "final_loss": final_loss, "host_enqueue_ms_per_step": host_ms,
                            "algorithmic_tflops": value / 2 * GFLOP_PER_PAIR[args.net] * (1.25 if coclr else 1.0) * (T / 32.0) / 1e3,
                            "mixed_precision": mixed, "phase_timeline_ms": timeline},

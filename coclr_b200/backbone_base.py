@@ -23,7 +23,7 @@ class EngineBackbone(nn.Module):
     def _get_engine(self):
         w = dict(self.named_parameters())[self._probe]
         if not w.is_cuda:
-            raise RuntimeError("coclr_b200 backbones run on CUDA (sm_100a) only; move the module to the GPU")
+            raise RuntimeError("coclr_b200 backbones run on CUDA (sm_90a) only; move the module to the GPU")
         if self._engine is None or self._engine.store.device != w.device or \
                 w.data_ptr() != self._engine.store.view(self._probe).data_ptr():
             graph = Graph(self._stages, self.input_channel, head_dim=None)

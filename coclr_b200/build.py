@@ -1,6 +1,6 @@
-"""Builds libcoclr_b200.so (the C-ABI library of sm_100a kernels) in-tree with nvcc.
+"""Builds libcoclr_b200.so (the C-ABI library of sm_90a kernels) in-tree with nvcc.
 
-The library is compiled only for sm_100a (`-gencode arch=compute_100a,code=sm_100a`); nvcc
+The library is compiled only for sm_90a (`-gencode arch=compute_90a,code=sm_90a`, NVIDIA H100); nvcc
 cross-compiles without a GPU, so this also is the "does it build" check of `__graft_entry__.build()`.
 """
 import hashlib
@@ -15,7 +15,7 @@ LIB = os.path.join(HERE, "libcoclr_b200.so")
 STAMP = os.path.join(HERE, ".libcoclr_b200.stamp")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "-I", os.path.join(ROOT, "include"),

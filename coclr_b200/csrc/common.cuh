@@ -1,8 +1,8 @@
-// Shared device helpers for the sm_100a kernels: mbarrier, bulk copy (TMA engine, 1-D),
-// tcgen05 (alloc / mma / commit / ld / fences), shared-memory matrix descriptors and the
+// Shared device helpers for the sm_90a kernels: mbarrier, bulk copy (TMA engine, 1-D),
+// wgmma (fences / mma / commit / wait), shared-memory matrix descriptors and the
 // 128-byte swizzle used by every operand tile in this library.
 //
-// Everything here is inline PTX for sm_100a; there is no fallback path.
+// Everything here is inline PTX for sm_90a; there is no fallback path.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -22,7 +22,7 @@ COCLR_DEVINL uint32_t smem_u32(const void* p) {
 
 // Operand tiles are stored as rows of 128 bytes (64 16-bit elements of one pixel / one weight row),
 // eight rows per 1024-byte swizzle atom; the 16-byte chunk index inside a row is XOR-ed with (row & 7).
-// This is the canonical SWIZZLE_128B layout of tcgen05 shared-memory descriptors, and the same bytes
+// This is the canonical SWIZZLE_128B layout of wgmma shared-memory descriptors, and the same bytes
 // can be read K-major (row = M/N index, 64 elements = K) or MN-major (row = K index, 64 elements = M/N).
 COCLR_DEVINL uint32_t swz128_offset(uint32_t row, uint32_t chunk16) {
   return row * 128u + (((chunk16 ^ row) & 7u) << 4);
@@ -66,7 +66,7 @@ COCLR_DEVINL void mbar_wait(uint64_t* bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
 }
-// latency-critical waiter (the single MMA-issuing warp): default (short) suspend time
+// latency-critical waiter (the MMA-issuing warpgroups): default (short) suspend time
 COCLR_DEVINL void mbar_wait_spin(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   do {
@@ -80,7 +80,7 @@ COCLR_DEVINL void mbar_wait_spin(uint64_t* bar, uint32_t parity) {
   } while (!ok);
 }
 
-// generic-proxy writes (st.shared) -> async-proxy readers (tcgen05.mma / bulk copy)
+// generic-proxy writes (st.shared, cp.async) -> async-proxy readers (wgmma / bulk copy)
 COCLR_DEVINL void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------
@@ -112,53 +112,22 @@ COCLR_DEVINL void cp_async_wait() {
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05: tensor memory + MMA
+// wgmma (sm_90a): D[registers of one warpgroup] (+)= A[smem] * B[smem], M = 64 rows per warpgroup
 // ---------------------------------------------------------------------------------------------
-template <uint32_t kCols>
-COCLR_DEVINL void tmem_alloc(uint32_t* smem_holder) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+COCLR_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+COCLR_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+COCLR_DEVINL void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory");
 }
-template <uint32_t kCols>
-COCLR_DEVINL void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-COCLR_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-COCLR_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]; one thread issues on behalf of the CTA.
-COCLR_DEVINL void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed
-COCLR_DEVINL void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int kN>
+COCLR_DEVINL void acc_fence(float (&d)[kN]) {
+#pragma unroll
+  for (int i = 0; i < kN; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i <-> lane base+i)
-COCLR_DEVINL void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-COCLR_DEVINL void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// Shared-memory matrix descriptor, SWIZZLE_128B, version 1 (sm_100).
+// Shared-memory matrix descriptor, SWIZZLE_128B (sm_90 layout type 1).
 //   K-major operand : rows = M/N index (128 B = 64 K-elements), SBO = byte stride between 8-row groups
 //   MN-major operand: rows = K index   (128 B = 64 M/N elements), SBO = stride between 8-row (K) groups,
 //                     LBO = stride between consecutive 64-element M/N blocks
@@ -167,23 +136,105 @@ COCLR_DEVINL uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uin
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;  // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;  // SWIZZLE_128B
   return d;
 }
 
-// Instruction descriptor for kind::f16: fp32 accumulate, A / B format 0 = fp16, 1 = bf16 (independent).
-COCLR_DEVINL uint32_t make_idesc(uint32_t a_format, uint32_t b_format, uint32_t a_mn_major, uint32_t b_mn_major,
-                                 uint32_t M, uint32_t N) {
-  uint32_t d = 0;
-  d |= 1u << 4;                // c_format = F32
-  d |= (a_format & 7u) << 7;   // a_format
-  d |= (b_format & 7u) << 10;  // b_format
-  d |= (a_mn_major & 1u) << 15;
-  d |= (b_mn_major & 1u) << 16;
-  d |= ((N >> 3) & 0x3Fu) << 17;
-  d |= ((M >> 4) & 0x1Fu) << 24;
-  return d;
+// m64 x n{32,64} x k16, fp32 accumulate; kTA / kTB = 1: the operand is MN-major.  Both operands have one 16-bit
+// format (fp16 or bf16).  scale_d = 0 overwrites the accumulator.
+template <bool kBf16, int kTA, int kTB>
+COCLR_DEVINL void wgmma_n64(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+  if constexpr (kBf16) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(kTA), "n"(kTB));
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(kTA), "n"(kTB));
+  }
+}
+template <bool kBf16, int kTA, int kTB>
+COCLR_DEVINL void wgmma_n32(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+  if constexpr (kBf16) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(kTA), "n"(kTB));
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(kTA), "n"(kTB));
+  }
+}
+
+// One 64- (n64) or 32-column block of a warpgroup's product: t holds 32 (16) accumulator registers.
+template <int kTA, int kTB>
+COCLR_DEVINL void wgmma_blk(float (&t)[32], uint64_t a, uint64_t b, bool n64, bool bf16, uint32_t scale_d) {
+  if (n64) {
+    if (bf16) wgmma_n64<true, kTA, kTB>(t, a, b, scale_d);
+    else wgmma_n64<false, kTA, kTB>(t, a, b, scale_d);
+  } else {
+    if (bf16) wgmma_n32<true, kTA, kTB>(t, a, b, scale_d);
+    else wgmma_n32<false, kTA, kTB>(t, a, b, scale_d);
+  }
+}
+
+// One pipeline stage: acc += sum over the nprod (<= 3) operand pairs (ad[p], bd[p]) of 4 K = 16 steps (descriptor
+// increments a_inc / b_inc), ncols (multiple of 32) columns, b_step64 = descriptor step per 64 B columns.  Each
+// 64-column block is summed by the tensor core in a fresh accumulator and added to acc with fp32 adds: long
+// reductions keep fp32 accuracy.  acc[16 c + r] = row 16 (warp % 4) + lane / 4 + 8 ((r >> 1) & 1), column
+// 32 c + 8 (r >> 2) + 2 (lane % 4) + (r & 1) of the warpgroup's 64 rows.
+template <int kChunks, int kTA, int kTB>
+COCLR_DEVINL void wgmma_stage(float (&acc)[16 * kChunks], const uint64_t (&ad)[3], const uint64_t (&bd)[3], int nprod,
+                              uint32_t a_inc, uint32_t b_inc, uint32_t b_step64, int ncols, bool bf16) {
+#pragma unroll
+  for (int j = 0; j < kChunks / 2; ++j) {
+    if (64 * j < ncols) {
+      const bool n64 = 64 * j + 64 <= ncols;
+      float t[32];
+      wgmma_fence();
+#pragma unroll
+      for (int p = 0; p < 3; ++p) {
+        if (p < nprod) {
+#pragma unroll
+          for (uint32_t k = 0; k < 4; ++k)
+            wgmma_blk<kTA, kTB>(t, ad[p] + k * a_inc, bd[p] + k * b_inc + (uint64_t)j * b_step64, n64, bf16,
+                                (p | (int)k) != 0);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(t);
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if (n64 || i < 16) acc[32 * j + i] += t[i];
+    }
+  }
+}
+
+// Writes 32-column chunk c of a warpgroup's accumulator into rows [64 wg, 64 wg + 64) of a [128][pitch] fp32 tile, so
+// that lane i of warp w can afterwards read row 32 w + i (the row-per-lane view the epilogues work on).
+template <int kChunks>
+COCLR_DEVINL void acc_chunk_to_smem(const float (&acc)[16 * kChunks], int c, float* tile, int pitch, int wg,
+                                    int tid_in_wg) {
+  const int row0 = 64 * wg + 16 * (tid_in_wg >> 5) + ((tid_in_wg & 31) >> 2);
+  const int col0 = 2 * (tid_in_wg & 3);
+#pragma unroll
+  for (int cc = 0; cc < kChunks; ++cc) {
+    if (cc == c) {
+#pragma unroll
+      for (int r = 0; r < 16; ++r)
+        tile[(row0 + 8 * ((r >> 1) & 1)) * pitch + col0 + 8 * (r >> 2) + (r & 1)] = acc[16 * cc + r];
+    }
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -196,10 +247,8 @@ COCLR_DEVINL float4 ldg_nc_f4(const float* p) {
 }
 
 // One lane of a converged warp.  Unlike `lane == 0`, ptxas knows that code under an elect.sync predicate is executed by
-// exactly one thread, so operands of uniform-datapath instructions issued there (tcgen05.mma / .commit, cp.async.bulk.*)
-// are moved to uniform registers ONCE; under a plain lane test every such instruction is wrapped in a "waterfall" loop
-// (ELECT / 5x R2UR.BROADCAST / BRA.U.ANY, ~15 instructions and ~100 cycles per MMA) that caps the tensor pipe at the
-// issue rate of the loop instead of the rate of the MMAs.
+// exactly one thread, so operands of uniform-datapath instructions issued there (cp.async.bulk.*) are moved to uniform
+// registers once instead of being wrapped in a per-instruction "waterfall" loop.
 COCLR_DEVINL bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
@@ -258,83 +307,6 @@ COCLR_DEVINL void tma_reduce_add_5d(const void* tmap, uint32_t smem_src, int c0,
       "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
 }
-// ---- CTA pairs (clusters of 2, tcgen05 cta_group::2) ----
-COCLR_DEVINL uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-COCLR_DEVINL void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the object at `local_addr` in the rank-0 CTA of the cluster
-COCLR_DEVINL uint32_t mapa_rank0(uint32_t local_addr) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(0));
-  return r;
-}
-COCLR_DEVINL void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-COCLR_DEVINL void mbar_arrive_expect_tx_cluster(uint32_t cluster_addr, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.release.cluster.shared::cluster.b64 _, [%0], %1;" ::"r"(cluster_addr), "r"(bytes)
-               : "memory");
-}
-// loads into THIS CTA's shared memory whose completion is signalled on a barrier of the pair's rank-0 CTA
-COCLR_DEVINL void tma_load_5d_2cta(uint32_t smem_dst, const void* tmap, uint32_t bar_cluster_addr, int c0, int c1, int c2,
-                                   int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, "
-      "%4, %5, %6}], [%7];" ::"r"(smem_dst),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4), "r"(bar_cluster_addr)
-      : "memory");
-}
-COCLR_DEVINL void tma_load_2d_2cta(uint32_t smem_dst, const void* tmap, uint32_t bar_cluster_addr, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, "
-      "%3}], [%4];" ::"r"(smem_dst),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(bar_cluster_addr)
-      : "memory");
-}
-template <uint32_t kCols>
-COCLR_DEVINL void tmem_alloc_2cta(uint32_t* smem_holder) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-COCLR_DEVINL void tmem_dealloc_2cta(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-template <bool kPair>
-COCLR_DEVINL void umma_f16_t(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (kPair) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    umma_f16(tmem_d, adesc, bdesc, idesc, accumulate);
-  }
-}
-// pair mode: the arrival is delivered to the barrier at this offset in BOTH CTAs
-template <bool kPair>
-COCLR_DEVINL void umma_commit_t(uint64_t* bar) {
-  if constexpr (kPair) {
-    const uint16_t mask = 3;
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(mask)
-                 : "memory");
-  } else {
-    umma_commit(bar);
-  }
-}
-
 COCLR_DEVINL void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // the shared-memory source of all but the newest kPending committed bulk groups may be overwritten
 template <int kPending>

@@ -1,4 +1,4 @@
-// Implicit-GEMM 3-D convolution on tcgen05 tensor cores (sm_100a): forward, data-gradient and
+// Implicit-GEMM 3-D convolution on wgmma tensor cores (sm_90a): forward, data-gradient and
 // weight-gradient kernels plus the weight packer.
 //
 // Replaces nn.Conv3d + the statistics half of nn.BatchNorm3d of the reference
@@ -12,23 +12,28 @@
 //  * producer warps only generate addresses: 16-byte cp.async (LDGSTS) copies with hardware zero-fill for
 //    padding land 128 pixels x 64 K-elements straight in 128B-swizzled shared-memory tiles; weights arrive
 //    pre-split and pre-swizzled through one bulk (TMA-engine) copy per stage;
-//  * one elected thread issues tcgen05.mma (M=128, N<=256, K=16) for the three products hi*lo, lo*hi, hi*hi
-//    into one fp32 TMEM accumulator (fp32-equivalent result), or hi*hi only in single-pass mode;
-//  * four epilogue warps drain the other TMEM accumulator (previous tile) concurrently, transpose through
-//    shared memory for coalesced stores and accumulate the per-channel sum / sum-of-squares that train-mode
-//    BatchNorm needs.
+//  * two consumer warpgroups (64 pixel rows each) issue wgmma (M=64, N<=128, K=16) for the three products
+//    hi*lo, lo*hi, hi*hi into one fp32 register accumulator (fp32-equivalent result), or hi*hi only in
+//    single-pass mode;
+//  * the accumulator goes through shared memory 32 columns at a time; four of the consumer warps then make
+//    coalesced stores and accumulate the per-channel sum / sum-of-squares that train-mode BatchNorm needs.
 #include "common.cuh"
 #include "coclr_b200.h"
 #include "conv_tma.h"
 
 namespace coclr {
 
-static constexpr int kTileM = 128;      // pixels per tile (UMMA M)
+static constexpr int kTileM = 128;      // pixels per tile (two warpgroups of M = 64)
 static constexpr int kChunkK = 64;      // K elements per pipeline stage (one 128B swizzle row)
-static constexpr int kProducerWarps = 8;
-static constexpr int kEpiWarps = 4;
-// warp roles: [0,4) epilogue, [4,12) producers, 12 MMA issuer, 13 weight loader + TMEM owner
-static constexpr int kThreads = (kEpiWarps + kProducerWarps + 2) * 32;
+static constexpr int kProducerWarps = 8;       // weight-gradient kernel: 256 threads gather 64 rows x 2 operands
+static constexpr int kFwdProducerWarps = 4;    // forward / dgrad kernel: 128 threads gather 128 rows
+static constexpr int kMmaWarps = 8;     // two consumer warpgroups: MMA, then the epilogue
+static constexpr int kEpiWarps = 4;     // consumer warps that store a tile (32 rows each)
+static constexpr int kMaxBN = 128;      // output columns per tile (register accumulator: 64 fp32 per thread)
+static constexpr int kAccChunks = kMaxBN / 32;
+// warp roles: [0,8) MMA + epilogue, [8,12) producers, 12 weight loader
+static constexpr int kThreads = (kMmaWarps + kFwdProducerWarps + 1) * 32;
+static constexpr int kWgradThreads = (kMmaWarps + kProducerWarps) * 32;
 static constexpr int kStagePitch = 33;  // floats per staged row (conflict-free transpose)
 static constexpr int kMaxStages = 6;
 
@@ -68,9 +73,9 @@ COCLR_DEVINL void row_coords(const coclr_geom_t& G, int Td, int Hd, int Wd, int 
   }
 }
 
-// Issue the cp.async copies of NI*32 rows x 64 K-columns [kbase, kbase+64) of the implicit operand into one
+// Issue the cp.async copies of NI*kRowStride rows x 64 K-columns [kbase, kbase+64) of the implicit operand into one
 // swizzled [rows][128 B] block (hi plane) and its lo twin.  Thread (ck, r0) owns the 16-byte chunk ck
-// (8 consecutive K elements) of rows r0 + 32*i.  K index k = tap*C + channel, C % 8 == 0.
+// (8 consecutive K elements) of rows r0 + kRowStride*i.  K index k = tap*C + channel, C % 8 == 0.
 // Position of one 16-byte K granule in (tap, channel) space; kept per thread and advanced incrementally so the
 // pipelined loops never divide.
 struct TapPos {
@@ -103,7 +108,7 @@ COCLR_DEVINL void tap_advance(TapPos& p, const coclr_src_t& S, const coclr_geom_
   }
 }
 
-template <bool kLo, int NI>
+template <bool kLo, int NI, int kRowStride = 32>
 COCLR_DEVINL void gather_block_async(const coclr_src_t& S, const coclr_geom_t& G, int Kreal, const TapPos& tp, int ck,
                                      int r0, const int* rb, const int* rt, const int* ry, const int* rx,
                                      uint32_t blk_hi, uint32_t blk_lo) {
@@ -134,7 +139,7 @@ COCLR_DEVINL void gather_block_async(const coclr_src_t& S, const coclr_geom_t& G
     in = in && ((unsigned)ts < (unsigned)S.T) && ((unsigned)ys < (unsigned)S.H) && ((unsigned)xs < (unsigned)S.W);
     const int pix = in ? (rb[i] * S.T + ts) * HW + ys * S.W + xs : 0;
     const size_t off = (size_t)(unsigned)pix * (unsigned)S.ld;
-    const uint32_t dst = swz128_offset((uint32_t)(r0 + 32 * i), (uint32_t)ck);
+    const uint32_t dst = swz128_offset((uint32_t)(r0 + kRowStride * i), (uint32_t)ck);
     const uint32_t nbytes = in ? 16u : 0u;
     cp_async16(blk_hi + dst, hi + off, nbytes);
     if constexpr (kLo) cp_async16(blk_lo + dst, lo + off, nbytes);
@@ -149,7 +154,7 @@ struct ConvSmemLayout {
   uint32_t b_bytes;      // per copy
   uint32_t stage_bytes;  // all copies of A and B of one stage
   uint32_t stages;
-  uint32_t off_stage;    // transpose staging for the epilogue
+  uint32_t off_stage;    // [128 rows][kStagePitch] fp32: one 32-column chunk of the accumulator for the epilogue
   uint32_t off_stats;    // float [epilogue warps][2][n_tiles*BN + 4]: per-warp BN-statistic partial sums
   uint32_t off_bars;
   uint32_t total;
@@ -183,7 +188,7 @@ __host__ __device__ inline ConvSmemLayout conv_smem_layout(int BN, int n_tiles, 
 
 // Transposed (dgrad) pass of a temporally strided conv: a tap only meets every other output frame, so for a tile that
 // lies inside ONE frame (Hd*Wd % 128 == 0) and K chunks that lie inside one tap (C % 64 == 0) whole chunks are zero.
-// Bit kc of the returned mask = chunk kc contributes nothing to this tile; producers, weight loader and MMA issuer all
+// Bit kc of the returned mask = chunk kc contributes nothing to this tile; producers, weight loader and MMA warpgroups all
 // derive the same mask and skip those chunks.  0 when the shortcut does not apply.
 COCLR_DEVINL uint64_t zero_chunk_mask(const coclr_conv_t& P, int nkc, int m_tile) {
   if (!P.g.transposed || P.g.st != 2 || (P.src.C & 63) || ((P.Hd * P.Wd) % kTileM) || nkc > 64) return 0ull;
@@ -218,49 +223,36 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const coclr_con
   const int stat_cols = stat_table_cols(P.BN, P.n_tiles) + 4;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L.off_bars);  // [kMaxStages]
   uint64_t* empty_bar = full_bar + kMaxStages;                           // [kMaxStages]
-  uint64_t* tfull_bar = empty_bar + kMaxStages;                          // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;                                  // [2]
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kMaxStages; ++s) {
-      mbar_init(&full_bar[s], kProducerWarps * 32 + 1);  // every producer thread (async, via cp.async) + the weight loader
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull_bar[a], 1);
-      mbar_init(&tempty_bar[a], kEpiWarps);
+      mbar_init(&full_bar[s], kFwdProducerWarps * 32 + 1);  // every producer thread (async, via cp.async) + the weight loader
+      mbar_init(&empty_bar[s], kMmaWarps);               // one arrival per consumer warp
     }
     mbar_fence_init();
   }
   if (P.stats_sum != nullptr) {
     for (int i = threadIdx.x; i < kEpiWarps * 2 * stat_cols; i += kThreads) wstats[i] = 0.f;
   }
-  if (warp == 13) {
-    tmem_alloc<512>(tmem_holder);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_holder, 0);   // warp-uniform for the compiler
 
-  if (warp >= kEpiWarps && warp < kEpiWarps + kProducerWarps) {
+  if (warp >= kMmaWarps && warp < kMmaWarps + kFwdProducerWarps) {
     // ===================== A-operand producers (address generation + cp.async only) =====================
-    const int pt = threadIdx.x - kEpiWarps * 32;  // 0..255
+    const int pt = threadIdx.x - kMmaWarps * 32;  // 0..127
     const int ck = pt & 7;
-    const int r0 = pt >> 3;  // 0..31; rows r0 + 32*i
+    const int r0 = pt >> 3;  // 0..15; rows r0 + 16*i
     const uint32_t smem_base = smem_u32(smem);
     uint32_t stage = 0, phase = 0;
     const TapPos tap0 = tap_of(P.src, P.g, ck * 8);  // this thread's K granule in chunk 0 (the only division)
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int m_tile = tile / P.n_tiles;
-      int rb[4], rt[4], ry[4], rx[4];
+      int rb[8], rt[8], ry[8], rx[8];
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
-        row_coords(P.g, P.Td, P.Hd, P.Wd, M, m_tile * kTileM + r0 + 32 * i, rb[i], rt[i], ry[i], rx[i]);
+      for (int i = 0; i < 8; ++i)
+        row_coords(P.g, P.Td, P.Hd, P.Wd, M, m_tile * kTileM + r0 + 16 * i, rb[i], rt[i], ry[i], rx[i]);
       TapPos tp = tap0;
       const uint64_t zmask = zero_chunk_mask(P, nkc, m_tile);
       for (int kc = 0; kc < nkc; ++kc) {
@@ -270,14 +262,14 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const coclr_con
         }
         mbar_wait(&empty_bar[stage], phase ^ 1u);
         const uint32_t sa = smem_base + stage * L.stage_bytes;
-        gather_block_async<kLo, 4>(P.src, P.g, P.Kreal, tp, ck, r0, rb, rt, ry, rx, sa, sa + L.a_bytes);
+        gather_block_async<kLo, 8, 16>(P.src, P.g, P.Kreal, tp, ck, r0, rb, rt, ry, rx, sa, sa + L.a_bytes);
         tap_advance(tp, P.src, P.g, kChunkK);
         // asynchronous arrival when this thread's copies have landed: the producer never waits for data
         cp_async_mbar_arrive_noinc(&full_bar[stage]);
         if (++stage == nstages) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp == 13) {
+  } else if (warp == kMmaWarps + kFwdProducerWarps) {
     // ===================== weight loader (bulk copies) =====================
     if (elect_one()) {
       const uint32_t copies = kLo ? 2u : 1u;
@@ -298,73 +290,55 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const coclr_con
         }
       }
     }
-  } else if (warp == 12) {
-    // ===================== MMA issuer =====================
-    const uint32_t idesc = make_idesc(P.a_bf16 ? 1u : 0u, P.b_bf16 ? 1u : 0u, 0u, 0u, kTileM, (uint32_t)P.BN);
+  } else if (warp < kMmaWarps) {
+    // ===================== MMA (two warpgroups of 64 rows), then the epilogue =====================
+    const int wg = warp >> 2;
+    const int tid_wg = threadIdx.x & 127;
+    const bool bf16 = P.a_bf16 != 0;
+    const uint32_t a_row_off = (uint32_t)wg * 64u * 128u;   // this warpgroup's 64 rows of the A tile
+    float* my_stage = stage_buf + warp * 32 * kStagePitch;
+    float acc[16 * kAccChunks];
     uint32_t stage = 0, phase = 0;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const uint32_t acc = it & 1u;
-      const uint32_t acc_phase = (it >> 1) & 1u;
-      mbar_wait_spin(&tempty_bar[acc], acc_phase ^ 1u);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * 256u;
-      const uint64_t zmask = zero_chunk_mask(P, nkc, tile / P.n_tiles);
-      uint32_t started = 0;   // 0 until the first MMA of the tile has overwritten the accumulator
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const int m_tile = tile / P.n_tiles;
+      const int n_tile = tile % P.n_tiles;
+      const uint64_t zmask = zero_chunk_mask(P, nkc, m_tile);
+#pragma unroll
+      for (int i = 0; i < 16 * kAccChunks; ++i) acc[i] = 0.f;
       for (int kc = 0; kc < nkc; ++kc) {
         if ((zmask >> kc) & 1ull) continue;
         mbar_wait_spin(&full_bar[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t sa = smem_u32(smem + stage * L.stage_bytes);
-          const uint32_t sb = sa + (kLo ? 2u : 1u) * L.a_bytes;
-          const uint64_t a_hi = make_smem_desc(sa, 16, 1024);
-          const uint64_t b_hi = make_smem_desc(sb, 16, 1024);
-          if constexpr (kLo) {
-            const uint64_t a_lo = make_smem_desc(sa + L.a_bytes, 16, 1024);
-            const uint64_t b_lo = make_smem_desc(sb + L.b_bytes, 16, 1024);
-#pragma unroll
-            for (uint32_t k = 0; k < 4; ++k) umma_f16(tmem_d, a_hi + 2 * k, b_lo + 2 * k, idesc, (started | k) != 0);
-#pragma unroll
-            for (uint32_t k = 0; k < 4; ++k) umma_f16(tmem_d, a_lo + 2 * k, b_hi + 2 * k, idesc, 1u);
-#pragma unroll
-            for (uint32_t k = 0; k < 4; ++k) umma_f16(tmem_d, a_hi + 2 * k, b_hi + 2 * k, idesc, 1u);
-          } else {
-#pragma unroll
-            for (uint32_t k = 0; k < 4; ++k) umma_f16(tmem_d, a_hi + 2 * k, b_hi + 2 * k, idesc, (started | k) != 0);
-          }
-          umma_commit(&empty_bar[stage]);
+        fence_proxy_async_smem();   // cp.async (generic proxy) data -> wgmma (async proxy)
+        const uint32_t sa = smem_u32(smem + stage * L.stage_bytes);
+        const uint32_t sb = sa + (kLo ? 2u : 1u) * L.a_bytes;
+        const uint64_t a_hi = make_smem_desc(sa + a_row_off, 16, 1024);
+        const uint64_t b_hi = make_smem_desc(sb, 16, 1024);
+        if constexpr (kLo) {
+          const uint64_t a_lo = make_smem_desc(sa + L.a_bytes + a_row_off, 16, 1024);
+          const uint64_t b_lo = make_smem_desc(sb + L.b_bytes, 16, 1024);
+          const uint64_t ad[3] = {a_hi, a_lo, a_hi}, bd[3] = {b_lo, b_hi, b_hi};   // small products first
+          wgmma_stage<kAccChunks, 0, 0>(acc, ad, bd, 3, 2u, 2u, 512u, P.BN, bf16);
+        } else {
+          const uint64_t ad[3] = {a_hi, a_hi, a_hi}, bd[3] = {b_hi, b_hi, b_hi};
+          wgmma_stage<kAccChunks, 0, 0>(acc, ad, bd, 1, 2u, 2u, 512u, P.BN, bf16);
         }
-        started = 1u;
         __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);   // this warp's reads of the stage are complete
         if (++stage == nstages) { stage = 0; phase ^= 1u; }
       }
-      if (elect_one()) umma_commit(&tfull_bar[acc]);   // fires when every MMA of this tile has completed
-      __syncwarp();
-    }
-  } else if (warp < kEpiWarps) {
-    // ===================== epilogue =====================
-    float* my_stage = stage_buf + warp * 32 * kStagePitch;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int m_tile = tile / P.n_tiles;
-      const int n_tile = tile % P.n_tiles;
-      const uint32_t acc = it & 1u;
-      const uint32_t acc_phase = (it >> 1) & 1u;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
       const int row_base = m_tile * kTileM + warp * 32;
       const int rows_here = min(32, M - row_base);
       // store mapping after the transpose: lane = (row group rg, column quad cq); one 16-byte store per lane covers
       // 4 rows x 128 B per warp instruction
       const int rg = lane >> 3, cq = lane & 7;
-      for (int c0 = 0; c0 < P.BN; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(warp * 32) << 16) + acc * 256u + (uint32_t)c0, v);
-        tmem_ld_wait();
 #pragma unroll
-        for (int j = 0; j < 32; ++j) my_stage[lane * kStagePitch + j] = __uint_as_float(v[j]);
-        __syncwarp();
+      for (int c = 0; c < kAccChunks; ++c) {
+        const int c0 = c * 32;
+        if (c0 >= P.BN) break;
+        named_bar_sync(2, kMmaWarps * 32);   // the previous chunk's readers are done with the staging tile
+        acc_chunk_to_smem<kAccChunks>(acc, c, stage_buf, kStagePitch, wg, tid_wg);
+        named_bar_sync(2, kMmaWarps * 32);
+        if (warp >= kEpiWarps) continue;
         const int colq = n_tile * P.BN + c0 + cq * 4;  // first of this lane's 4 output channels
         float us[4] = {1.f, 1.f, 1.f, 1.f};
         if (P.wunscale != nullptr) {
@@ -435,10 +409,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const coclr_con
         }
         __syncwarp();
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      if (stats_per_tile && P.stats_sum != nullptr) {
+      if (warp < kEpiWarps && stats_per_tile && P.stats_sum != nullptr) {
         named_bar_sync(1, kEpiWarps * 32);
         for (int c = threadIdx.x; c < P.BN; c += kEpiWarps * 32) {
           double a = 0.0, b = 0.0;
@@ -458,7 +429,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const coclr_con
         named_bar_sync(1, kEpiWarps * 32);
       }
     }
-    if (P.stats_sum != nullptr && !stats_per_tile) {
+    if (warp < kEpiWarps && P.stats_sum != nullptr && !stats_per_tile) {
       named_bar_sync(1, kEpiWarps * 32);
       for (int c = threadIdx.x; c < P.N; c += kEpiWarps * 32) {
         double a = 0.0, b = 0.0;
@@ -472,18 +443,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const coclr_con
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 13) {
-    tc_fence_after();
-    __syncwarp();
-    tmem_dealloc<512>(tmem_base);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
-// weight-gradient kernel: D[cout (128 lanes), kcol (<=256)] = sum over pixels dY[px, cout] * A[px, kcol]
+// weight-gradient kernel: D[cout (128 rows, 64 per warpgroup), kcol (<=128)] = sum over pixels dY[px, cout] * A[px, kcol]
 // both operands are MN-major (the 64-element swizzle rows run along cout / kcol, pixels are K).
 // ------------------------------------------------------------------------------------------------
 static constexpr int kWgPx = 64;  // pixels per pipeline stage
@@ -511,14 +474,14 @@ __host__ __device__ inline WgradSmemLayout wgrad_smem_layout(int BNk, int npass)
 }
 
 __host__ __device__ inline int wgrad_bnk(int Kreal) {
-  // width of one K-column tile: multiple of 64, at most 256, balanced over the tiles
-  int kt = (Kreal + 255) / 256;
+  // width of one K-column tile: multiple of 64, at most kMaxBN, balanced over the tiles
+  int kt = (Kreal + kMaxBN - 1) / kMaxBN;
   int w = (Kreal + kt - 1) / kt;
   return ((w + 63) / 64) * 64;
 }
 
 template <int kNPass>
-__global__ void __launch_bounds__(kThreads, 1) conv_wgrad_kernel(const coclr_wgrad_t P) {
+__global__ void __launch_bounds__(kWgradThreads, 1) conv_wgrad_kernel(const coclr_wgrad_t P) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr bool kLo = kNPass > 1;
@@ -530,9 +493,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgrad_kernel(const coclr_wgr
   const int c_tiles = (P.Cout + 127) / 128;
   const WgradSmemLayout L = wgrad_smem_layout(BNk, kNPass);
   const uint32_t nstages = L.stages;
-  // Cout <= 64 in split-precision mode: the hi and the lo plane of dY are the two 64-row halves of ONE M = 128 operand
+  // Cout <= 64 in split-precision mode: the hi and the lo plane of dY are the two 64-row halves of the M = 128 tile
   // ([dY_hi; dY_lo] x A_hi, then x A_lo: 2 instructions per K step instead of 3 on a half-empty tile, and the lo x lo
-  // term comes for free); lanes 64..127 hold the dY_lo products of channels 0..63 and are added by the epilogue
+  // term comes for free); rows 64..127 hold the dY_lo products of channels 0..63 and are added by the epilogue
   const bool stack_m = kLo && P.Cout <= 64;
 
   // work item: (split, c_tile, k_tile)
@@ -549,27 +512,20 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgrad_kernel(const coclr_wgr
 
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L.off_bars);  // [kMaxStages]
   uint64_t* empty_bar = full_bar + kMaxStages;
-  uint64_t* tfull_bar = empty_bar + kMaxStages;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tfull_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int s = 0; s < kMaxStages; ++s) {
       mbar_init(&full_bar[s], kProducerWarps * 32);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], kMmaWarps);
     }
-    mbar_init(&tfull_bar[0], 1);
     mbar_fence_init();
   }
-  if (warp == 13) tmem_alloc<256>(tmem_holder);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_holder, 0);   // warp-uniform for the compiler
 
-  if (warp >= kEpiWarps && warp < kEpiWarps + kProducerWarps) {
-    const int pt = threadIdx.x - kEpiWarps * 32;
+  if (warp >= kMmaWarps) {
+    const int pt = threadIdx.x - kMmaWarps * 32;
     const int ck = pt & 7;
     const int r0 = pt >> 3;  // rows r0 + 32*i, i < 2
     const uint32_t smem_base = smem_u32(smem);
@@ -580,11 +536,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgrad_kernel(const coclr_wgr
     ident.pt = ident.ph = ident.pw = 0;
     ident.transposed = 0;
     // the K granules this thread copies are the same for every pixel chunk: decompose them once
-    TapPos tp_dy[2], tp_a[4];
+    TapPos tp_dy[2], tp_a[kMaxBN / 64];
 #pragma unroll
     for (int blk = 0; blk < 2; ++blk) tp_dy[blk] = tap_of(P.dy, ident, c_tile * 128 + blk * 64 + ck * 8);
 #pragma unroll
-    for (int blk = 0; blk < 4; ++blk) tp_a[blk] = tap_of(P.src, P.g, k_tile * BNk + blk * 64 + ck * 8);
+    for (int blk = 0; blk < kMaxBN / 64; ++blk) tp_a[blk] = tap_of(P.src, P.g, k_tile * BNk + blk * 64 + ck * 8);
     for (int ch = ch_begin; ch < ch_begin + nch; ++ch) {
       int rb[2], rt[2], ry[2], rx[2];    // source-space bases for the activation gather
       int qb[2], qt[2], qy[2], qx[2];    // plain destination coordinates for dY
@@ -611,7 +567,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgrad_kernel(const coclr_wgr
         }
       }
 #pragma unroll
-      for (int blk = 0; blk < 4; ++blk) {
+      for (int blk = 0; blk < kMaxBN / 64; ++blk) {
         if (blk < BNk / 64)
           gather_block_async<kLo, 2>(P.src, P.g, Kreal, tp_a[blk], ck, r0, rb, rt, ry, rx,
                                      s_a + blk * (kWgPx * 128), s_a + L.a_bytes + blk * (kWgPx * 128));
@@ -619,72 +575,72 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgrad_kernel(const coclr_wgr
       cp_async_mbar_arrive_noinc(&full_bar[stage]);
       if (++stage == nstages) { stage = 0; phase ^= 1u; }
     }
-  } else if (warp == 12) {
-    const uint32_t idesc = make_idesc(P.dy_bf16 ? 1u : 0u, P.src_bf16 ? 1u : 0u, 1u, 1u, 128u, (uint32_t)BNk);
+  } else {
+    // ===================== MMA: warpgroup wg owns cout rows [64 wg, 64 wg + 64) of the tile =====================
+    const int wg = warp >> 2;
+    const bool bf16 = P.dy_bf16 != 0;
+    float acc[16 * kAccChunks];
+#pragma unroll
+    for (int i = 0; i < 16 * kAccChunks; ++i) acc[i] = 0.f;
     uint32_t stage = 0, phase = 0;
     for (int ch = 0; ch < nch; ++ch) {
       mbar_wait_spin(&full_bar[stage], phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t s_dy = smem_u32(smem + stage * L.stage_bytes);
-        const uint32_t s_a = s_dy + (kLo ? 2u : 1u) * L.dy_bytes;
-        // MN-major: LBO = stride between 64-element MN blocks (64 px * 128 B), SBO = 8-pixel group stride
-        const uint64_t a_hi = make_smem_desc(s_dy, kWgPx * 128, 1024);
-        const uint64_t b_hi = make_smem_desc(s_a, kWgPx * 128, 1024);
-        // one K=16 step = 16 pixels = 2 swizzle atoms = 2048 B -> +128 in descriptor units
-        if constexpr (kLo) {
-          const uint64_t a_lo = make_smem_desc(s_dy + L.dy_bytes, kWgPx * 128, 1024);
-          const uint64_t b_lo = make_smem_desc(s_a + L.a_bytes, kWgPx * 128, 1024);
-#pragma unroll
-          for (uint32_t k = 0; k < 4; ++k) umma_f16(tmem_base, a_hi + 128 * k, b_lo + 128 * k, idesc, (ch | k) != 0);
-          if (!stack_m) {
-#pragma unroll
-            for (uint32_t k = 0; k < 4; ++k) umma_f16(tmem_base, a_lo + 128 * k, b_hi + 128 * k, idesc, 1u);
-          }
-#pragma unroll
-          for (uint32_t k = 0; k < 4; ++k) umma_f16(tmem_base, a_hi + 128 * k, b_hi + 128 * k, idesc, 1u);
-        } else {
-#pragma unroll
-          for (uint32_t k = 0; k < 4; ++k) umma_f16(tmem_base, a_hi + 128 * k, b_hi + 128 * k, idesc, (ch | k) != 0);
-        }
-        umma_commit(&empty_bar[stage]);
-        if (ch == nch - 1) umma_commit(&tfull_bar[0]);
+      fence_proxy_async_smem();   // cp.async (generic proxy) data -> wgmma (async proxy)
+      const uint32_t s_dy = smem_u32(smem + stage * L.stage_bytes) + (uint32_t)wg * (kWgPx * 128);
+      const uint32_t s_a = smem_u32(smem + stage * L.stage_bytes) + (kLo ? 2u : 1u) * L.dy_bytes;
+      // MN-major: LBO = stride between 64-element MN blocks (64 px * 128 B), SBO = 8-pixel group stride
+      const uint64_t a_hi = make_smem_desc(s_dy, kWgPx * 128, 1024);
+      const uint64_t b_hi = make_smem_desc(s_a, kWgPx * 128, 1024);
+      const uint32_t b_step = (kWgPx * 128) >> 4;
+      // one K=16 step = 16 pixels = 2 swizzle atoms = 2048 B -> +128 in descriptor units
+      if constexpr (kLo) {
+        const uint64_t a_lo = make_smem_desc(s_dy + L.dy_bytes, kWgPx * 128, 1024);
+        const uint64_t b_lo = make_smem_desc(s_a + L.a_bytes, kWgPx * 128, 1024);
+        const uint64_t ad[3] = {a_hi, stack_m ? a_hi : a_lo, a_hi}, bd[3] = {b_lo, b_hi, b_hi};
+        wgmma_stage<kAccChunks, 1, 1>(acc, ad, bd, stack_m ? 2 : 3, 128u, 128u, b_step, BNk, bf16);
+      } else {
+        const uint64_t ad[3] = {a_hi, a_hi, a_hi}, bd[3] = {b_hi, b_hi, b_hi};
+        wgmma_stage<kAccChunks, 1, 1>(acc, ad, bd, 1, 128u, 128u, b_step, BNk, bf16);
       }
       __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
       if (++stage == nstages) { stage = 0; phase ^= 1u; }
     }
-  } else if (warp < kEpiWarps) {
-    if (nch > 0) {
-      mbar_wait(&tfull_bar[0], 0);
-      tc_fence_after();
-      int n = c_tile * 128 + warp * 32 + lane;  // output channel of this thread
-      if (stack_m) n &= 63;
-      const float os = P.out_scale != nullptr ? __ldg(P.out_scale) : 1.f;
-      for (int c0 = 0; c0 < BNk; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
-        tmem_ld_wait();
-        if (n < P.Cout) {
+    const int tw = threadIdx.x & 127;
+    if (stack_m) {
+      // dY_lo rows (warpgroup 1) join the dY_hi rows via smem
+      float* xs = reinterpret_cast<float*>(smem);
+      named_bar_sync(1, kMmaWarps * 32);   // MMAs done
+      if (wg == 1) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int k = k_tile * BNk + c0 + j;
-            if (k < Kreal) {
-              const int tap = k / P.src.C;
-              const int ci = k - tap * P.src.C;
-              if (ci < P.Cin_real)
-                atomicAdd(P.dw + ((size_t)n * P.Cin_real + ci) * taps + tap, __uint_as_float(v[j]) * os);
-            }
+        for (int i = 0; i < 16 * kAccChunks; ++i) xs[i * 128 + tw] = acc[i];
+      }
+      named_bar_sync(1, kMmaWarps * 32);
+      if (wg == 0) {
+#pragma unroll
+        for (int i = 0; i < 16 * kAccChunks; ++i) acc[i] += xs[i * 128 + tw];
+      }
+    }
+    if (nch > 0 && !(stack_m && wg == 1)) {
+      // fp32 atomics into dW[cout, cin, tap], one per element when splits == 1
+      const int row0 = 64 * wg + 16 * (tw >> 5) + ((tw & 31) >> 2);
+      const int col0 = 2 * (tw & 3);
+      const float os = P.out_scale != nullptr ? __ldg(P.out_scale) : 1.f;
+#pragma unroll
+      for (int c = 0; c < kAccChunks; ++c) {
+        if (c * 32 >= BNk) break;
+#pragma unroll
+        for (int r = 0; r < 16; ++r) {
+          const int n = c_tile * 128 + row0 + 8 * ((r >> 1) & 1);   // output channel
+          const int k = k_tile * BNk + c * 32 + col0 + 8 * (r >> 2) + (r & 1);
+          if (n < P.Cout && k < Kreal) {
+            const int tap = k / P.src.C;
+            const int ci = k - tap * P.src.C;
+            if (ci < P.Cin_real) atomicAdd(P.dw + ((size_t)n * P.Cin_real + ci) * taps + tap, acc[16 * c + r] * os);
           }
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 13) {
-    tc_fence_after();
-    __syncwarp();
-    tmem_dealloc<256>(tmem_base);
   }
 }
 
@@ -751,7 +707,7 @@ __global__ void pack_weights_kernel(const coclr_pack_t P, int N, int BN, int n_t
 }
 
 __host__ __device__ inline void tile_plan_hd(int N, int* BN, int* n_tiles) {
-  int nt = (N + 255) / 256;
+  int nt = (N + kMaxBN - 1) / kMaxBN;
   int w = (N + nt - 1) / nt;
   *BN = ((w + 31) / 32) * 32;
   *n_tiles = nt;
@@ -847,7 +803,8 @@ static int launch_conv(const coclr_conv_t& P, int num_sms, cudaStream_t s) {
 extern "C" int coclr_conv_igemm(const coclr_conv_t* p, int num_sms, coclr_stream_t stream) {
   if (!p || !p->wpk || !p->dst) return COCLR_E_ARG;
   if (!src_ok(p->src, p->npass > 1)) return COCLR_E_ARG;
-  if (p->BN % 32 != 0 || p->BN > 256 || p->BN < 32 || p->n_tiles < 1) return COCLR_E_ARG;
+  if (p->BN % 32 != 0 || p->BN > kMaxBN || p->BN < 32 || p->n_tiles < 1) return COCLR_E_ARG;
+  if (p->a_bf16 != p->b_bf16) return COCLR_E_ARG;   // wgmma takes one 16-bit format for both operands
   if (p->dst_ld % 4 != 0 || p->dst_coff % 4 != 0 || ((uintptr_t)p->dst & 15)) return COCLR_E_ARG;  // 16-byte stores
   if (p->Kreal != p->g.kt * p->g.kh * p->g.kw * p->src.C) return COCLR_E_ARG;
   if ((p->g.st != 1 && p->g.st != 2) || (p->g.sh != 1 && p->g.sh != 2) || (p->g.sw != 1 && p->g.sw != 2))
@@ -873,7 +830,7 @@ static int launch_wgrad(const coclr_wgrad_t& P, cudaStream_t s) {
   cudaError_t e = cudaFuncSetAttribute(conv_wgrad_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total);
   if (e != cudaSuccess) return COCLR_E_LAUNCH;
   const int grid = k_tiles * c_tiles * P.splits;
-  conv_wgrad_kernel<NP><<<grid, kThreads, L.total, s>>>(P);
+  conv_wgrad_kernel<NP><<<grid, kWgradThreads, L.total, s>>>(P);
   return cudaGetLastError() == cudaSuccess ? COCLR_OK : COCLR_E_LAUNCH;
 }
 
@@ -881,6 +838,7 @@ extern "C" int coclr_conv_wgrad(const coclr_wgrad_t* p, coclr_stream_t stream) {
   if (!p || !p->dw) return COCLR_E_ARG;
   if (!src_ok(p->src, p->npass > 1) || !src_ok(p->dy, p->npass > 1)) return COCLR_E_ARG;
   if (p->splits < 1 || p->g.transposed) return COCLR_E_ARG;
+  if (p->dy_bf16 != p->src_bf16) return COCLR_E_ARG;   // wgmma takes one 16-bit format for both operands
   if ((long long)p->B * p->src.T * p->src.H * p->src.W >= (1ll << 31) ||
       (long long)p->B * p->dy.T * p->dy.H * p->dy.W >= (1ll << 31))
     return COCLR_E_ARG;  // 32-bit pixel indices

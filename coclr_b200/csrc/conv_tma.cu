@@ -1,4 +1,4 @@
-// TMA-staged implicit-GEMM convolution on tcgen05 tensor cores (sm_100a): forward and data-gradient of the
+// TMA-staged implicit-GEMM convolution on wgmma tensor cores (sm_90a): forward and data-gradient of the
 // stride-1 (1,k,k) / (k,1,1) / 1x1x1 convolutions and of the temporally strided (k,1,1) stem conv of the
 // reference's backbones (backbone/s3dg.py:11-13 BasicConv3d, :39-42 STConv3d conv1 / conv2; cuDNN dgrad behind
 // loss.backward(), main_nce.py:330).  Same C ABI as conv_igemm.cu (coclr_conv_igemm dispatches here first); what
@@ -11,16 +11,17 @@
 //    are the TMA unit's out-of-bounds zero fill.  No thread computes an address.
 //  * the taps along the reuse dimension (dy of a (1,3,3) conv, dt of a (k,1,1) conv) are served from the SAME
 //    slab: their A descriptors differ by a whole number of 8-row swizzle atoms (tile rows are a multiple of 8
-//    pixels wide), so every slab byte fetched from L2 feeds up to kh (kt) x 12 tensor-core instructions;
+//    pixels wide), so every slab byte fetched from L2 feeds up to kh (kt) x 12 K-steps of tensor-core instructions;
 //  * weights: the pre-swizzled hi / lo tile images of coclr_pack_weights, either streamed through a ring of
 //    bulk copies or -- for narrow layers whose whole image fits -- loaded ONCE per CTA and kept resident;
-//  * the epilogue drains TMEM into a swizzled staging row block, accumulates the BatchNorm statistics from it,
-//    and writes it with ONE cp.async.bulk.tensor store (or add-reduction, for gradient accumulation) per
-//    32 rows x 32 channels: edge clipping, channel slices of concat buffers and the strided frame order of the
-//    transposed stem conv are properties of the output tensor map, not code.
+//  * two consumer warpgroups (64 tile rows each) accumulate in registers with wgmma; the accumulator goes
+//    through a [128][33] fp32 transpose tile 32 columns at a time, from which warps 0-3 (32 rows each) fill a
+//    swizzled staging row block, accumulate the BatchNorm statistics from it, and write it with ONE
+//    cp.async.bulk.tensor store (or add-reduction, for gradient accumulation) per 32 rows x 32 channels: edge
+//    clipping, channel slices of concat buffers and the strided frame order of the transposed stem conv are
+//    properties of the output tensor map, not code.
 //
-// Warp roles (224 threads): 0-3 epilogue (TMEM lane quadrant = warp), 4 A loader, 5 weight loader + TMEM owner,
-// 6 MMA issuer.
+// Warp roles (320 threads): 0-7 MMA + epilogue, 8 A loader, 9 weight loader.
 #include <cuda.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -32,7 +33,11 @@
 
 namespace coclr {
 
-static constexpr int kTmaThreads = 7 * 32;
+static constexpr int kTmaThreads = 10 * 32;
+static constexpr int kTmaMmaWarps = 8;
+static constexpr int kTmaAccChunks = 4;        // BN <= 128: 64 fp32 accumulator registers per thread
+static constexpr int kXPitch = 33;             // floats per row of the accumulator transpose tile
+static constexpr uint32_t kXTileBytes = 128u * kXPitch * 4u;
 static constexpr int kTmaMaxASlots = 4;
 static constexpr int kTmaMaxBSlots = 4;
 static constexpr uint32_t kStageBytes = 4096;  // 32 rows x 32 fp32 columns per epilogue warp and buffer
@@ -41,14 +46,11 @@ struct TmaTile {
   int idx[4];
   int n_tile;
 };
-// Work item -> tile.  Items enumerate (pixel tile, N tile) with the N tile fastest; in pair mode an item is a PAIR of
-// consecutive pixel tiles (one per CTA of the cluster).  A pixel-tile number past the end (the odd tile out of a pair)
-// decodes to a batch index past the tensor: its loads are zero-filled, its stores clipped, its rows invalid.
-COCLR_DEVINL TmaTile tma_decode(const TmaPlan& L, int item, int pair, int rank) {
+// Work item -> tile.  Items enumerate (pixel tile, N tile) with the N tile fastest.
+COCLR_DEVINL TmaTile tma_decode(const TmaPlan& L, int item) {
   TmaTile t;
   t.n_tile = item % L.n_tiles_n;
   int m = item / L.n_tiles_n;
-  if (pair) m = 2 * m + rank;
 #pragma unroll
   for (int d = 0; d < 3; ++d) {
     t.idx[d] = m % L.ntiles[d];
@@ -58,19 +60,10 @@ COCLR_DEVINL TmaTile tma_decode(const TmaPlan& L, int item, int pair, int rank) 
   return t;
 }
 
-// kPair: the kernel runs as clusters of two CTAs that execute ONE tcgen05.mma.cta_group::2 stream (issued by the rank-0
-// CTA) over M = 256 pixels -- 128 per CTA, each in its own shared memory and tensor memory -- against a weight tile that
-// is SPLIT between the two CTAs (each holds half of its rows): per CTA and MMA the weight bytes read from shared memory
-// and fetched from L2 halve, and one instruction does the work of two.  Both matter here: M=128 x N<=192 instructions
-// are bound by shared-memory operand bandwidth (and a ~110-cycle per-instruction floor for N <= 64), not by the tensor
-// pipe (DESIGN.md section 4).  Synchronisation: loads of both CTAs complete on the rank-0 CTA's "full" barriers
-// (cp.async.bulk.tensor.cta_group::2 may signal the peer's mbarrier); tcgen05.commit multicasts the "empty" / "tile done"
-// arrivals to both CTAs; the epilogue warps of both CTAs arrive on rank 0's accumulator-free barrier.
-template <int kNPass, bool kPair>
+template <int kNPass>
 __global__ void __launch_bounds__(kTmaThreads, 1)
     conv_tma_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
-                    const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_w,
-                    const __grid_constant__ TmaArgs P) {
+                    const __grid_constant__ CUtensorMap map_out, const __grid_constant__ TmaArgs P) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr bool kLo = kNPass > 1;
@@ -80,57 +73,42 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
   const uint32_t a_base = smem_base;
   const uint32_t b_base = smem_base + L.off_b;
   const uint32_t stage_base = smem_base + L.off_stage;
+  float* xtile = reinterpret_cast<float*>(smem + L.off_misc + 1024u);   // [128][kXPitch] accumulator transpose tile
   float* unscale_tab = reinterpret_cast<float*>(smem + L.off_misc);
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + L.off_bars);
   uint64_t* a_empty = a_full + kTmaMaxASlots;
   uint64_t* b_full = a_empty + kTmaMaxASlots;
   uint64_t* b_empty = b_full + kTmaMaxBSlots;
-  uint64_t* t_full = b_empty + kTmaMaxBSlots;
-  uint64_t* t_empty = t_full + 2;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(t_empty + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = kPair ? cluster_ctarank() : 0u;
-  const uint32_t ncta = kPair ? 2u : 1u;
-  const int first_item = kPair ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int item_stride = kPair ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int n_items = kPair ? L.pair_items : L.total_tiles;
+  const int first_item = (int)blockIdx.x;
+  const int item_stride = (int)gridDim.x;
+  const int n_items = L.total_tiles;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kTmaMaxASlots; ++s) {
-      mbar_init(&a_full[s], ncta);     // one arrive.expect_tx per loading CTA
-      mbar_init(&a_empty[s], 1);
+      mbar_init(&a_full[s], 1);
+      mbar_init(&a_empty[s], kTmaMmaWarps);   // one arrival per consumer warp
     }
     for (int s = 0; s < kTmaMaxBSlots; ++s) {
-      mbar_init(&b_full[s], ncta);
-      mbar_init(&b_empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&t_full[a], 1);
-      mbar_init(&t_empty[a], 4 * ncta);
+      mbar_init(&b_full[s], 1);
+      mbar_init(&b_empty[s], kTmaMmaWarps);
     }
     mbar_fence_init();
   }
   for (int i = threadIdx.x; i < 256; i += kTmaThreads)
     unscale_tab[i] = 1.f;  // per tile the epilogue reads n_tile*BN + c; filled below when there is a table
-  if (warp == 5) {
-    if constexpr (kPair) tmem_alloc_2cta<512>(tmem_holder); else tmem_alloc<512>(tmem_holder);
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (kPair) cluster_sync_all();   // the peer's barriers are initialised before anything signals them
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_holder, 0);   // warp-uniform for the compiler
 
-  if (warp == 4) {
+  if (warp == kTmaMmaWarps) {
     // ===================== A loader: one TMA box (hi) + one (lo) per slab =====================
     if (elect_one()) {
       tma_prefetch_desc(&map_hi);
       if (kLo) tma_prefetch_desc(&map_lo);
       uint32_t slot = 0, phase = 0;
       for (int item = first_item; item < n_items; item += item_stride) {
-        const TmaTile t = tma_decode(L, item, kPair, (int)rank);
+        const TmaTile t = tma_decode(L, item);
         const int ty0 = L.sel_dim >= 0 ? t.idx[L.sel_dim] : 0;
         const int ty1 = L.sel_dim >= 0 ? ty0 + 1 : L.n_types;
         for (int cc = 0; cc < L.nc; ++cc) {
@@ -143,223 +121,84 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
             const int c3 = t.idx[2] * L.a_mul[2] + S.d[2];
             const int c4 = t.idx[3] * L.a_mul[3] + S.d[3];
             const uint32_t dst = a_base + slot * (uint32_t)L.a_slot_bytes;
-            if constexpr (kPair) {
-              const uint32_t bar = mapa_rank0(smem_u32(&a_full[slot]));
-              mbar_arrive_expect_tx_cluster(bar, kPlanes * (uint32_t)L.slab_bytes);
-              tma_load_5d_2cta(dst, &map_hi, bar, c0, c1, c2, c3, c4);
-              if (kLo) tma_load_5d_2cta(dst + (uint32_t)L.plane_stride, &map_lo, bar, c0, c1, c2, c3, c4);
-            } else {
-              mbar_arrive_expect_tx(&a_full[slot], kPlanes * (uint32_t)L.slab_bytes);
-              tma_load_5d(dst, &map_hi, &a_full[slot], c0, c1, c2, c3, c4);
-              if (kLo) tma_load_5d(dst + (uint32_t)L.plane_stride, &map_lo, &a_full[slot], c0, c1, c2, c3, c4);
-            }
+            mbar_arrive_expect_tx(&a_full[slot], kPlanes * (uint32_t)L.slab_bytes);
+            tma_load_5d(dst, &map_hi, &a_full[slot], c0, c1, c2, c3, c4);
+            if (kLo) tma_load_5d(dst + (uint32_t)L.plane_stride, &map_lo, &a_full[slot], c0, c1, c2, c3, c4);
             if (++slot == (uint32_t)L.a_slots) { slot = 0; phase ^= 1u; }
           }
         }
       }
     }
-  } else if (warp == 5) {
-    // ===================== weight loader =====================
+  } else if (warp == kTmaMmaWarps + 1) {
+    // ===================== weight loader: bulk copies of pre-swizzled tile images =====================
     if (elect_one()) {
-      if constexpr (kPair) {
-        // Tensor-map loads of BN/2-row boxes of the pre-swizzled packed image (rows of 128 bytes: hi rows of a K chunk,
-        // then its lo rows).  Plain 3-pass mode: this CTA's half of the hi rows and of the lo rows.  Stacked mode
-        // (see the MMA issuer): region Y (BN rows) = ALL hi rows on rank 0 / ALL lo rows on rank 1 -- the two halves of the
-        // N = 2*BN operand of a_hi x [b_hi; b_lo] -- and region X (BN/2 rows) = this CTA's half of the hi rows for
-        // a_lo x b_hi.
-        tma_prefetch_desc(&map_w);
-        const uint32_t half_bytes = (uint32_t)(L.BN / 2) * 128u;
-        const uint32_t step_bytes = (uint32_t)L.b_tile_bytes;
-        const bool stacked = kLo && L.stacked;
-        auto load_step = [&](uint32_t dst, uint32_t bar, int n_tile, int kc) {
-          const int row0 = (n_tile * L.nkc + kc) * 2 * L.BN;      // hi rows [row0, +BN), lo rows [row0 + BN, +BN)
-          const int h = L.BN / 2;
-          if (stacked) {
-            const int y0 = row0 + (int)rank * L.BN;                 // rank 0: hi plane, rank 1: lo plane
-            tma_load_2d_2cta(dst, &map_w, bar, 0, y0);
-            tma_load_2d_2cta(dst + half_bytes, &map_w, bar, 0, y0 + h);
-            tma_load_2d_2cta(dst + 2u * half_bytes, &map_w, bar, 0, row0 + (int)rank * h);
-          } else {
-            tma_load_2d_2cta(dst, &map_w, bar, 0, row0 + (int)rank * h);
-            if (kLo) tma_load_2d_2cta(dst + half_bytes, &map_w, bar, 0, row0 + L.BN + (int)rank * h);
-          }
-        };
-        if (L.b_resident) {
-          const uint32_t bar = mapa_rank0(smem_u32(&b_full[0]));
-          mbar_arrive_expect_tx_cluster(bar, (uint32_t)L.nkc * step_bytes);
-          for (int kc = 0; kc < L.nkc; ++kc) load_step(b_base + (uint32_t)kc * step_bytes, bar, 0, kc);
-        } else {
-          uint32_t slot = 0, phase = 0;
-          for (int item = first_item; item < n_items; item += item_stride) {
-            const TmaTile t = tma_decode(L, item, kPair, (int)rank);
-            const int ty0 = L.sel_dim >= 0 ? t.idx[L.sel_dim] : 0;
-            const int ty1 = L.sel_dim >= 0 ? ty0 + 1 : L.n_types;
-            for (int cc = 0; cc < L.nc; ++cc) {
-              for (int ty = ty0; ty < ty1; ++ty) {
-                const TmaSlabType& S = L.type[ty];
-                for (int j = 0; j < S.nshift; ++j) {
-                  mbar_wait(&b_empty[slot], phase ^ 1u);
-                  const uint32_t bar = mapa_rank0(smem_u32(&b_full[slot]));
-                  mbar_arrive_expect_tx_cluster(bar, step_bytes);
-                  load_step(b_base + slot * step_bytes, bar, t.n_tile, S.tap[j] * L.nc + cc);
-                  if (++slot == (uint32_t)L.b_slots) { slot = 0; phase ^= 1u; }
-                }
-              }
-            }
-          }
-        }
+      const uint32_t tile_bytes = kPlanes * (uint32_t)L.BN * 128u;          // what one K chunk needs in smem
+      const size_t img_stride = (size_t)2u * (size_t)L.BN * 128u;            // packed image: hi and lo of every chunk
+      const uint8_t* wbase = reinterpret_cast<const uint8_t*>(P.wpk);
+      if (L.b_resident) {
+        // the whole [nkc] image of the (single) N tile, once
+        mbar_arrive_expect_tx(&b_full[0], (uint32_t)L.nkc * tile_bytes);
+        for (int kc = 0; kc < L.nkc; ++kc)
+          bulk_g2s(smem + L.off_b + (size_t)kc * tile_bytes, wbase + (size_t)kc * img_stride, tile_bytes, &b_full[0]);
       } else {
-        // bulk copies of pre-swizzled tile images
-        const uint32_t tile_bytes = kPlanes * (uint32_t)L.BN * 128u;          // what one K chunk needs in smem
-        const size_t img_stride = (size_t)2u * (size_t)L.BN * 128u;            // packed image: hi and lo of every chunk
-        const uint8_t* wbase = reinterpret_cast<const uint8_t*>(P.wpk);
-        if (L.b_resident) {
-          // the whole [nkc] image of the (single) N tile, once
-          mbar_arrive_expect_tx(&b_full[0], (uint32_t)L.nkc * tile_bytes);
-          for (int kc = 0; kc < L.nkc; ++kc)
-            bulk_g2s(smem + L.off_b + (size_t)kc * tile_bytes, wbase + (size_t)kc * img_stride, tile_bytes, &b_full[0]);
-        } else {
-          uint32_t slot = 0, phase = 0;
-          for (int item = first_item; item < n_items; item += item_stride) {
-            const TmaTile t = tma_decode(L, item, kPair, (int)rank);
-            const int ty0 = L.sel_dim >= 0 ? t.idx[L.sel_dim] : 0;
-            const int ty1 = L.sel_dim >= 0 ? ty0 + 1 : L.n_types;
-            for (int cc = 0; cc < L.nc; ++cc) {
-              for (int ty = ty0; ty < ty1; ++ty) {
-                const TmaSlabType& S = L.type[ty];
-                for (int j = 0; j < S.nshift; ++j) {
-                  const int kc = S.tap[j] * L.nc + cc;
-                  mbar_wait(&b_empty[slot], phase ^ 1u);
-                  mbar_arrive_expect_tx(&b_full[slot], tile_bytes);
-                  bulk_g2s(smem + L.off_b + (size_t)slot * tile_bytes,
-                           wbase + ((size_t)t.n_tile * L.nkc + kc) * img_stride, tile_bytes, &b_full[slot]);
-                  if (++slot == (uint32_t)L.b_slots) { slot = 0; phase ^= 1u; }
-                }
+        uint32_t slot = 0, phase = 0;
+        for (int item = first_item; item < n_items; item += item_stride) {
+          const TmaTile t = tma_decode(L, item);
+          const int ty0 = L.sel_dim >= 0 ? t.idx[L.sel_dim] : 0;
+          const int ty1 = L.sel_dim >= 0 ? ty0 + 1 : L.n_types;
+          for (int cc = 0; cc < L.nc; ++cc) {
+            for (int ty = ty0; ty < ty1; ++ty) {
+              const TmaSlabType& S = L.type[ty];
+              for (int j = 0; j < S.nshift; ++j) {
+                const int kc = S.tap[j] * L.nc + cc;
+                mbar_wait(&b_empty[slot], phase ^ 1u);
+                mbar_arrive_expect_tx(&b_full[slot], tile_bytes);
+                bulk_g2s(smem + L.off_b + (size_t)slot * tile_bytes,
+                         wbase + ((size_t)t.n_tile * L.nkc + kc) * img_stride, tile_bytes, &b_full[slot]);
+                if (++slot == (uint32_t)L.b_slots) { slot = 0; phase ^= 1u; }
               }
             }
           }
         }
       }
-    }
-  } else if (warp == 6) {
-    // ===================== MMA issuer (rank 0 only in pair mode) =====================
-    if (!kPair || rank == 0) {
-    const uint32_t mma_m = kPair ? 256u : 128u;
-    const uint32_t idesc = make_idesc(P.a_bf16 ? 1u : 0u, P.b_bf16 ? 1u : 0u, 0u, 0u, mma_m, (uint32_t)L.BN);
-    // stacked mode (narrow layers): the hi rows and the lo rows of a weight tile are adjacent in shared memory, so
-    // a_hi x [b_hi; b_lo] is ONE instruction with N = 2*BN whose second half of the accumulator collects a_hi*b_lo;
-    // with a_lo x b_hi that is 2 instructions per K step instead of 3, and a third less operand traffic from shared
-    // memory -- which, not the tensor pipe, bounds M=128 x N<=128 instructions (A 4 KB + B 32*N bytes per 16-deep step
-    // against 128 B/clk).  The epilogue adds the two halves.
-    const uint32_t idesc2 = make_idesc(P.a_bf16 ? 1u : 0u, P.b_bf16 ? 1u : 0u, 0u, 0u, mma_m, 2u * (uint32_t)L.BN);
-    const bool stacked = kLo && L.stacked;
-    const uint32_t tile_bytes = (uint32_t)L.b_tile_bytes;
-    // offset of the second weight region of a step: lo rows (plain), or region X of the stacked pair layout
-    const uint32_t b_second = kPair ? (stacked ? (uint32_t)L.BN * 128u : (uint32_t)(L.BN / 2) * 128u) : (uint32_t)L.BN * 128u;
-    uint32_t aslot = 0, aphase = 0, bslot = 0, bphase = 0, it = 0;
-    if (L.b_resident) {
-      mbar_wait_spin(&b_full[0], 0);
-      tc_fence_after();
-    }
-    for (int item = first_item; item < n_items; item += item_stride, ++it) {
-      const TmaTile t = tma_decode(L, item, kPair, 0);
-      const int ty0 = L.sel_dim >= 0 ? t.idx[L.sel_dim] : 0;
-      const int ty1 = L.sel_dim >= 0 ? ty0 + 1 : L.n_types;
-      const uint32_t acc = it & 1u;
-      mbar_wait_spin(&t_empty[acc], ((it >> 1) & 1u) ^ 1u);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * 256u;
-      uint32_t started = 0;
-      for (int cc = 0; cc < L.nc; ++cc) {
-        for (int ty = ty0; ty < ty1; ++ty) {
-          const TmaSlabType& S = L.type[ty];
-          mbar_wait_spin(&a_full[aslot], aphase);
-          tc_fence_after();
-          const uint32_t sa0 = a_base + aslot * (uint32_t)L.a_slot_bytes;
-          for (int j = 0; j < S.nshift; ++j) {
-            uint32_t sb;
-            if (L.b_resident) {
-              sb = b_base + (uint32_t)(S.tap[j] * L.nc + cc) * tile_bytes;
-            } else {
-              mbar_wait_spin(&b_full[bslot], bphase);
-              tc_fence_after();
-              sb = b_base + bslot * tile_bytes;
-            }
-            if (elect_one() && !(L.dbg & 8)) {
-              const uint32_t sa = sa0 + (uint32_t)j * (uint32_t)L.shift_bytes;
-              const uint64_t a_hi = make_smem_desc(sa, 16, 1024);
-              const uint64_t b_hi = make_smem_desc(sb, 16, 1024);
-              if constexpr (kLo) {
-                const uint64_t a_lo = make_smem_desc(sa + (uint32_t)L.plane_stride, 16, 1024);
-                const uint64_t b_2 = make_smem_desc(sb + b_second, 16, 1024);
-                if (stacked) {
-                  // pair mode: b_hi points at region Y (N = 2*BN over the pair), b_2 at region X (this CTA's hi half)
-                  const uint64_t b_x = kPair ? b_2 : b_hi;
-#pragma unroll
-                  for (uint32_t k = 0; k < 4; ++k)
-                    umma_f16_t<kPair>(tmem_d, a_hi + 2 * k, b_hi + 2 * k, idesc2, (started | k) != 0);
-#pragma unroll
-                  for (uint32_t k = 0; k < 4; ++k) umma_f16_t<kPair>(tmem_d, a_lo + 2 * k, b_x + 2 * k, idesc, 1u);
-                } else {
-#pragma unroll
-                  for (uint32_t k = 0; k < 4; ++k)
-                    umma_f16_t<kPair>(tmem_d, a_hi + 2 * k, b_2 + 2 * k, idesc, (started | k) != 0);
-#pragma unroll
-                  for (uint32_t k = 0; k < 4; ++k) umma_f16_t<kPair>(tmem_d, a_lo + 2 * k, b_hi + 2 * k, idesc, 1u);
-#pragma unroll
-                  for (uint32_t k = 0; k < 4; ++k) umma_f16_t<kPair>(tmem_d, a_hi + 2 * k, b_hi + 2 * k, idesc, 1u);
-                }
-              } else {
-#pragma unroll
-                for (uint32_t k = 0; k < 4; ++k)
-                  umma_f16_t<kPair>(tmem_d, a_hi + 2 * k, b_hi + 2 * k, idesc, (started | k) != 0);
-              }
-              if (!L.b_resident) umma_commit_t<kPair>(&b_empty[bslot]);
-            } else if ((L.dbg & 8) && !L.b_resident && elect_one()) {
-              umma_commit_t<kPair>(&b_empty[bslot]);
-            }
-            started = 1u;
-            __syncwarp();
-            if (!L.b_resident) {
-              if (++bslot == (uint32_t)L.b_slots) { bslot = 0; bphase ^= 1u; }
-            }
-          }
-          if (elect_one()) umma_commit_t<kPair>(&a_empty[aslot]);   // the slab may be overwritten once these MMAs have read it
-          __syncwarp();
-          if (++aslot == (uint32_t)L.a_slots) { aslot = 0; aphase ^= 1u; }
-        }
-      }
-      if (elect_one()) umma_commit_t<kPair>(&t_full[acc]);
-      __syncwarp();
-    }
     }
   } else {
-    // ===================== epilogue (warps 0-3) =====================
+    // ===================== MMA (warps 0-7: two warpgroups of 64 rows), then the epilogue (warps 0-3) =====================
+    const int wg = warp >> 2;
+    const int tid_wg = threadIdx.x & 127;
+    const bool bf16 = P.a_bf16 != 0;
+    const bool epi = warp < 4;
+    const uint32_t tile_bytes = (uint32_t)L.b_tile_bytes;
+    const uint32_t a_row_off = (uint32_t)wg * 64u * 128u;   // this warpgroup's 64 rows of the slab window
+    float acc[16 * kTmaAccChunks];
+    uint32_t aslot = 0, aphase = 0, bslot = 0, bphase = 0;
+    if (L.b_resident) mbar_wait_spin(&b_full[0], 0);
+
     const bool want_stats = P.stats_sum != nullptr;
     // the bulk-tensor stores of a warp are issued, committed and waited for by ONE thread (bulk async-groups are
     // per-thread state): elected once (elect.sync is deterministic for a given member mask)
     const bool leader = elect_one();
     const float oscale = P.out_scale != nullptr ? __ldg(P.out_scale) : 1.f;
-    if ((P.wunscale != nullptr || P.out_scale != nullptr) && L.n_tiles_n == 1) {
+    if (epi && (P.wunscale != nullptr || P.out_scale != nullptr) && L.n_tiles_n == 1) {
       for (int i = threadIdx.x; i < L.BN; i += 128)
         unscale_tab[i] = (P.wunscale != nullptr ? __ldg(P.wunscale + i) : 1.f) * oscale;
     }
-    named_bar_sync(1, 128);
-    const uint32_t my_stage = stage_base + (uint32_t)warp * (uint32_t)L.stage_bufs * kStageBytes;
+    if (epi) named_bar_sync(1, 128);
+    const uint32_t my_stage = stage_base + (uint32_t)(warp & 3) * (uint32_t)L.stage_bufs * kStageBytes;
     // BatchNorm statistics: per column, sum and sum of squares of d = x - x0 in fp32, where x0 is the first value of
     // the column this CTA sees; converted exactly in double when they leave the CTA:
     //   sum x = sum d + n x0,  sum x^2 = sum d^2 + 2 x0 sum d + n x0^2,
     // so that var = E[x^2] - mean^2 (formed in double by the finalize step) does not lose the variance of channels whose
     // spread is small against their mean to fp32 rounding of the raw sums (nn.BatchNorm3d is two-pass)
-    float s1[8], s2[8], x0[8];
+    float s1[4], s2[4], x0[4];
     uint32_t x0_set = 0u;
     int nrows = 0;
 #pragma unroll
-    for (int i = 0; i < 8; ++i) s1[i] = s2[i] = x0[i] = 0.f;
+    for (int i = 0; i < 4; ++i) s1[i] = s2[i] = x0[i] = 0.f;
     // box-relative position of this lane's row (rows are in box order, dim 1 fastest)
     int ri[4];
     {
-      int r = warp * 32 + lane;
+      int r = (warp & 3) * 32 + lane;
 #pragma unroll
       for (int d = 0; d < 3; ++d) {
         ri[d] = r % L.obox[d];
@@ -367,43 +206,75 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
       }
       ri[3] = r;
     }
-    uint32_t it = 0, nstore = 0;
-    for (int item = first_item; item < n_items; item += item_stride, ++it) {
-      const TmaTile t = tma_decode(L, item, kPair, (int)rank);
-      const uint32_t acc = it & 1u;
+    uint32_t nstore = 0;
+    for (int item = first_item; item < n_items; item += item_stride) {
+      const TmaTile t = tma_decode(L, item);
+      const int ty0 = L.sel_dim >= 0 ? t.idx[L.sel_dim] : 0;
+      const int ty1 = L.sel_dim >= 0 ? ty0 + 1 : L.n_types;
+      // ---- MMA ----
+#pragma unroll
+      for (int i = 0; i < 16 * kTmaAccChunks; ++i) acc[i] = 0.f;
+      for (int cc = 0; cc < L.nc; ++cc) {
+        for (int ty = ty0; ty < ty1; ++ty) {
+          const TmaSlabType& S = L.type[ty];
+          mbar_wait_spin(&a_full[aslot], aphase);
+          const uint32_t sa0 = a_base + aslot * (uint32_t)L.a_slot_bytes;
+          for (int j = 0; j < S.nshift; ++j) {
+            uint32_t sb;
+            if (L.b_resident) {
+              sb = b_base + (uint32_t)(S.tap[j] * L.nc + cc) * tile_bytes;
+            } else {
+              mbar_wait_spin(&b_full[bslot], bphase);
+              sb = b_base + bslot * tile_bytes;
+            }
+            const uint32_t sa = sa0 + (uint32_t)j * (uint32_t)L.shift_bytes + a_row_off;
+            const uint64_t a_hi = make_smem_desc(sa, 16, 1024);
+            const uint64_t b_hi = make_smem_desc(sb, 16, 1024);
+            if constexpr (kLo) {
+              const uint64_t a_lo = make_smem_desc(sa + (uint32_t)L.plane_stride, 16, 1024);
+              const uint64_t b_lo = make_smem_desc(sb + (uint32_t)L.BN * 128u, 16, 1024);
+              const uint64_t ad[3] = {a_hi, a_lo, a_hi}, bd[3] = {b_lo, b_hi, b_hi};   // small products first
+              wgmma_stage<kTmaAccChunks, 0, 0>(acc, ad, bd, 3, 2u, 2u, 512u, L.BN, bf16);
+            } else {
+              const uint64_t ad[3] = {a_hi, a_hi, a_hi}, bd[3] = {b_hi, b_hi, b_hi};
+              wgmma_stage<kTmaAccChunks, 0, 0>(acc, ad, bd, 1, 2u, 2u, 512u, L.BN, bf16);
+            }
+            __syncwarp();
+            if (!L.b_resident) {
+              if (lane == 0) mbar_arrive(&b_empty[bslot]);
+              if (++bslot == (uint32_t)L.b_slots) { bslot = 0; bphase ^= 1u; }
+            }
+          }
+          if (lane == 0) mbar_arrive(&a_empty[aslot]);   // the slab may be overwritten once every warp has read it
+          if (++aslot == (uint32_t)L.a_slots) { aslot = 0; aphase ^= 1u; }
+        }
+      }
+      // ---- epilogue ----
       bool valid = true;
       int oc[4];
 #pragma unroll
       for (int d = 0; d < 4; ++d) {
         const int o = t.idx[d] * L.o_mul[d];
         valid = valid && (o + ri[d] < L.oext[d]);
-        oc[d] = o + L.sub[warp][d];
+        oc[d] = o + L.sub[warp & 3][d];
       }
       const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
-      if ((P.wunscale != nullptr || P.out_scale != nullptr) && L.n_tiles_n > 1) {
+      if (epi && (P.wunscale != nullptr || P.out_scale != nullptr) && L.n_tiles_n > 1) {
         named_bar_sync(1, 128);   // previous tile's readers are done with the table
         for (int i = threadIdx.x; i < L.BN; i += 128)
           unscale_tab[i] = (P.wunscale != nullptr ? __ldg(P.wunscale + t.n_tile * L.BN + i) : 1.f) * oscale;
         named_bar_sync(1, 128);
       }
-      mbar_wait(&t_full[acc], (it >> 1) & 1u);
-      tc_fence_after();
 #pragma unroll
-      for (int kq = 0; kq < 8; ++kq) {
+      for (int kq = 0; kq < kTmaAccChunks; ++kq) {
         const int c0 = kq * 32;
         const int col0 = t.n_tile * L.BN + c0;
         if (c0 < L.BN && col0 < L.N && !(L.dbg & 4)) {
-          uint32_t v[32];
-          tmem_ld_32x32(tmem_base + ((uint32_t)(warp * 32) << 16) + acc * 256u + (uint32_t)c0, v);
-          if (kLo && L.stacked) {
-            uint32_t v2[32];
-            tmem_ld_32x32(tmem_base + ((uint32_t)(warp * 32) << 16) + acc * 256u + (uint32_t)(L.BN + c0), v2);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(v2[j]));
-          } else {
-            tmem_ld_wait();
-          }
+          named_bar_sync(2, kTmaMmaWarps * 32);   // the previous chunk's readers are done with the transpose tile
+          acc_chunk_to_smem<kTmaAccChunks>(acc, kq, xtile, kXPitch, wg, tid_wg);
+          named_bar_sync(2, kTmaMmaWarps * 32);
+          if (!epi) continue;
+          const float* xrow = xtile + (warp * 32 + lane) * kXPitch;
           const uint32_t buf = my_stage + (L.stage_bufs == 2 ? (nstore & 1u) : 0u) * kStageBytes;
           if (leader) {
             // the bulk store that last read this buffer must have finished reading it
@@ -415,8 +286,7 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
           for (int q = 0; q < 8; ++q) {
             const float4 u = *reinterpret_cast<const float4*>(unscale_tab + c0 + 4 * q);
             st_shared_v4(rowaddr + (((uint32_t)q ^ ((uint32_t)lane & 7u)) << 4),
-                         __uint_as_float(v[4 * q + 0]) * u.x, __uint_as_float(v[4 * q + 1]) * u.y,
-                         __uint_as_float(v[4 * q + 2]) * u.z, __uint_as_float(v[4 * q + 3]) * u.w);
+                         xrow[4 * q + 0] * u.x, xrow[4 * q + 1] * u.y, xrow[4 * q + 2] * u.z, xrow[4 * q + 3] * u.w);
           }
           fence_proxy_async_smem();
           __syncwarp();
@@ -427,8 +297,7 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
           }
           ++nstore;
           if (want_stats && !(L.dbg & 2)) {
-            // lane c sums column c over the warp's valid rows, reading the swizzled block back (conflict-free; a variant
-            // with 16-byte reads + shuffle reduction measured slower)
+            // lane c sums column c over the warp's valid rows, reading the swizzled block back (conflict-free)
             if (vmask != 0u) {
               float a = 0.f, b = 0.f;
               const uint32_t cchunk = (uint32_t)lane >> 2, cword = ((uint32_t)lane & 3u) << 2;
@@ -452,16 +321,11 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
           }
         }
       }
+      if (!epi) continue;
       nrows += __popc(vmask);
-      tc_fence_before();
-      __syncwarp();
-      if (leader) {
-        if constexpr (kPair) mbar_arrive_cluster(mapa_rank0(smem_u32(&t_empty[acc])));
-        else mbar_arrive(&t_empty[acc]);
-      }
       if (want_stats && L.n_tiles_n > 1) {
 #pragma unroll
-        for (int kq = 0; kq < 8; ++kq) {
+        for (int kq = 0; kq < kTmaAccChunks; ++kq) {
           const int col = t.n_tile * L.BN + kq * 32 + lane;
           if (kq * 32 < L.BN && col < L.N) {
             const double n = (double)nrows, xd = (double)x0[kq];
@@ -474,41 +338,34 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
         nrows = 0;
       }
     }
-    if (leader) bulk_wait_group_read<0>();
-    __syncwarp();
-    if (want_stats && L.n_tiles_n == 1) {
-      // combine the four warps' column sums in shared memory (the staging blocks are free now), one fp64 atomic per
-      // channel and CTA
-      double* tab = reinterpret_cast<double*>(smem + L.off_stage);   // [4 warps][2][256] = 16 KB = the staging blocks
-      named_bar_sync(1, 128);
+    if (epi) {
+      if (leader) bulk_wait_group_read<0>();
+      __syncwarp();
+      if (want_stats && L.n_tiles_n == 1) {
+        // combine the four warps' column sums in shared memory (the staging blocks are free now), one fp64 atomic per
+        // channel and CTA
+        double* tab = reinterpret_cast<double*>(smem + L.off_stage);   // [4 warps][2][128] = 8 KB of the staging blocks
+        named_bar_sync(1, 128);
 #pragma unroll
-      for (int kq = 0; kq < 8; ++kq) {
-        const double n = (double)nrows, xd = (double)x0[kq];
-        tab[(warp * 2 + 0) * 256 + kq * 32 + lane] = (double)s1[kq] + n * xd;
-        tab[(warp * 2 + 1) * 256 + kq * 32 + lane] = (double)s2[kq] + xd * (2.0 * (double)s1[kq] + n * xd);
-      }
-      named_bar_sync(1, 128);
-      for (int c = threadIdx.x; c < L.N; c += 128) {
-        double a = 0.0, b = 0.0;
-#pragma unroll
-        for (int w = 0; w < 4; ++w) {
-          a += tab[(w * 2 + 0) * 256 + c];
-          b += tab[(w * 2 + 1) * 256 + c];
+        for (int kq = 0; kq < kTmaAccChunks; ++kq) {
+          const double n = (double)nrows, xd = (double)x0[kq];
+          tab[(warp * 2 + 0) * 128 + kq * 32 + lane] = (double)s1[kq] + n * xd;
+          tab[(warp * 2 + 1) * 128 + kq * 32 + lane] = (double)s2[kq] + xd * (2.0 * (double)s1[kq] + n * xd);
         }
-        atomicAdd(&P.stats_sum[c], a);
-        atomicAdd(&P.stats_sq[c], b);
+        named_bar_sync(1, 128);
+        for (int c = threadIdx.x; c < L.N; c += 128) {
+          double a = 0.0, b = 0.0;
+#pragma unroll
+          for (int w = 0; w < 4; ++w) {
+            a += tab[(w * 2 + 0) * 128 + c];
+            b += tab[(w * 2 + 1) * 128 + c];
+          }
+          atomicAdd(&P.stats_sum[c], a);
+          atomicAdd(&P.stats_sq[c], b);
+        }
       }
+      if (leader) bulk_wait_group<0>();   // all global writes of this thread's bulk stores are complete
     }
-    if (leader) bulk_wait_group<0>();   // all global writes of this thread's bulk stores are complete
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (kPair) cluster_sync_all();   // the peer may still be signalling this CTA's barriers / reading its smem
-  if (warp == 5) {
-    tc_fence_after();
-    __syncwarp();
-    if constexpr (kPair) tmem_dealloc_2cta<512>(tmem_base); else tmem_dealloc<512>(tmem_base);
   }
 }
 
@@ -574,7 +431,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
   const bool window = g.kt == 1 && g.kw > 1 && S.C * g.kw == 64 && S.ld == S.C && S.coff == 0 && g.pw == 0 &&
                       !g.transposed && g.st == 1 && S.W >= P.Wd + g.kw - 1 && S.H == P.Hd && S.T == P.Td;
   if (S.C % 8 != 0 || (taps > 1 && S.C % 64 != 0 && !window)) return false;
-  if (P.BN % 32 != 0 || P.BN > 256 || P.n_tiles < 1) return false;
+  if (P.BN % 32 != 0 || P.BN > 32 * kTmaAccChunks || P.n_tiles < 1) return false;
   if (P.Kreal != g.kt * g.kh * g.kw * S.C) return false;
   if (g.sh != 1 || g.sw != 1) return false;
   const int planes = P.npass > 1 ? 2 : 1;
@@ -582,7 +439,6 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
   L.BN = P.BN;
   L.N = P.N;
   { const char* e = getenv("COCLR_TMA_DBG"); L.dbg = e ? atoi(e) : 0; }
-  L.stacked = (P.npass > 1 && P.BN <= 128 && getenv("COCLR_TMA_NOSTACK") == nullptr) ? 1 : 0;
   L.n_tiles_n = P.n_tiles;
   L.nc = window ? 1 : (S.C + 63) / 64;
   L.nkc = window ? g.kh : taps * L.nc;
@@ -801,27 +657,16 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
   if (((uintptr_t)O.base[0] & 15) || (old4 % 16) != 0 || (ld2 % 16) != 0) return false;
   for (int d = 0; d < 5; ++d)
     if (A.box[d] > 256 || O.box[d] > 256 || A.dims[d] == 0 || O.dims[d] == 0) return false;
-  // ---- CTA pairs ----
-  {
-    static int want_pair = -1;
-    if (want_pair < 0) {
-      const char* e = getenv("COCLR_TMA_PAIR");
-      want_pair = (e && e[0] == '1') ? 1 : 0;
-    }
-    L.pair = (want_pair && mt >= 2 && L.BN % 16 == 0) ? 1 : 0;
-    L.pair_items = (int)(((mt + 1) / 2) * L.n_tiles_n);
-  }
   // ---- shared memory ----
   L.plane_stride = (L.slab_bytes + 1023) & ~1023;
   L.a_slot_bytes = planes * L.plane_stride;
   L.b_tile_bytes = planes * L.BN * 128;
-  if (L.pair) L.b_tile_bytes = (L.stacked ? 3 : planes) * (L.BN / 2) * 128;
-  const int budget = 227 * 1024 - 1024 /*alignment slack*/ - 1024 /*unscale table*/ - 256 /*barriers*/;
+  const int budget = 227 * 1024 - 1024 /*alignment slack*/ - 1024 /*unscale table*/ - (int)kXTileBytes - 256 /*barriers*/;
   const int stage1 = 4 * (int)kStageBytes, stage2 = 8 * (int)kStageBytes;
   int steps_per_tile = 0;
   for (int ty = 0; ty < L.n_types; ++ty) steps_per_tile += L.type[ty].nshift;
   steps_per_tile *= L.nc;
-  const long tiles_per_cta = L.pair ? ((long)L.pair_items + 73) / 74 : ((long)L.total_tiles + 147) / 148;
+  const long tiles_per_cta = ((long)L.total_tiles + 131) / 132;   // one wave over the 132 SMs of an H100 SXM
   L.b_resident = 0;
   const long resident_bytes = (long)L.nkc * L.b_tile_bytes;
   if (L.n_tiles_n == 1 && tiles_per_cta >= 2 && resident_bytes + 2l * L.a_slot_bytes + stage1 <= budget) {
@@ -860,7 +705,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
   }
   L.off_stage = (L.off_stage + 1023u) & ~1023u;
   L.off_misc = L.off_stage + (uint32_t)(L.stage_bufs == 2 ? stage2 : stage1);
-  L.off_bars = L.off_misc + 1024u;
+  L.off_bars = L.off_misc + 1024u + kXTileBytes;
   L.total = L.off_bars + 256u + 1024u;
   if (L.total > 227u * 1024u) return false;
   if (L.stage_bufs == 1 && P.stats_sum != nullptr) {
@@ -930,7 +775,7 @@ int coclr::conv_tma_try(const coclr_conv_t& P, int num_sms, cudaStream_t stream)
   TmaArgs args;
   MapSpec A, O;
   if (!conv_tma_plan(P, args.plan, A, O)) return 1;
-  CUtensorMap m_hi, m_lo, m_out, m_w;
+  CUtensorMap m_hi, m_lo, m_out;
   if (!encode_map(&m_hi, A, 0)) return 1;
   if (P.npass > 1) {
     if (!encode_map(&m_lo, A, 1)) return 1;
@@ -939,23 +784,6 @@ int coclr::conv_tma_try(const coclr_conv_t& P, int num_sms, cudaStream_t stream)
   }
   if (!encode_map(&m_out, O, 0)) return 1;
   const TmaPlan& L = args.plan;
-  m_w = m_hi;
-  if (L.pair) {
-    // the packed weight image as rows of 128 bytes (64 16-bit elements): BN/2-row boxes, copied as they are
-    MapSpec Wm;
-    Wm.elem_bytes = 2;
-    Wm.base[0] = const_cast<void*>(P.wpk);
-    Wm.base[1] = nullptr;
-    Wm.dims[0] = 64;
-    Wm.dims[1] = (uint64_t)L.n_tiles_n * L.nkc * 2 * L.BN;
-    Wm.dims[2] = Wm.dims[3] = Wm.dims[4] = 1;
-    Wm.strides[0] = 128;
-    Wm.strides[1] = Wm.strides[2] = Wm.strides[3] = 128;
-    Wm.box[0] = 64;
-    Wm.box[1] = (uint32_t)(L.BN / 2);
-    Wm.box[2] = Wm.box[3] = Wm.box[4] = 1;
-    if (((uintptr_t)P.wpk & 15) || !encode_map(&m_w, Wm, 0, 2, false)) return 1;
-  }
   args.wpk = P.wpk;
   args.wunscale = P.wunscale;
   args.out_scale = P.out_scale;
@@ -964,35 +792,17 @@ int coclr::conv_tma_try(const coclr_conv_t& P, int num_sms, cudaStream_t stream)
   args.accumulate = P.accumulate;
   args.a_bf16 = P.a_bf16;
   args.b_bf16 = P.b_bf16;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.blockDim = dim3(kTmaThreads);
-  cfg.dynamicSmemBytes = L.total;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
+  const int grid = L.total_tiles < num_sms ? L.total_tiles : num_sms;
   cudaError_t e;
-#define COCLR_TMA_LAUNCH(NP, PAIR)                                                                                    \
-  do {                                                                                                                \
-    e = cudaFuncSetAttribute(conv_tma_kernel<NP, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total);   \
-    if (e != cudaSuccess) return COCLR_E_LAUNCH;                                                                      \
-    e = cudaLaunchKernelEx(&cfg, conv_tma_kernel<NP, PAIR>, m_hi, m_lo, m_out, m_w, args);                            \
-  } while (0)
-  if (L.pair) {
-    const int pairs = num_sms / 2;
-    const int nclusters = L.pair_items < pairs ? L.pair_items : pairs;
-    cfg.gridDim = dim3(2 * nclusters);
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    if (P.npass > 1) COCLR_TMA_LAUNCH(3, true); else COCLR_TMA_LAUNCH(1, true);
+  if (P.npass > 1) {
+    e = cudaFuncSetAttribute(conv_tma_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total);
+    if (e != cudaSuccess) return COCLR_E_LAUNCH;
+    conv_tma_kernel<3><<<grid, kTmaThreads, L.total, stream>>>(m_hi, m_lo, m_out, args);
   } else {
-    cfg.gridDim = dim3(L.total_tiles < num_sms ? L.total_tiles : num_sms);
-    if (P.npass > 1) COCLR_TMA_LAUNCH(3, false); else COCLR_TMA_LAUNCH(1, false);
+    e = cudaFuncSetAttribute(conv_tma_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total);
+    if (e != cudaSuccess) return COCLR_E_LAUNCH;
+    conv_tma_kernel<1><<<grid, kTmaThreads, L.total, stream>>>(m_hi, m_lo, m_out, args);
   }
-#undef COCLR_TMA_LAUNCH
   if (e != cudaSuccess) return COCLR_E_LAUNCH;
   return cudaGetLastError() == cudaSuccess ? COCLR_OK : COCLR_E_LAUNCH;
 }

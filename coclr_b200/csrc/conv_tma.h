@@ -36,10 +36,7 @@ struct TmaPlan {
   int a_slots, a_slot_bytes;
   int b_slots, b_tile_bytes, b_resident;
   int stage_bufs;
-  int pair;            // run as CTA pairs (tcgen05 cta_group::2); b_tile_bytes then is the per-CTA share of a K chunk
-  int pair_items;      // ceil(m_tiles / 2) * n_tiles_n
   int dbg;             // tuning experiments only (COCLR_TMA_DBG bit mask; 0 in production)
-  int stacked;         // 3-pass mode, BN <= 128: hi and lo weight rows form ONE N = 2*BN operand (see the MMA issuer)
   int sub[4][4];       // output coordinate offsets of each epilogue warp's 32-row sub-box
   int BN, N;
   uint32_t off_b, off_stage, off_misc, off_bars, total;

@@ -828,7 +828,7 @@ __global__ void __launch_bounds__(256) maxpool133s2_smem_kernel(const coclr_pool
 }
 
 // scatter form of the backward: every output element adds its gradient to the one input element that won
-// (fp32 reductions in L2; a window overlaps up to 27 others, so this is ~27x less work than the gather form)
+// (for non-overlapping windows only: with overlap, the order of the fp32 adds would depend on thread timing)
 __global__ void __launch_bounds__(256) maxpool_bwd_scatter_kernel(const coclr_pool_t P) {
   const int C4 = P.C >> 2;
   const int khw = P.g.kh * P.g.kw;
@@ -1264,9 +1264,10 @@ extern "C" int coclr_maxpool_fwd(const coclr_pool_t* p, coclr_stream_t stream) {
 }
 extern "C" int coclr_maxpool_bwd(const coclr_pool_t* p, coclr_stream_t stream) {
   if (!p || !p->dx || !p->dy || !p->idx || p->C % 4) return COCLR_E_ARG;
-  // scatter form whenever the destination can be zero-initialised with one memset (or already holds the other
-  // consumers' contributions); the gather kernel remains for strided destinations
-  if (p->accumulate || (p->ldx == p->C && p->x_coff == 0)) {
+  // scatter form (one add per input element) for disjoint windows and memset-able or accumulated destinations
+  const coclr_geom_t& g = p->g;
+  const bool disjoint = g.st >= g.kt && g.sh >= g.kh && g.sw >= g.kw;
+  if (disjoint && (p->accumulate || (p->ldx == p->C && p->x_coff == 0))) {
     cudaStream_t s = (cudaStream_t)stream;
     if (!p->accumulate) {
       const size_t bytes = (size_t)p->B * p->Ti * p->Hi * p->Wi * p->C * sizeof(float);

@@ -92,7 +92,7 @@ __global__ void __launch_bounds__(kNceThreads) nce_bwd_kernel(const float* __res
   }
 }
 
-// Long queues (config 3: K = 16384): one CTA per row leaves most of the 148 SMs idle and every CTA streams the whole
+// Long queues (config 3: K = 16384): one CTA per row leaves most of the 132 SMs idle and every CTA streams the whole
 // [D, K] queue through L2.  The split form cuts a row into K slices of kNceSlice columns on blockIdx.y:
 //   pass 1 (nce_fwd_slice_kernel): logits of the slice + the slice's (max, sum exp(l - max)) into ws[b][slice][2];
 //   pass 2 (nce_fwd_finish_kernel): every CTA folds the row's partials into the log-sum-exp, then loss / dlogits of its slice.
@@ -165,12 +165,12 @@ __global__ void __launch_bounds__(256) nce_fwd_finish_kernel(const float* __rest
   }
 }
 
-// dq over a K slice, accumulated with fp32 atomics (dq zeroed by the caller path below)
+// dq += K slice sl; one launch per slice, in order (dq zeroed by the caller path below)
 __global__ void __launch_bounds__(256) nce_bwd_slice_kernel(const float* __restrict__ dlogits, const float* __restrict__ k,
-                                                            const float* __restrict__ queue, float T, int D, int K,
+                                                            const float* __restrict__ queue, float T, int D, int K, int sl,
                                                             float* __restrict__ dq) {
   __shared__ float sd[kNceSlice];
-  const int b = blockIdx.x, sl = blockIdx.y;
+  const int b = blockIdx.x;
   const int j0 = sl * kNceSlice, n = min(K - j0, kNceSlice);
   for (int j = threadIdx.x; j < n; j += blockDim.x) sd[j] = dlogits[(long)b * (K + 1) + 1 + j0 + j];
   __syncthreads();
@@ -180,7 +180,7 @@ __global__ void __launch_bounds__(256) nce_bwd_slice_kernel(const float* __restr
     float a = 0.f;
     for (int j = lane; j < n; j += 32) a = fmaf(sd[j], __ldg(queue + (long)c * K + j0 + j), a);
     for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
-    if (lane == 0) atomicAdd(dq + (long)b * D + c, (a + (sl == 0 ? d0 * k[(long)b * D + c] : 0.f)) / T);
+    if (lane == 0) dq[(long)b * D + c] += (a + (sl == 0 ? d0 * k[(long)b * D + c] : 0.f)) / T;
   }
 }
 
@@ -207,8 +207,8 @@ extern "C" int coclr_nce_logits_bwd(const float* dlogits, const float* k, const 
   if (!dlogits || !k || !queue || !dq) return COCLR_E_ARG;
   if (K > 2 * kNceSlice) {
     if (cudaMemsetAsync(dq, 0, sizeof(float) * (size_t)B * D, (cudaStream_t)stream) != cudaSuccess) return COCLR_E_LAUNCH;
-    const dim3 grid(B, (K + kNceSlice - 1) / kNceSlice);
-    nce_bwd_slice_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(dlogits, k, queue, T, D, K, dq);
+    for (int sl = 0; sl < (K + kNceSlice - 1) / kNceSlice; ++sl)
+      nce_bwd_slice_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(dlogits, k, queue, T, D, K, sl, dq);
     return cudaGetLastError() == cudaSuccess ? COCLR_OK : COCLR_E_LAUNCH;
   }
   const size_t smem = (size_t)(K + 1) * sizeof(float);

@@ -1,4 +1,4 @@
-// TMA-staged weight gradient on tcgen05 tensor cores (sm_100a): the cuDNN wgrad reached through loss.backward()
+// TMA-staged weight gradient on wgmma tensor cores (sm_90a): the cuDNN wgrad reached through loss.backward()
 // (reference main_nce.py:330) for the stride-1 (1,k,k) / (k,1,1) / 1x1x1 convolutions of the backbones
 // (backbone/s3dg.py:11-13,39-42; backbone/resnet_2d3d.py).  Same C ABI as the gather kernel in conv_igemm.cu
 // (coclr_conv_wgrad dispatches here first; strided convs and the space-to-depth stem stay on the gather kernel).
@@ -12,17 +12,18 @@
 //  * a work item is (pixel range, group of 64-cout blocks, column group).  Per 64-pixel tile it loads the dY blocks
 //    [64 px][64 cout] of its cout group and ONE halo slab of X: the tile plus the rows the other taps of the reuse
 //    dimension (dy of a (1,3,3) conv, dt of a (k,1,1) conv) need.  The taps are whole 8-row swizzle atoms apart
-//    (tile rows are a multiple of 8 pixels), so they are the N blocks of ONE B descriptor whose "leading byte offset"
-//    is the tap shift: a single tcgen05.mma of N = 64 * kh columns multiplies the dY tile with all kh taps at once,
-//    and each slab byte fetched from L2 is used kh times (the gather kernel re-fetches every tap);
+//    (tile rows are a multiple of 8 pixels), so they are the N blocks of ONE B operand whose block stride is the tap
+//    shift: one K step of N = 64 * kh columns multiplies the dY tile with all kh taps at once, and each slab byte
+//    fetched from L2 is used kh times (the gather kernel re-fetches every tap);
 //  * 1x1x1 convs: the N blocks are up to four 64-channel tiles loaded next to each other;
 //  * convolution padding and ragged tile edges are the TMA unit's out-of-bounds zero fill (a zero dY row or a zero X
 //    row contributes nothing);
 //  * split precision (3 passes over fp16 hi / lo planes) as everywhere; Cout <= 64: hi and lo dY planes are the two
-//    halves of one M = 128 operand (2 instructions per K step, lo x lo included);
-//  * the pixel range is split over CTAs; every CTA ends with fp32 atomics of its [cout, columns] accumulator into dW.
+//    64-row halves of the M = 128 tile (2 products per K step instead of 3, lo x lo included);
+//  * the pixel range is split over CTAs; every CTA ends with its [cout, columns] register accumulator going to a
+//    workspace (summed by one reduction launch) or, without one, with fp32 atomics into dW.
 //
-// Warp roles (192 threads): 0-3 epilogue (TMEM lane quadrant = warp), 4 loader, 5 TMEM owner + MMA issuer.
+// Warp roles (288 threads): 0-7 two MMA warpgroups (64-cout block wg of the item each) + epilogue, 8 loader.
 #include <cuda.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -34,7 +35,9 @@
 
 namespace coclr {
 
-static constexpr int kWgThreads = 6 * 32;
+static constexpr int kWgMmaWarps = 8;
+static constexpr int kWgThreads = (kWgMmaWarps + 1) * 32;
+static constexpr int kWgAccChunks = 8;               // N <= 256: 128 fp32 accumulator registers per thread
 static constexpr int kWgTilePx = 64;                 // pixels per pipeline stage (4 K steps of 16)
 static constexpr int kWgBlockBytes = kWgTilePx * 128;  // one [64 px][64 ch] operand block
 static constexpr int kWgMaxStages = 4;
@@ -58,15 +61,14 @@ struct WgPlan {
   int lbo_bytes;     // distance between consecutive N blocks
   int N;             // columns of one MMA = 64 * blocks (the widest slab type; a type with fewer taps uses 64 * nblk)
   int win_c, win_kw; // window mode (space-to-depth stem): a 64-element block is win_kw pixels of win_c channels
-  int mb;            // 64-cout blocks per item (stacked: 2 = hi / lo plane of the one block)
+  int mb;            // 64-cout blocks per item, one per MMA warpgroup (stacked: 2 = hi / lo plane of the one block)
   int m_groups;      // cout groups
-  int m_tiles;       // M = 128 accumulators per item (1 or 2)
+  int m_tiles;       // M = 128 tiles per item (always 1: two warpgroups of 64 rows)
   int stacked;
   int planes;        // 1 (single pass) or 2 (hi / lo)
   int splits, tiles_per_split;
   int stages;
   uint32_t stage_bytes, off_x, off_bars, total;
-  uint32_t tmem_cols;
   int taps, C, Cin_real, Cout;
 };
 
@@ -124,33 +126,21 @@ wgrad_tma_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid_con
 
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L.off_bars);
   uint64_t* empty_bar = full_bar + kWgMaxStages;
-  uint64_t* tfull_bar = empty_bar + kWgMaxStages;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tfull_bar + 1);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kWgMaxStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], kWgMmaWarps);   // one arrival per consumer warp
     }
-    mbar_init(tfull_bar, 1);
     mbar_fence_init();
   }
-  if (warp == 5) {
-    if (L.tmem_cols == 512) tmem_alloc<512>(tmem_holder);
-    else if (L.tmem_cols == 256) tmem_alloc<256>(tmem_holder);
-    else if (L.tmem_cols == 128) tmem_alloc<128>(tmem_holder);
-    else tmem_alloc<64>(tmem_holder);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_holder, 0);
   const WgType& T = L.type[type_i];
   const int Nt = L.nload > 1 ? L.N : 64 * T.nblk;     // columns of this item's MMAs
   const uint32_t dy_plane_bytes = (uint32_t)L.mb * kWgBlockBytes;
   const uint32_t x_plane_bytes = (uint32_t)L.nload * (uint32_t)L.slab_bytes;
 
-  if (warp == 4) {
+  if (warp == kWgMmaWarps) {
     // ===================== loader =====================
     if (elect_one()) {
       tma_prefetch_desc(&map_dy_hi);
@@ -198,106 +188,75 @@ wgrad_tma_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid_con
         if (++stage == (uint32_t)L.stages) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp == 5) {
-    // ===================== MMA issuer =====================
-    const uint32_t idesc = make_idesc(P.dy_bf16 ? 1u : 0u, P.src_bf16 ? 1u : 0u, 1u, 1u, 128u, (uint32_t)Nt);
+  } else {
+    // ===================== MMA: warpgroup wg multiplies dY block wg (stacked: plane wg) with the X slab =====================
+    const int wg = warp >> 2;
+    const int tw = threadIdx.x & 127;
+    const bool active = L.stacked || wg < L.mb;
+    const bool bf16 = P.dy_bf16 != 0;
+    float acc[16 * kWgAccChunks];
+#pragma unroll
+    for (int i = 0; i < 16 * kWgAccChunks; ++i) acc[i] = 0.f;
     uint32_t stage = 0, phase = 0;
     for (int it = 0; it < ntile; ++it) {
       mbar_wait_spin(&full_bar[stage], phase);
-      tc_fence_after();
-      if (elect_one()) {
+      if (active) {
         const uint32_t s_dy = smem_u32(smem + stage * L.stage_bytes);
         const uint32_t s_x = s_dy + L.off_x;
         // MN-major: LBO = stride between 64-element MN blocks, SBO = stride between 8-pixel groups (one swizzle atom);
         // one K = 16 step = 16 pixels = 2048 bytes = +128 descriptor units
         const uint64_t b_hi = make_smem_desc(s_x, (uint32_t)L.lbo_bytes, 1024);
         const uint64_t b_lo = make_smem_desc(s_x + x_plane_bytes, (uint32_t)L.lbo_bytes, 1024);
-        for (int mt = 0; mt < L.m_tiles; ++mt) {
-          const uint32_t d = tmem_base + (uint32_t)(mt * L.N);
-          const uint64_t a_hi = make_smem_desc(s_dy + mt * 2 * kWgBlockBytes, kWgBlockBytes, 1024);
-          const uint64_t a_lo = make_smem_desc(s_dy + dy_plane_bytes + mt * 2 * kWgBlockBytes, kWgBlockBytes, 1024);
-#pragma unroll
-          for (uint32_t k = 0; k < kWgTilePx / 16; ++k) {
-            const uint32_t first = (it | (int)k) != 0;
-            if (L.planes == 1) {
-              umma_f16(d, a_hi + 128 * k, b_hi + 128 * k, idesc, first);
-            } else if (L.stacked) {
-              umma_f16(d, a_hi + 128 * k, b_lo + 128 * k, idesc, first);
-              umma_f16(d, a_hi + 128 * k, b_hi + 128 * k, idesc, 1u);
-            } else {
-              umma_f16(d, a_hi + 128 * k, b_lo + 128 * k, idesc, first);
-              umma_f16(d, a_lo + 128 * k, b_hi + 128 * k, idesc, 1u);
-              umma_f16(d, a_hi + 128 * k, b_hi + 128 * k, idesc, 1u);
-            }
-          }
+        const uint32_t b_step = (uint32_t)L.lbo_bytes >> 4;
+        const uint64_t a_hi = make_smem_desc(s_dy + (uint32_t)wg * kWgBlockBytes, kWgBlockBytes, 1024);
+        const uint64_t a_lo = make_smem_desc(s_dy + dy_plane_bytes + (uint32_t)wg * kWgBlockBytes, kWgBlockBytes, 1024);
+        if (L.planes == 1) {
+          const uint64_t ad[3] = {a_hi, a_hi, a_hi}, bd[3] = {b_hi, b_hi, b_hi};
+          wgmma_stage<kWgAccChunks, 1, 1>(acc, ad, bd, 1, 128u, 128u, b_step, Nt, bf16);
+        } else if (L.stacked) {
+          const uint64_t ad[3] = {a_hi, a_hi, a_hi}, bd[3] = {b_lo, b_hi, b_hi};
+          wgmma_stage<kWgAccChunks, 1, 1>(acc, ad, bd, 2, 128u, 128u, b_step, Nt, bf16);
+        } else {
+          const uint64_t ad[3] = {a_hi, a_lo, a_hi}, bd[3] = {b_lo, b_hi, b_hi};   // small products first
+          wgmma_stage<kWgAccChunks, 1, 1>(acc, ad, bd, 3, 128u, 128u, b_step, Nt, bf16);
         }
-        umma_commit(&empty_bar[stage]);
-        if (it == ntile - 1) umma_commit(tfull_bar);
       }
       __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
       if (++stage == (uint32_t)L.stages) { stage = 0; phase ^= 1u; }
     }
-  } else {
     // ===================== epilogue =====================
-    // with a workspace: the accumulator goes to ws[item][column][row] with plain coalesced stores (a warp writes 32
-    // consecutive rows of one column) and wgrad_reduce_kernel sums the pixel splits into dW; without one: fp32 atomics
-    // straight into dW[cout, cin, tap]
-    if (ntile > 0) {
-      mbar_wait(tfull_bar, 0);
-      tc_fence_after();
-    }
+    // with a workspace: the accumulator goes to ws[item][column][row] with plain stores and wgrad_reduce_kernel sums the
+    // pixel splits into dW; without one: fp32 atomics straight into dW[cout, cin, tap]
     const float os = P.out_scale != nullptr ? __ldg(P.out_scale) : 1.f;
-    const int R = 128 * L.m_tiles;
-    for (int mt = 0; mt < L.m_tiles; ++mt) {
-      const int row = warp * 32 + lane;               // lane of the accumulator
-      int n;
-      if (L.stacked) {
-        n = row & 63;
-      } else {
-        n = (mg * L.mb + mt * 2) * 64 + row;
-        if (mt * 2 + (row >> 6) >= L.mb) n = L.Cout;  // the upper half of an odd last M tile read a foreign block
-      }
-      for (int c0 = 0; c0 < Nt; c0 += 32) {
-        uint32_t v[32];
-        if (ntile > 0) {
-          tmem_ld_32x32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(mt * L.N + c0), v);
-          tmem_ld_wait();
-        } else {
+    const int R = 128;
+    const int row0 = 64 * wg + 16 * (tw >> 5) + ((tw & 31) >> 2);
+    const int col0 = 2 * (tw & 3);
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = 0u;
-        }
+    for (int c = 0; c < kWgAccChunks; ++c) {
+      if (c * 32 >= Nt) break;
+#pragma unroll
+      for (int r = 0; r < 16; ++r) {
+        const int row = row0 + 8 * ((r >> 1) & 1);      // row of the item's M = 128 tile
+        const int col = c * 32 + col0 + 8 * (r >> 2) + (r & 1);
+        const float v = acc[16 * c + r];
         if (P.ws != nullptr) {
-          float* dst = P.ws + ((size_t)blockIdx.x * L.N + c0) * R + mt * 128 + row;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) dst[(size_t)j * R] = __uint_as_float(v[j]);
-        } else if (n < L.Cout && ntile > 0) {
-          if (L.win_c) {                               // window mode: (tap, channel) changes every win_c columns
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const WgCol k = wg_col(L, T, cg, c0 + j);
-              if (k.c < L.Cin_real)
-                atomicAdd(P.dw + ((size_t)n * L.Cin_real + k.c) * L.taps + k.tap, __uint_as_float(v[j]) * os);
-            }
+          P.ws[((size_t)blockIdx.x * L.N + col) * R + row] = v;
+        } else if (ntile > 0) {
+          int n;
+          if (L.stacked) {
+            n = row & 63;
           } else {
-            const WgCol k = wg_col(L, T, cg, c0);
-            float* dst = P.dw + ((size_t)n * L.Cin_real + k.c) * L.taps + k.tap;
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (k.c + j < L.Cin_real) atomicAdd(dst + (size_t)j * L.taps, __uint_as_float(v[j]) * os);
+            n = (mg * L.mb) * 64 + row;
+            if ((row >> 6) >= L.mb) n = L.Cout;          // the second warpgroup of an odd last block has no rows
+          }
+          if (n < L.Cout) {
+            const WgCol k = wg_col(L, T, cg, col);
+            if (k.c < L.Cin_real) atomicAdd(P.dw + ((size_t)n * L.Cin_real + k.c) * L.taps + k.tap, v * os);
           }
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    __syncwarp();
-    if (L.tmem_cols == 512) tmem_dealloc<512>(tmem_base);
-    else if (L.tmem_cols == 256) tmem_dealloc<256>(tmem_base);
-    else if (L.tmem_cols == 128) tmem_dealloc<128>(tmem_base);
-    else tmem_dealloc<64>(tmem_base);
   }
 }
 
@@ -338,7 +297,7 @@ static int wg_num_sms() {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;
   }
   return n;
 }
@@ -530,21 +489,19 @@ static bool wgrad_tma_plan(const coclr_wgrad_t& P, bool with_ws, WgPlan& L, MapS
   }
   if (L.N > 256 || reuse > 4) return false;
   L.total_tiles = L.ntiles[0] * L.ntiles[1] * L.ntiles[2] * L.ntiles[3];
-  // ---- cout blocks per item: as many as shared memory (>= 2 stages) and tensor memory (2 accumulators) allow ----
+  // ---- cout blocks per item: one per MMA warpgroup, as many as shared memory (>= 2 stages) allows ----
   const int cout_blocks = wg_ceil_div(P.Cout, 64);
   L.stacked = (P.npass > 1 && P.Cout <= 64 && getenv("COCLR_WGRAD_NOSTACK") == nullptr) ? 1 : 0;
   const uint32_t x_bytes = (uint32_t)L.planes * L.nload * L.slab_bytes;
   const uint32_t budget = 227u * 1024u - 2048u;
-  int mb = cout_blocks < 4 ? cout_blocks : 4;
+  int mb = cout_blocks < 2 ? cout_blocks : 2;
   if (L.stacked) mb = 2;
   for (;; --mb) {
     if (mb < 1) return false;
-    const int m_tiles = wg_ceil_div(mb, 2);
-    // an odd block count leaves the upper half of the last M = 128 operand pointing at the next block in memory: the
-    // X region follows, so that read stays inside the stage
+    const int m_tiles = 1;
     const uint32_t dy_bytes = (uint32_t)(L.stacked ? 1 : L.planes) * mb * kWgBlockBytes;
     const uint32_t stage = dy_bytes + x_bytes;
-    if (m_tiles * L.N <= 512 && 2 * stage <= budget) {
+    if (2 * stage <= budget) {
       L.mb = mb;
       L.m_tiles = m_tiles;
       L.off_x = dy_bytes;
@@ -553,15 +510,11 @@ static bool wgrad_tma_plan(const coclr_wgrad_t& P, bool with_ws, WgPlan& L, MapS
     }
     if (L.stacked) return false;
   }
-  if ((L.mb & 1) && !L.stacked && x_bytes < (uint32_t)kWgBlockBytes) return false;
   L.m_groups = L.stacked ? 1 : wg_ceil_div(cout_blocks, L.mb);
   int st = (int)(budget / L.stage_bytes);
   L.stages = st > kWgMaxStages ? kWgMaxStages : st;
   L.off_bars = (uint32_t)L.stages * L.stage_bytes;
   L.total = L.off_bars + 256u + 1024u;
-  uint32_t cols = 32;
-  while (cols < (uint32_t)(L.m_tiles * L.N)) cols <<= 1;
-  L.tmem_cols = cols < 64 ? 64 : cols;
   // ---- pixel splits: one wave of CTAs.  Atomic epilogue: every CTA ends with Cout x N fp32 atomics, measured to
   // dominate once a CTA has fewer than ~16 tiles (and with more than ~74 splits on the same dW); workspace epilogue:
   // plain stores, 4 tiles per CTA are enough to amortise the prologue ----
@@ -610,9 +563,9 @@ int wgrad_tma_try(const coclr_wgrad_t& P, cudaStream_t stream) {
   args.src_bf16 = P.src_bf16;
   if (getenv("COCLR_TMA_DEBUG"))
     fprintf(stderr, "coclr wgrad_tma: tiles %d box %dx%dx%dx%d types %d cgroups %d nload %d N %d mb %d m_groups %d "
-            "stacked %d stages %d stage_bytes %u splits %d tmem %u\n", L.total_tiles, L.box[0], L.box[1], L.box[2],
+            "stacked %d stages %d stage_bytes %u splits %d\n", L.total_tiles, L.box[0], L.box[1], L.box[2],
             L.box[3], L.n_types, L.n_cgroups, L.nload, L.N, L.mb, L.m_groups, L.stacked, L.stages, L.stage_bytes,
-            L.splits, L.tmem_cols);
+            L.splits);
   cudaError_t e = cudaFuncSetAttribute(wgrad_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total);
   if (e != cudaSuccess) return COCLR_E_LAUNCH;
   const int grid = L.n_types * L.n_cgroups * L.m_groups * L.splits;

@@ -1,4 +1,4 @@
-"""Host-side executor of one encoder (S3D backbone + MoCo projection head) on the sm_100a kernels.
+"""Host-side executor of one encoder (S3D backbone + MoCo projection head) on the sm_90a kernels.
 
 The reference runs `encoder_q(x1)` / `encoder_k(x2)` (model/pretrain.py:153,165) as ~250 PyTorch
 module calls; here an encoder pass is a pre-built list of C-ABI kernel launches over pre-allocated
@@ -428,7 +428,7 @@ class Plan:
         fnp, fbf, bnp = PRECISIONS[eng.precision]
         # gradient planes: with fp16 forward planes dY is stored as fp16 hi/lo of dY * 2^k (k per tensor and step, chosen
         # by coclr_bn_bwd from the data's range) so that the weight-gradient GEMM pairs it with the forward planes --
-        # tcgen05 kind::f16 wants one 16-bit format for both operands -- instead of a bf16 twin of every activation
+        # wgmma wants one 16-bit format for both operands -- instead of a bf16 twin of every activation
         gbf = 1 if fbf else 0
         # ---- activations ----
         acts = {}
@@ -693,14 +693,7 @@ class Plan:
                     geom = ops.Geometry(it.k_eff, it.s_eff, it.p_eff)
                     dy = a.dy.src(it.dst_coff, _round8(it.cout), a.dims[0], a.dims[1], a.dims[2])
                     kreal = geom.taps * it.src_C
-                    kt = (kreal + 255) // 256
-                    bnk = (((kreal + kt - 1) // kt) + 63) // 64 * 64
-                    tiles = ((kreal + bnk - 1) // bnk) * ((it.cout + 127) // 128)
-                    chunks = (a.M + 63) // 64
-                    # tiles * splits CTAs, one per SM at a time: stay at or just under whole waves (<= 2 * #SMs)
-                    # ... and every split should own >= 16 pixel chunks: each split ends with Cout x K fp32 atomics,
-                    # which dominate when the pixel range per CTA is short
-                    splits = max(1, min(chunks // 16 if chunks >= 16 else 1, (2 * nsm) // tiles))
+                    splits = 1   # one fp32 add per dW element: reproducible
                     wsrc = sa.plw.src(it.src_coff, it.src_C, sa.dims[0], sa.dims[1], src_w(sa))
                     if it.s2d:
                         # the weight gradient is produced in the space-to-depth layout, then scattered back

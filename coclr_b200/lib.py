@@ -109,7 +109,7 @@ def load():
     if not os.path.exists(_LIB_PATH):
         raise CoclrError(
             "libcoclr_b200.so is missing (%s). Build it with `python -m coclr_b200.build` "
-            "(needs nvcc with sm_100a support). There is no CPU fallback." % _LIB_PATH)
+            "(needs nvcc with sm_90a support). There is no CPU fallback." % _LIB_PATH)
     lib = C.CDLL(_LIB_PATH)
     from . import _signatures
     _signatures.declare(lib)
@@ -159,7 +159,7 @@ _num_sms = {}
 
 def num_sms(device=None):
     if DRY_RUN:
-        return 148
+        return 132   # H100 SXM
     dev = torch.cuda.current_device() if device is None else torch.device(device).index
     if dev not in _num_sms:
         _num_sms[dev] = torch.cuda.get_device_properties(dev).multi_processor_count

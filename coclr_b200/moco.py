@@ -20,9 +20,7 @@ from .engine import Graph, ParamStore, EncoderEngine
 from .s3d_spec import S3D_FEATURE_SIZE
 
 
-# Split all-reduce started in the middle of backward (see _EncodeFn.backward).  Off by default: on 8 x B200 over NVSwitch
-# the 36 MB all-reduce is 0.18 ms when it runs alone after backward, while running it next to the backward kernels
-# lengthened backward by 0.3 ms (profiles/r02_scale8_timeline.json); COCLR_OVERLAP_ALLREDUCE=1 enables it.
+# Split all-reduce started in the middle of backward (see _EncodeFn.backward); COCLR_OVERLAP_ALLREDUCE=1 enables it.
 OVERLAP_ALLREDUCE = os.environ.get("COCLR_OVERLAP_ALLREDUCE", "0") == "1"
 
 # Per-phase timeline of a step (bench.py --timeline): CUDA events on whatever stream the phase runs on; off by default.
@@ -134,7 +132,7 @@ class MoCoEncoder(nn.Sequential):
     def _engine_for(self, device):
         w = self[2].weight
         if not w.is_cuda:
-            raise L.CoclrError("coclr_b200 encoders run on CUDA (sm_100a) only; there is no CPU path")
+            raise L.CoclrError("coclr_b200 encoders run on CUDA (sm_90a) only; there is no CPU path")
         e = self._engine
         if e is None or e.store.device != w.device or w.data_ptr() != e.store.view("2.weight").data_ptr():
             bb = self[0]

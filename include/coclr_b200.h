@@ -1,5 +1,5 @@
 /*
- * coclr_b200 -- C ABI of the B200 (sm_100a) kernels behind the CoCLR data-parallel hot path.
+ * coclr_b200 -- C ABI of the H100 (sm_90a) kernels behind the CoCLR data-parallel hot path.
  *
  * The reference (TengdaHan/CoCLR) has no FFI layer: its hot path is Python calling nn.Conv3d /
  * nn.BatchNorm3d / nn.MaxPool3d / torch.einsum (SURVEY.md section 8b).  Each entry point below
@@ -28,7 +28,7 @@ extern "C" {
 #define COCLR_OK 0
 #define COCLR_E_ARG (-1)    /* bad argument (shape / alignment / null) */
 #define COCLR_E_LAUNCH (-2) /* CUDA launch error (cudaGetLastError != success) */
-#define COCLR_E_DEVICE (-3) /* not an sm_100 device */
+#define COCLR_E_DEVICE (-3) /* not an sm_90 device */
 
 typedef void* coclr_stream_t; /* cudaStream_t */
 
@@ -61,7 +61,7 @@ typedef struct {
   int Kreal;         /* taps * src.C */
   const void* wpk;   /* packed weights from coclr_pack_weights */
   const float* wunscale; /* [n_tiles*BN] per-column 1/scale, or NULL */
-  int N, BN, n_tiles;    /* real output channels, tile width (multiple of 32, <= 256), tiles */
+  int N, BN, n_tiles;    /* real output channels, tile width (multiple of 32, <= 128), tiles */
   float* dst;            /* fp32 [B,Td,Hd,Wd,dst_ld] */
   int dst_ld, dst_coff;
   int accumulate;    /* dst += result */
@@ -173,7 +173,7 @@ typedef struct {
   int out_ld, out_coff;
   int bf16;
   void* hi2; /* optional bf16 twin of the planes (same out_ld / out_coff) for the weight-gradient GEMM, whose */
-  void* lo2; /* two operands must share one 16-bit format (tcgen05 kind::f16); NULL to skip */
+  void* lo2; /* two operands must share one 16-bit format (wgmma); NULL to skip */
   /* optional fused BatchNorm finalize (bn.scale != NULL): scale/shift are derived in-kernel from the statistics
    * (bn.training) or the running stats, written to bn.scale/bn.shift/bn.save_* and the running stats are updated
    * by one block -- saves the separate coclr_bn_finalize launch; `scale`/`shift` above are then ignored */
@@ -215,7 +215,7 @@ typedef struct {
   /* dy_fp16 != 0: the planes are written as fp16 hi/lo of dY * s, s a power of two chosen per call so that the largest
    * |dY| the data allows (a per-channel bound from max |dz|, max |xhat| and the two means, reduced over the channels)
    * lands at 2^14: ~22 significant bits near the top of the range instead of bf16 hi/lo's 16, and the weight-gradient
-   * GEMM can pair them with the forward pass's fp16 activation planes (tcgen05 kind::f16 needs one format for both
+   * GEMM can pair them with the forward pass's fp16 activation planes (wgmma needs one format for both
    * operands) -- no bf16 twin of every activation.  dy_scale[0] = s, dy_scale[1] = 1/s (device, written by the call;
    * consumers pass &dy_scale[1] as out_scale).  amax: workspace [2*C] floats. */
   int dy_fp16;
@@ -310,7 +310,7 @@ int coclr_adam_step(const coclr_adam_t* p, int num_sms, coclr_stream_t stream);
  * logits[b, 0] = q_b.k_b / T, logits[b, 1+j] = q_b.queue[:, j] / T; loss_rows[b] = logsumexp - logits[b,0];
  * dlogits = d(mean_b loss_rows)/d(logits).  loss_rows / dlogits may be NULL.
  * ws: optional scratch of 2 * B * ceil(K / 1024) floats; with it, queues longer than 2048 are cut into 1024-column
- * slices on separate CTAs (config 3: K = 16384 would otherwise run on B of the 148 SMs). */
+ * slices on separate CTAs (config 3: K = 16384 would otherwise run on B of the 132 SMs). */
 int coclr_nce_logits_ce(const float* q, const float* k, const float* queue, float T, int B, int D, int K,
                         float* logits, float* loss_rows, float* dlogits, float* ws, coclr_stream_t stream);
 /* dq = d(logits)^T contraction with [k | queue] / T (no gradient to k or the queue, pretrain.py:160,176) */

@@ -3,7 +3,7 @@
 Same constructors, forward signatures, return values, buffers (`queue`, `queue_ptr`, `queue_label`,
 `queue_second`, `queue_vname`) and state_dict key names as TengdaHan/CoCLR model/pretrain.py:28-418, so
 main_nce.py / main_coclr.py and reference checkpoints keep working; the arithmetic runs on coclr_b200's
-sm_100a kernels (CUDA only -- constructing on CPU is fine, calling forward on CPU raises).
+sm_90a kernels (CUDA only -- constructing on CPU is fine, calling forward on CPU raises).
 
 What changed under the surface (see DESIGN.md):
   * encoders run as fused engine passes (coclr_b200.engine), BN/ReLU folded into the convs;
@@ -188,7 +188,7 @@ class InfoNCE(nn.Module):
 
     def _qk(self, block):
         if not block.is_cuda:
-            raise moco.L.CoclrError("coclr_b200 modules run on CUDA (sm_100a) only; there is no CPU path")
+            raise moco.L.CoclrError("coclr_b200 modules run on CUDA (sm_90a) only; there is no CPU path")
         x1, x2 = self._views(block)                # views; the .contiguous() copies are folded into packing
         in_train_mode = torch.is_grad_enabled() and any(p.requires_grad for p in self.encoder_q.parameters())  # :157
         # the key branch (EMA -> shuffle -> encoder_k) does not depend on the query forward: run it on a side stream
@@ -274,7 +274,7 @@ class CoCLR(InfoNCE):
         the second view -- on three streams; they only share read-only inputs (reference pretrain.py:358-374 runs them
         one after the other)."""
         if not x1.is_cuda:
-            raise moco.L.CoclrError("coclr_b200 modules run on CUDA (sm_100a) only; there is no CPU path")
+            raise moco.L.CoclrError("coclr_b200 modules run on CUDA (sm_90a) only; there is no CPU path")
         in_train_mode = torch.is_grad_enabled() and any(p.requires_grad for p in self.encoder_q.parameters())
         main = torch.cuda.current_stream()
         if self._side_stream is None:

@@ -5,13 +5,13 @@ S3D encoder + MoCo/InfoNCE step in stock PyTorch ops.  Only tests/, __graft_entr
 bench.py's cpu_baseline / --impl reference legs may import it; the product (coclr_b200/, model/,
 backbone/) never does.
 
-Pinned (in the build container, where /root/reference is mounted, the UNMODIFIED reference modules are executed
-and compared bit-for-bit on logits / loss / queue / masks and to 1e-6 on all post-step state):
+Pinned against what the UNMODIFIED reference modules computed (bit-for-bit on logits / loss / queue / masks, to 1e-6 on
+the recorded post-step state):
   tests/test_oracle.py       InfoNCE with the S3D and the ResNet2d3d-50 backbone; adam_step against torch.optim.Adam
   tests/test_oracle_ext.py   UberNCE, CoCLR (queue warm-up and queue-full phases, top-k mining)
   tests/test_oracle_dist.py  the simulated multi-rank world against the reference run as two gloo DDP ranks
-tests/golden/*.npz hold the reference outputs produced by tests/golden/make_golden*.py for use where the reference
-is absent (the GPU box); the same tests check the oracle against them.
+tests/golden/*.npz hold the reference outputs produced by tests/golden/make_golden*.py (run with COCLR_REFERENCE
+pointing at a reference checkout); the tests check the oracle against them.
 
 Every function cites the reference file:line it restates (paths relative to TengdaHan/CoCLR).
 State is a flat dict {state_dict key: tensor} with exactly the reference's key names, e.g.

@@ -1,5 +1,5 @@
 """Generates tests/golden/infonce_cfg1.npz (and, with the argument `r50` / `s3dg`, infonce_r50.npz / infonce_s3dg.npz) by running the UNMODIFIED reference (TengdaHan/CoCLR at
-/root/reference, model/pretrain.py InfoNCE) on BASELINE.json config 1 (S3D, moco-k=128, bs=4,
+$COCLR_REFERENCE, model/pretrain.py InfoNCE) on BASELINE.json config 1 (S3D, moco-k=128, bs=4,
 seq_len=8, 128x128, CPU) from the deterministic synthetic state of oracle.coclr_oracle.synth_state.
 
 Run in the build container only:  python tests/golden/make_golden.py
@@ -15,7 +15,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-REF = "/root/reference"
+REF = os.environ.get("COCLR_REFERENCE", "")   # a checkout of TengdaHan/CoCLR (only the generators read it)
 
 
 def make_inputs(B=4, T=8, HW=128, seed=1234):  # noqa
@@ -40,6 +40,30 @@ def compact(a, limit=16384):
         return a.copy(), None
     stride = -(-a.size // limit)
     return a.reshape(-1)[::stride].copy(), np.float64(np.linalg.norm(a.astype(np.float64)))
+
+
+STATE_SAMPLE = 32   # elements kept per post-step state tensor
+
+
+def state_record(model):
+    """Post-step state_dict keys and a strided sample of every tensor (aliases once), as one float64 array."""
+    msd = model.state_dict()
+    keys, parts, seen = [], [], set()
+    for k in sorted(msd):
+        v = msd[k]
+        if v.numel() and v.data_ptr() in seen:
+            continue
+        seen.add(v.data_ptr())
+        keys.append(k)
+        parts.append(compact(v.detach().numpy(), STATE_SAMPLE)[0].astype(np.float64).ravel())
+    return {"state_keys": np.array("\n".join(sorted(msd))), "state_sampled": np.array("\n".join(keys)),
+            "state_len": np.array([len(p) for p in parts]), "state_sample": np.concatenate(parts)}
+
+
+def state_samples(gold):
+    keys = str(gold["state_sampled"]).split("\n")
+    off = np.concatenate([[0], np.cumsum(gold["state_len"])])
+    return {k: gold["state_sample"][off[i]:off[i + 1]] for i, k in enumerate(keys)}
 
 
 GRAD_KEYS = ["encoder_q.0.Conv_1a.conv1.weight", "encoder_q.0.Conv_1a.bn2.weight", "encoder_q.0.Conv_2c.conv2.weight",
@@ -106,9 +130,12 @@ def run_reference(K=128, B=4, T=8, ptr=16, threads=8, network="s3d", HW=128):
     out = {"logits": logits.detach().numpy(), "loss": np.float64(loss.item()),
            "queue": model.queue.numpy().copy(), "queue_ptr": model.queue_ptr.numpy().copy()}
     named = dict(model.named_parameters())
+    out.update(state_record(model))
     if network == "s3d":
         for k in GRAD_KEYS:
-            out["grad/" + k] = named[k].grad.numpy().copy()
+            out["grad/" + k], nrm = compact(named[k].grad.numpy())
+            if nrm is not None:
+                out["gradnorm/" + k] = nrm
     if network == "s3dg":
         for k in GRAD_KEYS_S3DG:
             out["grad/" + k], nrm = compact(named[k].grad.numpy())
@@ -121,11 +148,11 @@ def run_reference(K=128, B=4, T=8, ptr=16, threads=8, network="s3d", HW=128):
             if nrm is not None:
                 out["gradnorm/" + k] = nrm
         full = model.state_dict()
-        out["ema/encoder_k.0.layer2.0.conv2.weight"] = named["encoder_k.0.layer2.0.conv2.weight"].detach().numpy().copy()
+        out["ema/encoder_k.0.layer2.0.conv2.weight"] = compact(named["encoder_k.0.layer2.0.conv2.weight"].detach().numpy())[0]
         out["bn/encoder_q.0.layer1.0.downsample.1.running_mean"] = full["encoder_q.0.layer1.0.downsample.1.running_mean"].numpy().copy()
         out["bn/encoder_k.0.layer4.2.bn3.running_var"] = full["encoder_k.0.layer4.2.bn3.running_var"].numpy().copy()
         return out, model
-    out["ema/encoder_k.0.Conv_2c.conv1.weight"] = named["encoder_k.0.Conv_2c.conv1.weight"].detach().numpy().copy()
+    out["ema/encoder_k.0.Conv_2c.conv1.weight"] = compact(named["encoder_k.0.Conv_2c.conv1.weight"].detach().numpy())[0]
     out["bn/encoder_q.0.Conv_1a.bn1.running_mean"] = model.state_dict()["encoder_q.0.Conv_1a.bn1.running_mean"].numpy().copy()
     out["bn/encoder_k.0.Mixed_5c.branch0.0.bn.running_var"] = model.state_dict()["encoder_k.0.Mixed_5c.branch0.0.bn.running_var"].numpy().copy()
     return out, model

@@ -14,6 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, HERE)
+import make_golden as MG  # noqa: E402
 
 CFG = dict(W=2, B=2, T=8, HW=64, K=32, ptr=8, threads=4, perm_seed=77)
 GRAD_KEYS = ["encoder_q.0.Conv_1a.conv1.weight", "encoder_q.0.Conv_2c.bn1.weight", "encoder_q.0.Mixed_3c.branch1.1.conv2.weight",
@@ -70,7 +71,7 @@ def run_reference_world2(out_dir):
     for k in r[0].files:
         if k.startswith("grad/") or k.startswith("ema/"):
             assert np.array_equal(r[0][k], r[1][k]), k          # DDP leaves identical averaged gradients on every rank
-            out[k] = r[0][k]
+            out[k] = MG.compact(r[0][k])[0]
     return out
 
 

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 implicit-GEMM convolution (forward, dgrad, wgrad), the BatchNorm-apply/ReLU/split
+"""GPU parity of the wgmma implicit-GEMM convolution (forward, dgrad, wgrad), the BatchNorm-apply/ReLU/split
 kernel that feeds it, and max-pooling, against torch.nn.functional evaluated in float64 -- the ops the reference
 reaches through nn.Conv3d / nn.BatchNorm3d / nn.MaxPool3d (backbone/s3dg.py:11-17,39-48,105).  Tolerances:
 3-pass fp16 split precision must be fp32-grade (2e-5 of the output scale), 3-pass bf16 2e-4; the single-pass
@@ -136,7 +136,7 @@ def test_conv_forward(case, npass, bf16, diag):
 
 @pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
 def test_conv_accumulate(case, diag):
-    """dst += result (bf16 planes x bf16 weights; tcgen05 kind::f16 needs one format for both operands)."""
+    """dst += result (bf16 planes x bf16 weights; wgmma needs one format for both operands)."""
     ops, geom, x, w = _setup(case, seed=3)
     name, Cin, Cout, k, s, p, B, T, H, W = case
     To, Ho, Wo = geom.out_dims(T, H, W)

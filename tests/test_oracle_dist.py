@@ -1,7 +1,7 @@
 """Pins the oracle's SIMULATED multi-rank world (oracle.infonce_forward with several blocks: shuffle-BN permutation,
 un-shuffle, global enqueue; model/pretrain.py:82-143) and the DDP gradient averaging (main_nce.py:172) against the
 unmodified reference run as two real gloo ranks: (1) against tests/golden/infonce_world2.npz -- runs anywhere;
-(2) live against the reference when /root/reference is mounted."""
+(2) bit-for-bit against the same recorded outputs."""
 import os
 import sys
 
@@ -46,9 +46,10 @@ def _check(sd, logits, losses, gold, tol_fwd, tol_grad):
         assert abs(float(losses[r]) - float(gold["loss%d" % r])) <= max(tol_fwd, 1e-12) * max(1.0, abs(float(gold["loss%d" % r])))
     assert _rel(sd["queue"].numpy(), gold["queue"]) <= tol_fwd
     assert int(sd["queue_ptr"]) == int(gold["queue_ptr"][0]) == c["ptr"] + c["B"] * c["W"]
-    assert _rel(sd["encoder_k.0.Conv_2c.conv1.weight"].detach().numpy(), gold["ema/encoder_k.0.Conv_2c.conv1.weight"]) <= 1e-6
+    ema = MD.MG.compact(sd["encoder_k.0.Conv_2c.conv1.weight"].detach().numpy())[0]
+    assert _rel(ema, gold["ema/encoder_k.0.Conv_2c.conv1.weight"]) <= 1e-6
     for k in MD.GRAD_KEYS:
-        assert _rel(sd[k].grad.numpy(), gold["grad/" + k]) <= tol_grad, k
+        assert _rel(MD.MG.compact(sd[k].grad.numpy())[0], gold["grad/" + k]) <= tol_grad, k
 
 
 def test_oracle_world2_matches_golden():
@@ -57,10 +58,10 @@ def test_oracle_world2_matches_golden():
     _check(sd, logits, losses, np.load(GOLD), tol_fwd=2e-4, tol_grad=5e-2)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/model"), reason="reference not mounted")
 @pytest.mark.timeout(900)
-def test_oracle_world2_vs_live_reference(tmp_path):
-    out = MD.run_reference_world2(str(tmp_path))
+def test_oracle_world2_bitwise_vs_reference():
+    """Bit-for-bit against the reference's recorded two-rank outputs (4 CPU threads per rank, x86-64 fp32 kernels)."""
+    out = np.load(GOLD)
     sd, logits, losses = _oracle_world2()
     for r in range(MD.CFG["W"]):
         assert np.array_equal(logits[r].detach().numpy(), out["logits%d" % r]), "per-rank logits differ from the reference"

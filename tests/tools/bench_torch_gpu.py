@@ -1,6 +1,6 @@
 """Measurement tool (test infrastructure, not product): times the oracle -- the reference's algorithm in stock
-PyTorch ops -- on the GPU, i.e. what the unmodified reference would do on a B200 through cuDNN/cuBLAS.
-Reported next to our numbers as "the Blackwell kernel to beat" (SURVEY.md 2a).  Usage:
+PyTorch ops -- on the GPU, i.e. what the unmodified reference would do on this GPU through cuDNN/cuBLAS.
+Reported next to our numbers as "the kernel to beat" (SURVEY.md 2a).  Usage:
     python tests/tools/bench_torch_gpu.py [--batch 32] [--steps 5] [--mode fp32|tf32|bf16]"""
 import argparse
 import json

@@ -1,6 +1,6 @@
 """Diagnostic (test infrastructure): the smoke() configuration (S3D, K=128, batch 2, 8 frames, 64x64) with every
 post-BN activation of encoder_q / encoder_k compared against the float64 oracle and the float32 oracle.  Env toggles of
-the library (COCLR_TMA=0, COCLR_POOL333_REG=1, COCLR_POOL133_REG=1, COCLR_TMA_NOSTACK=1) bisect a regression.
+the library (COCLR_TMA=0, COCLR_POOL333_REG=1, COCLR_POOL133_REG=1) bisect a regression.
   python tests/tools/smoke_layerwise.py [B] [T] [HW]"""
 import os
 import sys
