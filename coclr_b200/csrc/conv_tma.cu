@@ -14,14 +14,18 @@
 //    pixels wide), so every slab byte fetched from L2 feeds up to kh (kt) x 12 K-steps of tensor-core instructions;
 //  * weights: the pre-swizzled hi / lo tile images of coclr_pack_weights, either streamed through a ring of
 //    bulk copies or -- for narrow layers whose whole image fits -- loaded ONCE per CTA and kept resident;
-//  * two consumer warpgroups (64 tile rows each) accumulate in registers with wgmma; the accumulator goes
-//    through a [128][33] fp32 transpose tile 32 columns at a time, from which warps 0-3 (32 rows each) fill a
-//    swizzled staging row block, accumulate the BatchNorm statistics from it, and write it with ONE
+//  * two consumer warpgroups (64 tile rows each) accumulate in registers with wgmma: one m64 x BN x k16 instruction
+//    per product and K step, BN fixed at compile time.  Each 64-deep K chunk (a pipeline stage) is summed in a fresh
+//    register block and added to the accumulator in fp32; the next stage's instructions are issued before that add,
+//    so the tensor cores are not idle while a stage is folded and its shared-memory slots are released.  The
+//    accumulator goes through a [128][33] fp32 transpose tile 32 columns at a time, from which warps 4-7 (32 rows
+//    each) fill a swizzled staging row block, accumulate the BatchNorm statistics from it, and write it with ONE
 //    cp.async.bulk.tensor store (or add-reduction, for gradient accumulation) per 32 rows x 32 channels: edge
 //    clipping, channel slices of concat buffers and the strided frame order of the transposed stem conv are
 //    properties of the output tensor map, not code.
 //
-// Warp roles (320 threads): 0-7 MMA + epilogue, 8 A loader, 9 weight loader.
+// Warp roles (384 threads, three warpgroups): 0 A loader, 1 weight loader, 2-3 idle (warpgroup 0 gives its registers to
+// the consumers), 4-11 MMA (warpgroups 1 and 2), 4-7 also the epilogue.
 #include <cuda.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -33,9 +37,11 @@
 
 namespace coclr {
 
-static constexpr int kTmaThreads = 10 * 32;
+static constexpr int kTmaThreads = 12 * 32;
 static constexpr int kTmaMmaWarps = 8;
-static constexpr int kTmaAccChunks = 4;        // BN <= 128: 64 fp32 accumulator registers per thread
+static constexpr int kTmaFirstMmaWarp = 4;     // warpgroup 0 loads, warpgroups 1-2 compute
+static constexpr int kTmaMaxBN = 128;          // 64 fp32 accumulator registers per thread
+static constexpr uint32_t kTmaLoaderRegs = 40, kTmaMmaRegs = 232;   // 128 x 40 + 256 x 232 <= 64 Ki registers
 static constexpr int kXPitch = 33;             // floats per row of the accumulator transpose tile
 static constexpr uint32_t kXTileBytes = 128u * kXPitch * 4u;
 static constexpr int kTmaMaxASlots = 4;
@@ -60,7 +66,17 @@ COCLR_DEVINL TmaTile tma_decode(const TmaPlan& L, int item) {
   return t;
 }
 
-template <int kNPass>
+// The tile's first slab type: t.idx[sel_dim] when the tile index selects it, else 0.  Selected without indexing t.idx at
+// run time, which would put t in local memory.
+COCLR_DEVINL int tma_first_type(const TmaPlan& L, const TmaTile& t) {
+  int ty = 0;
+#pragma unroll
+  for (int d = 0; d < 4; ++d)
+    if (L.sel_dim == d) ty = t.idx[d];
+  return ty;
+}
+
+template <int kNPass, int kBN, bool kBf16>
 __global__ void __launch_bounds__(kTmaThreads, 1)
     conv_tma_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
                     const __grid_constant__ CUtensorMap map_out, const __grid_constant__ TmaArgs P) {
@@ -68,6 +84,8 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr bool kLo = kNPass > 1;
   constexpr uint32_t kPlanes = kLo ? 2u : 1u;
+  constexpr int kChunks = kBN / 32;                       // 32-column epilogue chunks
+  constexpr uint32_t kBTileBytes = kPlanes * kBN * 128u;  // one K chunk of weights (hi, lo) in shared memory
   const TmaPlan& L = P.plan;
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t a_base = smem_base;
@@ -80,7 +98,7 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
   uint64_t* b_full = a_empty + kTmaMaxASlots;
   uint64_t* b_empty = b_full + kTmaMaxBSlots;
 
-  const int warp = threadIdx.x >> 5;
+  const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);   // provably warp-uniform role branches for ptxas
   const int lane = threadIdx.x & 31;
   const int first_item = (int)blockIdx.x;
   const int item_stride = (int)gridDim.x;
@@ -89,11 +107,11 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
   if (threadIdx.x == 0) {
     for (int s = 0; s < kTmaMaxASlots; ++s) {
       mbar_init(&a_full[s], 1);
-      mbar_init(&a_empty[s], kTmaMmaWarps);   // one arrival per consumer warp
+      mbar_init(&a_empty[s], kTmaMmaWarps * 32);   // one arrival per consumer thread
     }
     for (int s = 0; s < kTmaMaxBSlots; ++s) {
       mbar_init(&b_full[s], 1);
-      mbar_init(&b_empty[s], kTmaMmaWarps);
+      mbar_init(&b_empty[s], kTmaMmaWarps * 32);
     }
     mbar_fence_init();
   }
@@ -101,61 +119,64 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
     unscale_tab[i] = 1.f;  // per tile the epilogue reads n_tile*BN + c; filled below when there is a table
   __syncthreads();
 
-  if (warp == kTmaMmaWarps) {
-    // ===================== A loader: one TMA box (hi) + one (lo) per slab =====================
-    if (elect_one()) {
-      tma_prefetch_desc(&map_hi);
-      if (kLo) tma_prefetch_desc(&map_lo);
-      uint32_t slot = 0, phase = 0;
-      for (int item = first_item; item < n_items; item += item_stride) {
-        const TmaTile t = tma_decode(L, item);
-        const int ty0 = L.sel_dim >= 0 ? t.idx[L.sel_dim] : 0;
-        const int ty1 = L.sel_dim >= 0 ? ty0 + 1 : L.n_types;
-        for (int cc = 0; cc < L.nc; ++cc) {
-          for (int ty = ty0; ty < ty1; ++ty) {
-            const TmaSlabType& S = L.type[ty];
-            mbar_wait(&a_empty[slot], phase ^ 1u);
-            const int c0 = cc * L.a_c0_step;
-            const int c1 = t.idx[0] * L.a_mul[0] + S.d[0];
-            const int c2 = t.idx[1] * L.a_mul[1] + S.d[1];
-            const int c3 = t.idx[2] * L.a_mul[2] + S.d[2];
-            const int c4 = t.idx[3] * L.a_mul[3] + S.d[3];
-            const uint32_t dst = a_base + slot * (uint32_t)L.a_slot_bytes;
-            mbar_arrive_expect_tx(&a_full[slot], kPlanes * (uint32_t)L.slab_bytes);
-            tma_load_5d(dst, &map_hi, &a_full[slot], c0, c1, c2, c3, c4);
-            if (kLo) tma_load_5d(dst + (uint32_t)L.plane_stride, &map_lo, &a_full[slot], c0, c1, c2, c3, c4);
-            if (++slot == (uint32_t)L.a_slots) { slot = 0; phase ^= 1u; }
-          }
-        }
-      }
-    }
-  } else if (warp == kTmaMmaWarps + 1) {
-    // ===================== weight loader: bulk copies of pre-swizzled tile images =====================
-    if (elect_one()) {
-      const uint32_t tile_bytes = kPlanes * (uint32_t)L.BN * 128u;          // what one K chunk needs in smem
-      const size_t img_stride = (size_t)2u * (size_t)L.BN * 128u;            // packed image: hi and lo of every chunk
-      const uint8_t* wbase = reinterpret_cast<const uint8_t*>(P.wpk);
-      if (L.b_resident) {
-        // the whole [nkc] image of the (single) N tile, once
-        mbar_arrive_expect_tx(&b_full[0], (uint32_t)L.nkc * tile_bytes);
-        for (int kc = 0; kc < L.nkc; ++kc)
-          bulk_g2s(smem + L.off_b + (size_t)kc * tile_bytes, wbase + (size_t)kc * img_stride, tile_bytes, &b_full[0]);
-      } else {
+  if (warp < kTmaFirstMmaWarp) {
+    setmaxnreg_dec<kTmaLoaderRegs>();   // warpgroup 0: the loader warps 0-1, and warps 2-3 idle
+    if (warp == 0) {
+      // ===================== A loader: one TMA box (hi) + one (lo) per slab =====================
+      if (elect_one()) {
+        tma_prefetch_desc(&map_hi);
+        if (kLo) tma_prefetch_desc(&map_lo);
         uint32_t slot = 0, phase = 0;
         for (int item = first_item; item < n_items; item += item_stride) {
           const TmaTile t = tma_decode(L, item);
-          const int ty0 = L.sel_dim >= 0 ? t.idx[L.sel_dim] : 0;
+          const int ty0 = tma_first_type(L, t);
           const int ty1 = L.sel_dim >= 0 ? ty0 + 1 : L.n_types;
           for (int cc = 0; cc < L.nc; ++cc) {
             for (int ty = ty0; ty < ty1; ++ty) {
               const TmaSlabType& S = L.type[ty];
-              for (int j = 0; j < S.nshift; ++j) {
-                const int kc = S.tap[j] * L.nc + cc;
-                mbar_wait(&b_empty[slot], phase ^ 1u);
-                mbar_arrive_expect_tx(&b_full[slot], tile_bytes);
-                bulk_g2s(smem + L.off_b + (size_t)slot * tile_bytes,
-                         wbase + ((size_t)t.n_tile * L.nkc + kc) * img_stride, tile_bytes, &b_full[slot]);
-                if (++slot == (uint32_t)L.b_slots) { slot = 0; phase ^= 1u; }
+              mbar_wait(&a_empty[slot], phase ^ 1u);
+              const int c0 = cc * L.a_c0_step;
+              const int c1 = t.idx[0] * L.a_mul[0] + S.d[0];
+              const int c2 = t.idx[1] * L.a_mul[1] + S.d[1];
+              const int c3 = t.idx[2] * L.a_mul[2] + S.d[2];
+              const int c4 = t.idx[3] * L.a_mul[3] + S.d[3];
+              const uint32_t dst = a_base + slot * (uint32_t)L.a_slot_bytes;
+              mbar_arrive_expect_tx(&a_full[slot], kPlanes * (uint32_t)L.slab_bytes);
+              tma_load_5d(dst, &map_hi, &a_full[slot], c0, c1, c2, c3, c4);
+              if (kLo) tma_load_5d(dst + (uint32_t)L.plane_stride, &map_lo, &a_full[slot], c0, c1, c2, c3, c4);
+              if (++slot == (uint32_t)L.a_slots) { slot = 0; phase ^= 1u; }
+            }
+          }
+        }
+      }
+    } else if (warp == 1) {
+      // ===================== weight loader: bulk copies of pre-swizzled tile images =====================
+      if (elect_one()) {
+        const uint32_t tile_bytes = kBTileBytes;                               // what one K chunk needs in smem
+        const size_t img_stride = (size_t)2u * (size_t)kBN * 128u;             // packed image: hi and lo of every chunk
+        const uint8_t* wbase = reinterpret_cast<const uint8_t*>(P.wpk);
+        if (L.b_resident) {
+          // the whole [nkc] image of the (single) N tile, once
+          mbar_arrive_expect_tx(&b_full[0], (uint32_t)L.nkc * tile_bytes);
+          for (int kc = 0; kc < L.nkc; ++kc)
+            bulk_g2s(smem + L.off_b + (size_t)kc * tile_bytes, wbase + (size_t)kc * img_stride, tile_bytes, &b_full[0]);
+        } else {
+          uint32_t slot = 0, phase = 0;
+          for (int item = first_item; item < n_items; item += item_stride) {
+            const TmaTile t = tma_decode(L, item);
+            const int ty0 = tma_first_type(L, t);
+            const int ty1 = L.sel_dim >= 0 ? ty0 + 1 : L.n_types;
+            for (int cc = 0; cc < L.nc; ++cc) {
+              for (int ty = ty0; ty < ty1; ++ty) {
+                const TmaSlabType& S = L.type[ty];
+                for (int j = 0; j < S.nshift; ++j) {
+                  const int kc = S.tap[j] * L.nc + cc;
+                  mbar_wait(&b_empty[slot], phase ^ 1u);
+                  mbar_arrive_expect_tx(&b_full[slot], tile_bytes);
+                  bulk_g2s(smem + L.off_b + (size_t)slot * tile_bytes,
+                           wbase + ((size_t)t.n_tile * L.nkc + kc) * img_stride, tile_bytes, &b_full[slot]);
+                  if (++slot == (uint32_t)L.b_slots) { slot = 0; phase ^= 1u; }
+                }
               }
             }
           }
@@ -163,14 +184,15 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
       }
     }
   } else {
-    // ===================== MMA (warps 0-7: two warpgroups of 64 rows), then the epilogue (warps 0-3) =====================
-    const int wg = warp >> 2;
+    setmaxnreg_inc<kTmaMmaRegs>();
+    // ===================== MMA (warps 4-11: two warpgroups of 64 rows), then the epilogue (warps 4-7) =====================
+    const int cwarp = warp - kTmaFirstMmaWarp;               // warp index among the consumers
+    const int ct = (int)threadIdx.x - kTmaFirstMmaWarp * 32;  // thread index among the consumers
+    const int wg = cwarp >> 2;
     const int tid_wg = threadIdx.x & 127;
-    const bool bf16 = P.a_bf16 != 0;
-    const bool epi = warp < 4;
-    const uint32_t tile_bytes = (uint32_t)L.b_tile_bytes;
+    const bool epi = cwarp < 4;
     const uint32_t a_row_off = (uint32_t)wg * 64u * 128u;   // this warpgroup's 64 rows of the slab window
-    float acc[16 * kTmaAccChunks];
+    float acc[kBN / 2];
     uint32_t aslot = 0, aphase = 0, bslot = 0, bphase = 0;
     if (L.b_resident) mbar_wait_spin(&b_full[0], 0);
 
@@ -180,25 +202,25 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
     const bool leader = elect_one();
     const float oscale = P.out_scale != nullptr ? __ldg(P.out_scale) : 1.f;
     if (epi && (P.wunscale != nullptr || P.out_scale != nullptr) && L.n_tiles_n == 1) {
-      for (int i = threadIdx.x; i < L.BN; i += 128)
+      for (int i = ct; i < kBN; i += 128)
         unscale_tab[i] = (P.wunscale != nullptr ? __ldg(P.wunscale + i) : 1.f) * oscale;
     }
     if (epi) named_bar_sync(1, 128);
-    const uint32_t my_stage = stage_base + (uint32_t)(warp & 3) * (uint32_t)L.stage_bufs * kStageBytes;
+    const uint32_t my_stage = stage_base + (uint32_t)(cwarp & 3) * (uint32_t)L.stage_bufs * kStageBytes;
     // BatchNorm statistics: per column, sum and sum of squares of d = x - x0 in fp32, where x0 is the first value of
     // the column this CTA sees; converted exactly in double when they leave the CTA:
     //   sum x = sum d + n x0,  sum x^2 = sum d^2 + 2 x0 sum d + n x0^2,
     // so that var = E[x^2] - mean^2 (formed in double by the finalize step) does not lose the variance of channels whose
     // spread is small against their mean to fp32 rounding of the raw sums (nn.BatchNorm3d is two-pass)
-    float s1[4], s2[4], x0[4];
+    float s1[kChunks], s2[kChunks], x0[kChunks];
     uint32_t x0_set = 0u;
     int nrows = 0;
 #pragma unroll
-    for (int i = 0; i < 4; ++i) s1[i] = s2[i] = x0[i] = 0.f;
+    for (int i = 0; i < kChunks; ++i) s1[i] = s2[i] = x0[i] = 0.f;
     // box-relative position of this lane's row (rows are in box order, dim 1 fastest)
     int ri[4];
     {
-      int r = (warp & 3) * 32 + lane;
+      int r = (cwarp & 3) * 32 + lane;
 #pragma unroll
       for (int d = 0; d < 3; ++d) {
         ri[d] = r % L.obox[d];
@@ -209,44 +231,81 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
     uint32_t nstore = 0;
     for (int item = first_item; item < n_items; item += item_stride) {
       const TmaTile t = tma_decode(L, item);
-      const int ty0 = L.sel_dim >= 0 ? t.idx[L.sel_dim] : 0;
+      const int ty0 = tma_first_type(L, t);
       const int ty1 = L.sel_dim >= 0 ? ty0 + 1 : L.n_types;
       // ---- MMA ----
+      // Stages (64-deep K chunks) in order cc, slab type, shift.  Stage s + 1 is issued into the other fresh block
+      // before stage s is waited for, added into acc and its A-slab / weight slots released, so one stage is always in
+      // flight while a warpgroup folds, releases and waits on the next barrier.
 #pragma unroll
-      for (int i = 0; i < 16 * kTmaAccChunks; ++i) acc[i] = 0.f;
-      for (int cc = 0; cc < L.nc; ++cc) {
-        for (int ty = ty0; ty < ty1; ++ty) {
-          const TmaSlabType& S = L.type[ty];
-          mbar_wait_spin(&a_full[aslot], aphase);
-          const uint32_t sa0 = a_base + aslot * (uint32_t)L.a_slot_bytes;
-          for (int j = 0; j < S.nshift; ++j) {
-            uint32_t sb;
-            if (L.b_resident) {
-              sb = b_base + (uint32_t)(S.tap[j] * L.nc + cc) * tile_bytes;
-            } else {
-              mbar_wait_spin(&b_full[bslot], bphase);
-              sb = b_base + bslot * tile_bytes;
-            }
-            const uint32_t sa = sa0 + (uint32_t)j * (uint32_t)L.shift_bytes + a_row_off;
-            const uint64_t a_hi = make_smem_desc(sa, 16, 1024);
-            const uint64_t b_hi = make_smem_desc(sb, 16, 1024);
-            if constexpr (kLo) {
-              const uint64_t a_lo = make_smem_desc(sa + (uint32_t)L.plane_stride, 16, 1024);
-              const uint64_t b_lo = make_smem_desc(sb + (uint32_t)L.BN * 128u, 16, 1024);
-              const uint64_t ad[3] = {a_hi, a_lo, a_hi}, bd[3] = {b_lo, b_hi, b_hi};   // small products first
-              wgmma_stage<kTmaAccChunks, 0, 0>(acc, ad, bd, 3, 2u, 2u, 512u, L.BN, bf16);
-            } else {
-              const uint64_t ad[3] = {a_hi, a_hi, a_hi}, bd[3] = {b_hi, b_hi, b_hi};
-              wgmma_stage<kTmaAccChunks, 0, 0>(acc, ad, bd, 1, 2u, 2u, 512u, L.BN, bf16);
-            }
-            __syncwarp();
-            if (!L.b_resident) {
-              if (lane == 0) mbar_arrive(&b_empty[bslot]);
-              if (++bslot == (uint32_t)L.b_slots) { bslot = 0; bphase ^= 1u; }
-            }
-          }
-          if (lane == 0) mbar_arrive(&a_empty[aslot]);   // the slab may be overwritten once every warp has read it
+      for (int i = 0; i < kBN / 2; ++i) acc[i] = 0.f;
+      int cc = 0, ty = ty0, j = 0;   // the next stage to issue
+      // Waits for the next stage's operands and issues it into t; rel_a / rel_b = the A and weight slots to release
+      // once it has completed (-1: none; an A slab is released after its last shift, resident weights never).
+      // Returns false after the tile's last stage.
+      auto issue = [&](float (&t)[kBN / 2], int& rel_a, int& rel_b) -> bool {
+        if (cc == L.nc) return false;
+        const TmaSlabType& S = L.type[ty];
+        if (j == 0) mbar_wait_spin(&a_full[aslot], aphase);
+        uint32_t sb;
+        if (L.b_resident) {
+          sb = b_base + (uint32_t)(S.tap[j] * L.nc + cc) * kBTileBytes;
+          rel_b = -1;
+        } else {
+          mbar_wait_spin(&b_full[bslot], bphase);
+          sb = b_base + bslot * kBTileBytes;
+          rel_b = (int)bslot;
+          if (++bslot == (uint32_t)L.b_slots) { bslot = 0; bphase ^= 1u; }
+        }
+        const uint32_t sa = a_base + aslot * (uint32_t)L.a_slot_bytes + (uint32_t)j * (uint32_t)L.shift_bytes + a_row_off;
+        const uint64_t a_hi = make_smem_desc(sa, 16, 1024);
+        const uint64_t b_hi = make_smem_desc(sb, 16, 1024);
+        if constexpr (kLo) {
+          const uint64_t a_lo = make_smem_desc(sa + (uint32_t)L.plane_stride, 16, 1024);
+          const uint64_t b_lo = make_smem_desc(sb + (uint32_t)kBN * 128u, 16, 1024);
+          const uint64_t ad[3] = {a_hi, a_lo, a_hi}, bd[3] = {b_lo, b_hi, b_hi};   // small products first
+          wgmma_stage_issue<kBN, kBf16, 3>(t, ad, bd, 2u, 2u);
+        } else {
+          const uint64_t ad[3] = {a_hi, a_hi, a_hi}, bd[3] = {b_hi, b_hi, b_hi};
+          wgmma_stage_issue<kBN, kBf16, 1>(t, ad, bd, 2u, 2u);
+        }
+        rel_a = -1;
+        if (++j == S.nshift) {
+          j = 0;
+          rel_a = (int)aslot;
           if (++aslot == (uint32_t)L.a_slots) { aslot = 0; aphase ^= 1u; }
+          if (++ty == ty1) { ty = ty0; ++cc; }
+        }
+        return true;
+      };
+      // Adds a completed stage into acc and releases its slots.
+      auto retire = [&](float (&t)[kBN / 2], int rel_a, int rel_b) {
+        acc_fence(t);
+#pragma unroll
+        for (int i = 0; i < kBN / 2; ++i) acc[i] += t[i];
+        // every consumer thread arrives: an arrival under `lane == 0` would be a thread-dependent branch inside the
+        // wgmma pipeline, which ptxas answers by serialising every wgmma of the kernel
+        if (rel_b >= 0) mbar_arrive(&b_empty[rel_b]);
+        if (rel_a >= 0) mbar_arrive(&a_empty[rel_a]);   // the slab may be overwritten once every thread has read it
+      };
+      float t0[kBN / 2], t1[kBN / 2];
+      int rel_a0, rel_b0, rel_a1, rel_b1;
+      if (issue(t0, rel_a0, rel_b0)) {
+        while (true) {
+          if (!issue(t1, rel_a1, rel_b1)) {
+            wgmma_wait<0>();
+            retire(t0, rel_a0, rel_b0);
+            break;
+          }
+          wgmma_wait<1>();
+          retire(t0, rel_a0, rel_b0);
+          if (!issue(t0, rel_a0, rel_b0)) {
+            wgmma_wait<0>();
+            retire(t1, rel_a1, rel_b1);
+            break;
+          }
+          wgmma_wait<1>();
+          retire(t1, rel_a1, rel_b1);
         }
       }
       // ---- epilogue ----
@@ -256,25 +315,25 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
       for (int d = 0; d < 4; ++d) {
         const int o = t.idx[d] * L.o_mul[d];
         valid = valid && (o + ri[d] < L.oext[d]);
-        oc[d] = o + L.sub[warp & 3][d];
+        oc[d] = o + L.sub[cwarp & 3][d];
       }
       const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
       if (epi && (P.wunscale != nullptr || P.out_scale != nullptr) && L.n_tiles_n > 1) {
         named_bar_sync(1, 128);   // previous tile's readers are done with the table
-        for (int i = threadIdx.x; i < L.BN; i += 128)
-          unscale_tab[i] = (P.wunscale != nullptr ? __ldg(P.wunscale + t.n_tile * L.BN + i) : 1.f) * oscale;
+        for (int i = ct; i < kBN; i += 128)
+          unscale_tab[i] = (P.wunscale != nullptr ? __ldg(P.wunscale + t.n_tile * kBN + i) : 1.f) * oscale;
         named_bar_sync(1, 128);
       }
 #pragma unroll
-      for (int kq = 0; kq < kTmaAccChunks; ++kq) {
+      for (int kq = 0; kq < kChunks; ++kq) {
         const int c0 = kq * 32;
-        const int col0 = t.n_tile * L.BN + c0;
-        if (c0 < L.BN && col0 < L.N && !(L.dbg & 4)) {
+        const int col0 = t.n_tile * kBN + c0;
+        if (col0 < L.N && !(L.dbg & 4)) {
           named_bar_sync(2, kTmaMmaWarps * 32);   // the previous chunk's readers are done with the transpose tile
-          acc_chunk_to_smem<kTmaAccChunks>(acc, kq, xtile, kXPitch, wg, tid_wg);
+          acc_chunk_to_smem<kChunks>(acc, kq, xtile, kXPitch, wg, tid_wg);
           named_bar_sync(2, kTmaMmaWarps * 32);
           if (!epi) continue;
-          const float* xrow = xtile + (warp * 32 + lane) * kXPitch;
+          const float* xrow = xtile + (cwarp * 32 + lane) * kXPitch;
           const uint32_t buf = my_stage + (L.stage_bufs == 2 ? (nstore & 1u) : 0u) * kStageBytes;
           if (leader) {
             // the bulk store that last read this buffer must have finished reading it
@@ -325,9 +384,9 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
       nrows += __popc(vmask);
       if (want_stats && L.n_tiles_n > 1) {
 #pragma unroll
-        for (int kq = 0; kq < kTmaAccChunks; ++kq) {
-          const int col = t.n_tile * L.BN + kq * 32 + lane;
-          if (kq * 32 < L.BN && col < L.N) {
+        for (int kq = 0; kq < kChunks; ++kq) {
+          const int col = t.n_tile * kBN + kq * 32 + lane;
+          if (col < L.N) {
             const double n = (double)nrows, xd = (double)x0[kq];
             atomicAdd(&P.stats_sum[col], (double)s1[kq] + n * xd);
             atomicAdd(&P.stats_sq[col], (double)s2[kq] + xd * (2.0 * (double)s1[kq] + n * xd));
@@ -347,13 +406,13 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
         double* tab = reinterpret_cast<double*>(smem + L.off_stage);   // [4 warps][2][128] = 8 KB of the staging blocks
         named_bar_sync(1, 128);
 #pragma unroll
-        for (int kq = 0; kq < kTmaAccChunks; ++kq) {
+        for (int kq = 0; kq < kChunks; ++kq) {
           const double n = (double)nrows, xd = (double)x0[kq];
-          tab[(warp * 2 + 0) * 128 + kq * 32 + lane] = (double)s1[kq] + n * xd;
-          tab[(warp * 2 + 1) * 128 + kq * 32 + lane] = (double)s2[kq] + xd * (2.0 * (double)s1[kq] + n * xd);
+          tab[(cwarp * 2 + 0) * 128 + kq * 32 + lane] = (double)s1[kq] + n * xd;
+          tab[(cwarp * 2 + 1) * 128 + kq * 32 + lane] = (double)s2[kq] + xd * (2.0 * (double)s1[kq] + n * xd);
         }
         named_bar_sync(1, 128);
-        for (int c = threadIdx.x; c < L.N; c += 128) {
+        for (int c = ct; c < L.N; c += 128) {
           double a = 0.0, b = 0.0;
 #pragma unroll
           for (int w = 0; w < 4; ++w) {
@@ -431,7 +490,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
   const bool window = g.kt == 1 && g.kw > 1 && S.C * g.kw == 64 && S.ld == S.C && S.coff == 0 && g.pw == 0 &&
                       !g.transposed && g.st == 1 && S.W >= P.Wd + g.kw - 1 && S.H == P.Hd && S.T == P.Td;
   if (S.C % 8 != 0 || (taps > 1 && S.C % 64 != 0 && !window)) return false;
-  if (P.BN % 32 != 0 || P.BN > 32 * kTmaAccChunks || P.n_tiles < 1) return false;
+  if (P.BN % 32 != 0 || P.BN < 32 || P.BN > kTmaMaxBN || P.n_tiles < 1) return false;
   if (P.Kreal != g.kt * g.kh * g.kw * S.C) return false;
   if (g.sh != 1 || g.sw != 1) return false;
   const int planes = P.npass > 1 ? 2 : 1;
@@ -768,6 +827,29 @@ extern "C" int coclr_conv_tma_plan(const coclr_conv_t* p, int* info) {
   return 1;
 }
 
+template <int kNPass, int kBN, bool kBf16>
+static int conv_tma_launch_bn(int grid, const CUtensorMap& m_hi, const CUtensorMap& m_lo, const CUtensorMap& m_out,
+                              const TmaArgs& args, cudaStream_t stream) {
+  const cudaError_t e = cudaFuncSetAttribute(conv_tma_kernel<kNPass, kBN, kBf16>,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)args.plan.total);
+  if (e != cudaSuccess) return COCLR_E_LAUNCH;
+  conv_tma_kernel<kNPass, kBN, kBf16><<<grid, kTmaThreads, args.plan.total, stream>>>(m_hi, m_lo, m_out, args);
+  return COCLR_OK;
+}
+
+// One kernel instance per (pass count, tile width, 16-bit format): the wgmma shape and type are compile-time constants.
+template <int kNPass, bool kBf16>
+static int conv_tma_launch(int BN, int grid, const CUtensorMap& m_hi, const CUtensorMap& m_lo, const CUtensorMap& m_out,
+                           const TmaArgs& args, cudaStream_t stream) {
+  switch (BN) {
+    case 32: return conv_tma_launch_bn<kNPass, 32, kBf16>(grid, m_hi, m_lo, m_out, args, stream);
+    case 64: return conv_tma_launch_bn<kNPass, 64, kBf16>(grid, m_hi, m_lo, m_out, args, stream);
+    case 96: return conv_tma_launch_bn<kNPass, 96, kBf16>(grid, m_hi, m_lo, m_out, args, stream);
+    case 128: return conv_tma_launch_bn<kNPass, 128, kBf16>(grid, m_hi, m_lo, m_out, args, stream);
+    default: return COCLR_E_ARG;
+  }
+}
+
 // Returns COCLR_OK when the launch was issued, 1 when this shape is not handled here (caller falls through to the
 // cp.async kernel), a negative COCLR_E_* on a launch error.
 int coclr::conv_tma_try(const coclr_conv_t& P, int num_sms, cudaStream_t stream) {
@@ -793,16 +875,12 @@ int coclr::conv_tma_try(const coclr_conv_t& P, int num_sms, cudaStream_t stream)
   args.a_bf16 = P.a_bf16;
   args.b_bf16 = P.b_bf16;
   const int grid = L.total_tiles < num_sms ? L.total_tiles : num_sms;
-  cudaError_t e;
-  if (P.npass > 1) {
-    e = cudaFuncSetAttribute(conv_tma_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total);
-    if (e != cudaSuccess) return COCLR_E_LAUNCH;
-    conv_tma_kernel<3><<<grid, kTmaThreads, L.total, stream>>>(m_hi, m_lo, m_out, args);
-  } else {
-    e = cudaFuncSetAttribute(conv_tma_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total);
-    if (e != cudaSuccess) return COCLR_E_LAUNCH;
-    conv_tma_kernel<1><<<grid, kTmaThreads, L.total, stream>>>(m_hi, m_lo, m_out, args);
-  }
-  if (e != cudaSuccess) return COCLR_E_LAUNCH;
+  const bool bf16 = P.a_bf16 != 0;
+  int rc;
+  if (P.npass > 1) rc = bf16 ? conv_tma_launch<3, true>(L.BN, grid, m_hi, m_lo, m_out, args, stream)
+                             : conv_tma_launch<3, false>(L.BN, grid, m_hi, m_lo, m_out, args, stream);
+  else rc = bf16 ? conv_tma_launch<1, true>(L.BN, grid, m_hi, m_lo, m_out, args, stream)
+                 : conv_tma_launch<1, false>(L.BN, grid, m_hi, m_lo, m_out, args, stream);
+  if (rc != COCLR_OK) return rc;
   return cudaGetLastError() == cudaSuccess ? COCLR_OK : COCLR_E_LAUNCH;
 }
