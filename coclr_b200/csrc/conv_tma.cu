@@ -27,8 +27,6 @@
 // Warp roles (384 threads, three warpgroups): 0 A loader, 1 weight loader, 2-3 idle (warpgroup 0 gives its registers to
 // the consumers), 4-11 MMA (warpgroups 1 and 2), 4-7 also the epilogue.
 #include <cuda.h>
-#include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
@@ -328,7 +326,7 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
       for (int kq = 0; kq < kChunks; ++kq) {
         const int c0 = kq * 32;
         const int col0 = t.n_tile * kBN + c0;
-        if (col0 < L.N && !(L.dbg & 4)) {
+        if (col0 < L.N) {
           named_bar_sync(2, kTmaMmaWarps * 32);   // the previous chunk's readers are done with the transpose tile
           acc_chunk_to_smem<kChunks>(acc, kq, xtile, kXPitch, wg, tid_wg);
           named_bar_sync(2, kTmaMmaWarps * 32);
@@ -349,13 +347,13 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
           }
           fence_proxy_async_smem();
           __syncwarp();
-          if (leader && !(L.dbg & 1)) {
+          if (leader) {
             if (P.accumulate) tma_reduce_add_5d(&map_out, buf, col0, oc[0], oc[1], oc[2], oc[3]);
             else tma_store_5d(&map_out, buf, col0, oc[0], oc[1], oc[2], oc[3]);
             bulk_commit_group();
           }
           ++nstore;
-          if (want_stats && !(L.dbg & 2)) {
+          if (want_stats) {
             // lane c sums column c over the warp's valid rows, reading the swizzled block back (conflict-free)
             if (vmask != 0u) {
               float a = 0.f, b = 0.f;
@@ -461,14 +459,9 @@ bool encode_map(CUtensorMap* m, const MapSpec& s, int which, int rank, bool swiz
   }
   for (int i = 0; i < 4; ++i) strides[i] = s.strides[i];
   const CUtensorMapDataType dt = s.elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16;
-  CUresult r = fn(m, dt, rank, s.base[which], dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    if (getenv("COCLR_TMA_DEBUG")) fprintf(stderr, "coclr: cuTensorMapEncodeTiled failed (%d)\n", (int)r);
-    return false;
-  }
-  return true;
+  return fn(m, dt, rank, s.base[which], dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 static int ceil_div(int a, int b) { return (a + b - 1) / b; }
@@ -497,7 +490,6 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
   const long ld2 = (long)S.ld * 2;
   L.BN = P.BN;
   L.N = P.N;
-  { const char* e = getenv("COCLR_TMA_DBG"); L.dbg = e ? atoi(e) : 0; }
   L.n_tiles_n = P.n_tiles;
   L.nc = window ? 1 : (S.C + 63) / 64;
   L.nkc = window ? g.kh : taps * L.nc;
@@ -722,9 +714,6 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
   L.b_tile_bytes = planes * L.BN * 128;
   const int budget = 227 * 1024 - 1024 /*alignment slack*/ - 1024 /*unscale table*/ - (int)kXTileBytes - 256 /*barriers*/;
   const int stage1 = 4 * (int)kStageBytes, stage2 = 8 * (int)kStageBytes;
-  int steps_per_tile = 0;
-  for (int ty = 0; ty < L.n_types; ++ty) steps_per_tile += L.type[ty].nshift;
-  steps_per_tile *= L.nc;
   const long tiles_per_cta = ((long)L.total_tiles + 131) / 132;   // one wave over the 132 SMs of an H100 SXM
   L.b_resident = 0;
   const long resident_bytes = (long)L.nkc * L.b_tile_bytes;
@@ -771,7 +760,6 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
     // the end-of-kernel statistics table (4 warps x 2 x 256 floats = 8 KB) lives in the staging area
     if (4 * (int)kStageBytes < 8192) return false;
   }
-  (void)steps_per_tile;
   return true;
 }
 
@@ -780,9 +768,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
 bool conv_tma_plan(const coclr_conv_t& P, TmaPlan& L, MapSpec& A, MapSpec& O) {
   bool have = false;
   long best = -1;
-  const char* fv = getenv("COCLR_TMA_VARIANT");      // tuning experiments: force one tile-shape variant
   for (int v = 0; v < 3; ++v) {
-    if (fv && atoi(fv) != v) continue;
     TmaPlan l;
     MapSpec a, o;
     if (!conv_tma_plan_variant(P, v, l, a, o)) continue;
@@ -801,17 +787,9 @@ bool conv_tma_plan(const coclr_conv_t& P, TmaPlan& L, MapSpec& A, MapSpec& O) {
 
 using namespace coclr;
 
-static int g_tma_enabled = -1;
+static bool g_tma_enabled = true;
 
-static bool tma_enabled() {
-  if (g_tma_enabled < 0) {
-    const char* e = getenv("COCLR_TMA");
-    g_tma_enabled = (e && e[0] == '0') ? 0 : 1;
-  }
-  return g_tma_enabled == 1;
-}
-
-extern "C" void coclr_set_conv_tma(int enabled) { g_tma_enabled = enabled ? 1 : 0; }
+extern "C" void coclr_set_conv_tma(int enabled) { g_tma_enabled = enabled != 0; }
 
 // Debug / test entry: the tile plan this launch shape would get (no GPU needed). Returns 1 when the TMA kernel
 // applies and fills info[] = {a_slots, b_slots, b_resident, stage_bufs, total smem, total tiles, slab bytes, n_types}.
@@ -853,7 +831,7 @@ static int conv_tma_launch(int BN, int grid, const CUtensorMap& m_hi, const CUte
 // Returns COCLR_OK when the launch was issued, 1 when this shape is not handled here (caller falls through to the
 // cp.async kernel), a negative COCLR_E_* on a launch error.
 int coclr::conv_tma_try(const coclr_conv_t& P, int num_sms, cudaStream_t stream) {
-  if (!tma_enabled()) return 1;
+  if (!g_tma_enabled) return 1;
   TmaArgs args;
   MapSpec A, O;
   if (!conv_tma_plan(P, args.plan, A, O)) return 1;

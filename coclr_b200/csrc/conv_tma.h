@@ -36,7 +36,6 @@ struct TmaPlan {
   int a_slots, a_slot_bytes;
   int b_slots, b_tile_bytes, b_resident;
   int stage_bufs;
-  int dbg;             // tuning experiments only (COCLR_TMA_DBG bit mask; 0 in production)
   int sub[4][4];       // output coordinate offsets of each epilogue warp's 32-row sub-box
   int BN, N;
   uint32_t off_b, off_stage, off_misc, off_bars, total;

@@ -2,8 +2,6 @@
 // global average pooling, input packing, L2-normalise, momentum (EMA) update, queue enqueue, Adam.
 // Activations are channels-last rows; channel counts are multiples of 8 for the 16-bit planes and every
 // kernel moves 8-16 bytes per thread with consecutive threads on consecutive addresses.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "coclr_b200.h"
 
@@ -1238,9 +1236,8 @@ extern "C" int coclr_maxpool_fwd(const coclr_pool_t* p, coclr_stream_t stream) {
   const coclr_geom_t& g = p->g;
   if (g.kt == 3 && g.kh == 3 && g.kw == 3 && g.st == 1 && g.sh == 1 && g.sw == 1 && g.pt == 1 && g.ph == 1 &&
       g.pw == 1 && (p->Wo % 4) == 0 && p->Wo == p->Wi && p->Ho == p->Hi && p->To == p->Ti) {
-    static const bool reg_form = getenv("COCLR_POOL333_REG") != nullptr;   // A/B timing: the register-only kernel
     const int threads = 2 * p->Wi * kPoolTY;
-    if (!reg_form && p->Wi >= 8 && threads <= 256 && p->C % 16 == 0 && p->x_coff % 8 == 0 && p->y_coff % 8 == 0 &&
+    if (p->Wi >= 8 && threads <= 256 && p->C % 16 == 0 && p->x_coff % 8 == 0 && p->y_coff % 8 == 0 &&
         p->ldx % 8 == 0 && p->ldy % 8 == 0) {
       const size_t smem = (size_t)3 * (kPoolTY + 2) * (p->Wi + 2) * 64;
       const int grid = p->B * ((p->Hi + kPoolTY - 1) / kPoolTY) * (p->C / 16);
@@ -1251,7 +1248,7 @@ extern "C" int coclr_maxpool_fwd(const coclr_pool_t* p, coclr_stream_t stream) {
     return LAUNCH_OK();
   }
   if (g.kt == 1 && g.kh == 3 && g.kw == 3 && g.st == 1 && g.sh == 2 && g.sw == 2 && g.pt == 0 && g.ph == 1 && g.pw == 1 &&
-      getenv("COCLR_POOL133_REG") == nullptr && p->To == p->Ti && 2 * p->Ho == p->Hi && 2 * p->Wo == p->Wi &&
+      p->To == p->Ti && 2 * p->Ho == p->Hi && 2 * p->Wo == p->Wi &&
       2 * p->Wo * kPool133TY <= 256 && p->C % 16 == 0 && p->x_coff % 8 == 0 && p->y_coff % 8 == 0 && p->ldx % 8 == 0 &&
       p->ldy % 8 == 0) {
     const size_t smem = (size_t)(2 * kPool133TY + 1) * (p->Wi + 1) * 64;

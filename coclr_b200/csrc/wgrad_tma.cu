@@ -1,7 +1,8 @@
 // TMA-staged weight gradient on wgmma tensor cores (sm_90a): the cuDNN wgrad reached through loss.backward()
 // (reference main_nce.py:330) for the stride-1 (1,k,k) / (k,1,1) / 1x1x1 convolutions of the backbones
 // (backbone/s3dg.py:11-13,39-42; backbone/resnet_2d3d.py).  Same C ABI as the gather kernel in conv_igemm.cu
-// (coclr_conv_wgrad dispatches here first; strided convs and the space-to-depth stem stay on the gather kernel).
+// (coclr_conv_wgrad dispatches here first when the call brings a large enough workspace; spatially strided convs
+// and calls without a workspace stay on the gather kernel).
 //
 //   dW[cout, tap, cin] += sum over pixels  dY[px, cout] * X[px + tap, cin]
 //
@@ -20,13 +21,11 @@
 //    row contributes nothing);
 //  * split precision (3 passes over fp16 hi / lo planes) as everywhere; Cout <= 64: hi and lo dY planes are the two
 //    64-row halves of the M = 128 tile (2 products per K step instead of 3, lo x lo included);
-//  * the pixel range is split over CTAs; every CTA ends with its [cout, columns] register accumulator going to a
-//    workspace (summed by one reduction launch) or, without one, with fp32 atomics into dW.
+//  * the pixel range is split over CTAs; every CTA ends with plain stores of its [cout, columns] register
+//    accumulator into the workspace, and one reduction launch sums the splits into dW (no atomics).
 //
 // Warp roles (288 threads): 0-7 two MMA warpgroups (64-cout block wg of the item each) + epilogue, 8 loader.
 #include <cuda.h>
-#include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
@@ -76,7 +75,7 @@ struct WgArgs {
   WgPlan plan;
   float* dw;
   const float* out_scale;
-  float* ws;            // partial accumulators [item][column][row] (see the epilogue), or nullptr: fp32 atomics into dw
+  float* ws;            // partial accumulators [item][column][row] (see the epilogue)
   int dy_bf16, src_bf16;
 };
 
@@ -226,9 +225,7 @@ wgrad_tma_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid_con
       if (++stage == (uint32_t)L.stages) { stage = 0; phase ^= 1u; }
     }
     // ===================== epilogue =====================
-    // with a workspace: the accumulator goes to ws[item][column][row] with plain stores and wgrad_reduce_kernel sums the
-    // pixel splits into dW; without one: fp32 atomics straight into dW[cout, cin, tap]
-    const float os = P.out_scale != nullptr ? __ldg(P.out_scale) : 1.f;
+    // the accumulator goes to ws[item][column][row] with plain stores; wgrad_reduce_kernel sums the pixel splits into dW
     const int R = 128;
     const int row0 = 64 * wg + 16 * (tw >> 5) + ((tw & 31) >> 2);
     const int col0 = 2 * (tw & 3);
@@ -239,22 +236,7 @@ wgrad_tma_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid_con
       for (int r = 0; r < 16; ++r) {
         const int row = row0 + 8 * ((r >> 1) & 1);      // row of the item's M = 128 tile
         const int col = c * 32 + col0 + 8 * (r >> 2) + (r & 1);
-        const float v = acc[16 * c + r];
-        if (P.ws != nullptr) {
-          P.ws[((size_t)blockIdx.x * L.N + col) * R + row] = v;
-        } else if (ntile > 0) {
-          int n;
-          if (L.stacked) {
-            n = row & 63;
-          } else {
-            n = (mg * L.mb) * 64 + row;
-            if ((row >> 6) >= L.mb) n = L.Cout;          // the second warpgroup of an odd last block has no rows
-          }
-          if (n < L.Cout) {
-            const WgCol k = wg_col(L, T, cg, col);
-            if (k.c < L.Cin_real) atomicAdd(P.dw + ((size_t)n * L.Cin_real + k.c) * L.taps + k.tap, v * os);
-          }
-        }
+        P.ws[((size_t)blockIdx.x * L.N + col) * R + row] = acc[16 * c + r];
       }
     }
   }
@@ -306,8 +288,7 @@ static long wg_ws_floats(const WgPlan& L) {
   return (long)L.n_types * L.n_cgroups * L.m_groups * L.splits * L.N * 128 * L.m_tiles;
 }
 
-// with_ws: plan for the workspace epilogue (one wave of CTAs, no atomics); otherwise for the atomic epilogue
-static bool wgrad_tma_plan(const coclr_wgrad_t& P, bool with_ws, WgPlan& L, MapSpec& DY, MapSpec& X) {
+static bool wgrad_tma_plan(const coclr_wgrad_t& P, WgPlan& L, MapSpec& DY, MapSpec& X) {
   const coclr_geom_t& g = P.g;
   const coclr_src_t& S = P.src;
   const coclr_src_t& D = P.dy;
@@ -491,7 +472,7 @@ static bool wgrad_tma_plan(const coclr_wgrad_t& P, bool with_ws, WgPlan& L, MapS
   L.total_tiles = L.ntiles[0] * L.ntiles[1] * L.ntiles[2] * L.ntiles[3];
   // ---- cout blocks per item: one per MMA warpgroup, as many as shared memory (>= 2 stages) allows ----
   const int cout_blocks = wg_ceil_div(P.Cout, 64);
-  L.stacked = (P.npass > 1 && P.Cout <= 64 && getenv("COCLR_WGRAD_NOSTACK") == nullptr) ? 1 : 0;
+  L.stacked = (P.npass > 1 && P.Cout <= 64) ? 1 : 0;
   const uint32_t x_bytes = (uint32_t)L.planes * L.nload * L.slab_bytes;
   const uint32_t budget = 227u * 1024u - 2048u;
   int mb = cout_blocks < 2 ? cout_blocks : 2;
@@ -515,39 +496,25 @@ static bool wgrad_tma_plan(const coclr_wgrad_t& P, bool with_ws, WgPlan& L, MapS
   L.stages = st > kWgMaxStages ? kWgMaxStages : st;
   L.off_bars = (uint32_t)L.stages * L.stage_bytes;
   L.total = L.off_bars + 256u + 1024u;
-  // ---- pixel splits: one wave of CTAs.  Atomic epilogue: every CTA ends with Cout x N fp32 atomics, measured to
-  // dominate once a CTA has fewer than ~16 tiles (and with more than ~74 splits on the same dW); workspace epilogue:
-  // plain stores, 4 tiles per CTA are enough to amortise the prologue ----
+  // ---- pixel splits: one wave of CTAs; 4 tiles per CTA are enough to amortise the prologue ----
   const int items = L.n_types * L.n_cgroups * L.m_groups;
   int splits = wg_num_sms() / items;
-  if (!with_ws && splits > wg_num_sms() / 2) splits = wg_num_sms() / 2;   // CTAs adding to the same dW elements
-  const int min_tiles = with_ws ? 4 : 16;
-  const int max_splits = L.total_tiles / min_tiles > 0 ? L.total_tiles / min_tiles : 1;
+  const int max_splits = L.total_tiles / 4 > 0 ? L.total_tiles / 4 : 1;
   if (splits > max_splits) splits = max_splits;
   if (splits < 1) splits = 1;
-  { const char* e = getenv("COCLR_WGRAD_SPLITS"); if (e && atoi(e) > 0) splits = atoi(e); }
   L.tiles_per_split = wg_ceil_div(L.total_tiles, splits);
   L.splits = wg_ceil_div(L.total_tiles, L.tiles_per_split);
   return true;
 }
 
-static int g_wgrad_tma = -1;
+static bool g_wgrad_tma = true;
 
 int wgrad_tma_try(const coclr_wgrad_t& P, cudaStream_t stream) {
-  if (g_wgrad_tma < 0) {
-    const char* e = getenv("COCLR_WGRAD_TMA");
-    g_wgrad_tma = (e && e[0] == '0') ? 0 : 1;
-  }
-  if (!g_wgrad_tma) return 1;
+  if (!g_wgrad_tma || P.ws == nullptr || ((uintptr_t)P.ws & 15)) return 1;
   WgArgs args;
   MapSpec DY, X;
-  bool with_ws = P.ws != nullptr;
-  if (!wgrad_tma_plan(P, with_ws, args.plan, DY, X)) return 1;
-  if (with_ws && (wg_ws_floats(args.plan) > P.ws_floats || ((uintptr_t)P.ws & 15))) {
-    with_ws = false;                                   // workspace too small: atomic epilogue
-    if (!wgrad_tma_plan(P, false, args.plan, DY, X)) return 1;
-  }
-  args.ws = with_ws ? P.ws : nullptr;
+  if (!wgrad_tma_plan(P, args.plan, DY, X) || wg_ws_floats(args.plan) > P.ws_floats) return 1;
+  args.ws = P.ws;
   CUtensorMap m_dy_hi, m_dy_lo, m_x_hi, m_x_lo;
   if (!encode_map(&m_dy_hi, DY, 0) || !encode_map(&m_x_hi, X, 0)) return 1;
   if (P.npass > 1) {
@@ -561,34 +528,28 @@ int wgrad_tma_try(const coclr_wgrad_t& P, cudaStream_t stream) {
   args.out_scale = P.out_scale;
   args.dy_bf16 = P.dy_bf16;
   args.src_bf16 = P.src_bf16;
-  if (getenv("COCLR_TMA_DEBUG"))
-    fprintf(stderr, "coclr wgrad_tma: tiles %d box %dx%dx%dx%d types %d cgroups %d nload %d N %d mb %d m_groups %d "
-            "stacked %d stages %d stage_bytes %u splits %d\n", L.total_tiles, L.box[0], L.box[1], L.box[2],
-            L.box[3], L.n_types, L.n_cgroups, L.nload, L.N, L.mb, L.m_groups, L.stacked, L.stages, L.stage_bytes,
-            L.splits);
   cudaError_t e = cudaFuncSetAttribute(wgrad_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total);
   if (e != cudaSuccess) return COCLR_E_LAUNCH;
   const int grid = L.n_types * L.n_cgroups * L.m_groups * L.splits;
   wgrad_tma_kernel<<<grid, kWgThreads, L.total, stream>>>(m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, args);
-  if (args.ws != nullptr) {
-    const int rows = L.stacked ? 64 : L.mb * 64;
-    const dim3 rgrid((L.N * rows + 255) / 256, L.n_types * L.n_cgroups * L.m_groups);
-    wgrad_reduce_kernel<<<rgrid, 256, 0, stream>>>(args);
-  }
+  const int rows = L.stacked ? 64 : L.mb * 64;
+  const dim3 rgrid((L.N * rows + 255) / 256, L.n_types * L.n_cgroups * L.m_groups);
+  wgrad_reduce_kernel<<<rgrid, 256, 0, stream>>>(args);
   return cudaGetLastError() == cudaSuccess ? COCLR_OK : COCLR_E_LAUNCH;
 }
 
 }  // namespace coclr
 
-extern "C" void coclr_set_wgrad_tma(int enabled) { coclr::g_wgrad_tma = enabled ? 1 : 0; }
+extern "C" void coclr_set_wgrad_tma(int enabled) { coclr::g_wgrad_tma = enabled != 0; }
 
-// 1 when coclr_conv_wgrad would run this shape on the TMA-staged kernel; info[8] = {tile pixels dim 0, dim 1, dim 2,
-// columns per MMA, cout blocks per item, pipeline stages, pixel splits, work items}
+// 1 when the TMA-staged kernel's planner accepts this shape (coclr_conv_wgrad then runs it there, given a workspace of
+// coclr_wgrad_ws_floats floats); info[8] = {tile pixels dim 0, dim 1, dim 2, columns per MMA, cout blocks per item,
+// pipeline stages, pixel splits, work items}
 extern "C" int coclr_wgrad_tma_plan(const coclr_wgrad_t* p, int* info) {
   if (!p) return 0;
   coclr::WgPlan L;
   coclr::MapSpec DY, X;
-  if (!coclr::wgrad_tma_plan(*p, p->ws != nullptr, L, DY, X)) return 0;
+  if (!coclr::wgrad_tma_plan(*p, L, DY, X)) return 0;
   if (info) {
     info[0] = L.box[0]; info[1] = L.box[1]; info[2] = L.box[2]; info[3] = L.N; info[4] = L.mb; info[5] = L.stages;
     info[6] = L.splits; info[7] = L.n_types * L.n_cgroups * L.m_groups * L.splits;
@@ -596,12 +557,11 @@ extern "C" int coclr_wgrad_tma_plan(const coclr_wgrad_t* p, int* info) {
   return 1;
 }
 
-// workspace (in floats) with which coclr_conv_wgrad replaces the fp32 atomics of this shape by plain stores + one
-// reduction launch; 0 when the shape does not run on the TMA-staged kernel
+// workspace (in floats) this shape needs to run on the TMA-staged kernel; 0 when the shape does not run there
 extern "C" long coclr_wgrad_ws_floats(const coclr_wgrad_t* p) {
   if (!p) return 0;
   coclr::WgPlan L;
   coclr::MapSpec DY, X;
-  if (!coclr::wgrad_tma_plan(*p, true, L, DY, X)) return 0;
+  if (!coclr::wgrad_tma_plan(*p, L, DY, X)) return 0;
   return coclr::wg_ws_floats(L);
 }

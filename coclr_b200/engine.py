@@ -12,7 +12,6 @@ gradient buffer).  Parameters live in ONE flat fp32 buffer per encoder (nn.Param
 EMA / Adam / all-reduce are single launches over it.
 """
 import ctypes as C
-import os
 
 import torch
 
@@ -24,10 +23,11 @@ BN_EPS = 1e-5
 BN_MOMENTUM = 0.1
 S2D_PAD = 2   # zero pixels kept on either side of every row of the space-to-depth input planes (= the 4x4 stem's padding)
 
-# name -> (fwd_npass, fwd_bf16, bwd_npass): forward planes fp16 (hi/lo) or bf16; gradients are always bf16 planes
+# name -> (fwd_npass, fwd_bf16, bwd_npass): forward planes fp16 (hi/lo) or bf16; the backbone's gradient planes take the
+# forward planes' format (fp16: hi/lo of dY * 2^k, see Plan), the head's gradient planes are bf16
 PRECISIONS = {
-    "parity": (3, 0, 3),   # fp16 hi/lo split forward (fp32-grade), bf16 hi/lo split backward
-    "mixed": (3, 0, 1),    # fp32-grade forward (same logits/loss/queue as parity), single-pass bf16 backward
+    "parity": (3, 0, 3),   # fp16 hi/lo split forward (fp32-grade), hi/lo split backward
+    "mixed": (3, 0, 1),    # fp32-grade forward (same logits/loss/queue as parity), single-pass backward
     "fast": (1, 1, 1),     # single-pass bf16 everywhere (does NOT meet the 1e-3 parity bar)
 }
 
@@ -92,13 +92,8 @@ class _LaneList(list):
 class Graph:
     """Shape-independent description of the encoder: tensors, convs, pools in forward order."""
 
-    # the 1x1x1 convs that open branches 1 and 2 of a SepInception read the same input: run them as ONE conv
-    # (N = o1a + o2a instead of e.g. 96 and 16 output channels) into one buffer that the two branches slice
-    fuse_b12_default = os.environ.get("COCLR_FUSE_B12", "1") != "0"
-
     def __init__(self, stages, first_channel=3, head_dim=None, feature_size=S3D_FEATURE_SIZE, bb_prefix="",
-                 stem_s2d=True, fuse_b12=None):
-        self.fuse_b12 = Graph.fuse_b12_default if fuse_b12 is None else bool(fuse_b12)
+                 stem_s2d=True):
         self.tensors, self.items = [], _LaneList(self)   # items: ("conv", ConvSpec) | ("pool", PoolSpec) | ("bn", TensorSpec)
         self.item_lane, self.item_flag = [], []   # per item: stream lane (Inception branches run concurrently) and FORK/JOIN
         self.cur_lane, self.next_flag = 0, 0
@@ -218,49 +213,28 @@ class Graph:
             cat.gates = [(name + ".gating_b0", 0, o0), (name + ".gating_b1", o0, o1b),
                          (name + ".gating_b2", o0 + o1b, o2b), (name + ".gating_b3", o0 + o1b + o2b, o3b)]
         one = ((1, 1, 1), (1, 1, 1), (0, 0, 0))
-        if self.fuse_b12:
-            t12 = self._tensor(name + ".b12a", o1a + o2a, self._same(x))
-            self.cur_lane, self.next_flag = 1, FORK     # lane 1: fused 1x1 conv + its BN, then branch 1
-            cv = self._conv(name + ".branch1.0.conv", x, t12, 0, cin, o1a + o2a, *one)
-            cv.weight_names, cv.couts = [name + ".branch1.0.conv", name + ".branch2.0.conv"], [o1a, o2a]
-            t12.bn_members += [(name + ".branch1.0.bn", 0, o1a), (name + ".branch2.0.bn", o1a, o2a)]
-            self.items.append(("bn", t12))
-            self.cur_lane, self.next_flag = 2, AFTER1   # lane 2: branch 2 starts once the shared buffer is ready
-            self._st(name + ".branch2.1", t12, cat, o0 + o1b, o2a, o2b, 3, 1, 1, 1, src_coff=o1a)
-            self.cur_lane = 1
-            self._st(name + ".branch1.1", t12, cat, o0, o1a, o1b, 3, 1, 1, 1, src_coff=0)
-            self.cur_lane = 0
-            self._conv(name + ".branch0.0.conv", x, cat, 0, cin, o0, *one)
-            cat.bn_members.append((name + ".branch0.0.bn", 0, o0))
-            self.cur_lane = 3
-            tp = self._pool(name + ".branch3.0", x, (3, 3, 3), (1, 1, 1), (1, 1, 1))
-            self._conv(name + ".branch3.1.conv", tp, cat, o0 + o1b + o2b, cin, o3b, *one)
-            cat.bn_members.append((name + ".branch3.1.bn", o0 + o1b + o2b, o3b))
-            # the branches were issued out of channel order; the per-tensor BatchNorm needs its members' parameters laid
-            # out in channel order (one gamma / beta vector for the whole concat buffer)
-            cat.bn_members.sort(key=lambda m: m[1])
-            self.cur_lane, self.next_flag = 0, JOIN
-            self.items.append(("bn", cat))
-            return cat
-        self.cur_lane, self.next_flag = 0, FORK     # the four branches only share the (read-only) input planes
+        # the 1x1x1 convs that open branches 1 and 2 read the same input: they run as ONE conv (N = o1a + o2a instead
+        # of e.g. 96 and 16 output channels) into one buffer that the two branches slice
+        t12 = self._tensor(name + ".b12a", o1a + o2a, self._same(x))
+        self.cur_lane, self.next_flag = 1, FORK     # lane 1: fused 1x1 conv + its BN, then branch 1
+        cv = self._conv(name + ".branch1.0.conv", x, t12, 0, cin, o1a + o2a, *one)
+        cv.weight_names, cv.couts = [name + ".branch1.0.conv", name + ".branch2.0.conv"], [o1a, o2a]
+        t12.bn_members += [(name + ".branch1.0.bn", 0, o1a), (name + ".branch2.0.bn", o1a, o2a)]
+        self.items.append(("bn", t12))
+        self.cur_lane, self.next_flag = 2, AFTER1   # lane 2: branch 2 starts once the shared buffer is ready
+        self._st(name + ".branch2.1", t12, cat, o0 + o1b, o2a, o2b, 3, 1, 1, 1, src_coff=o1a)
+        self.cur_lane = 1
+        self._st(name + ".branch1.1", t12, cat, o0, o1a, o1b, 3, 1, 1, 1, src_coff=0)
+        self.cur_lane = 0
         self._conv(name + ".branch0.0.conv", x, cat, 0, cin, o0, *one)
         cat.bn_members.append((name + ".branch0.0.bn", 0, o0))
-        self.cur_lane = 1
-        t1 = self._tensor(name + ".b1a", o1a, self._same(x))
-        self._conv(name + ".branch1.0.conv", x, t1, 0, cin, o1a, *one)
-        t1.bn_members.append((name + ".branch1.0.bn", 0, o1a))
-        self.items.append(("bn", t1))
-        self._st(name + ".branch1.1", t1, cat, o0, o1a, o1b, 3, 1, 1, 1)
-        self.cur_lane = 2
-        t2 = self._tensor(name + ".b2a", o2a, self._same(x))
-        self._conv(name + ".branch2.0.conv", x, t2, 0, cin, o2a, *one)
-        t2.bn_members.append((name + ".branch2.0.bn", 0, o2a))
-        self.items.append(("bn", t2))
-        self._st(name + ".branch2.1", t2, cat, o0 + o1b, o2a, o2b, 3, 1, 1, 1)
         self.cur_lane = 3
         tp = self._pool(name + ".branch3.0", x, (3, 3, 3), (1, 1, 1), (1, 1, 1))
         self._conv(name + ".branch3.1.conv", tp, cat, o0 + o1b + o2b, cin, o3b, *one)
         cat.bn_members.append((name + ".branch3.1.bn", o0 + o1b + o2b, o3b))
+        # the branches were issued out of channel order; the per-tensor BatchNorm needs its members' parameters laid
+        # out in channel order (one gamma / beta vector for the whole concat buffer)
+        cat.bn_members.sort(key=lambda m: m[1])
         self.cur_lane, self.next_flag = 0, JOIN
         self.items.append(("bn", cat))
         return cat
@@ -409,7 +383,7 @@ class ParamStore:
 # shape-specific plan
 # ---------------------------------------------------------------------------------------------
 class _Act:
-    __slots__ = ("spec", "dims", "data", "pl", "plw", "grad", "dy", "scale", "shift", "mean", "rstd", "ssum", "ssq", "idx",
+    __slots__ = ("spec", "dims", "data", "pl", "grad", "dy", "scale", "shift", "mean", "rstd", "ssum", "ssq", "idx",
                  "bsums", "grad_written", "M", "dy_scale", "bamax", "gmean", "gate", "dgate", "dmean")
 
 
@@ -446,8 +420,8 @@ class Plan:
             padded = g.stem_s2d and t is g.input
             if padded:
                 shape = (B,) + a.dims[:2] + (a.dims[2] + 2 * S2D_PAD, t.C)
-            a.pl = ops.Planes(shape, fbf, dev, lo=fnp > 1, zero=padded)   # what every forward consumer reads
-            a.plw = a.pl if with_backward else None     # ... and the weight-gradient GEMM (same 16-bit format as dY)
+            # what every forward consumer reads, and the weight-gradient GEMM (same 16-bit format as dY)
+            a.pl = ops.Planes(shape, fbf, dev, lo=fnp > 1, zero=padded)
             a.data = a.grad = a.dy = a.idx = a.bsums = a.dy_scale = a.bamax = None
             a.gmean = a.gate = a.dgate = a.dmean = None
             a.grad_written = False
@@ -521,9 +495,8 @@ class Plan:
                 geom = ops.Geometry(it.k, it.s, it.p)
                 if with_backward:
                     da.idx = torch.empty(da.M * it.dst.C, dtype=torch.uint8, device=dev)
-                t_hi, t_lo = twin_ptrs(da.pl, da.plw)
                 pl = L.Pool(L.dptr(sa.pl.hi), L.dptr(sa.pl.lo), it.src.C, 0, L.dptr(da.pl.hi), L.dptr(da.pl.lo),
-                            it.dst.C, 0, t_hi, t_lo, L.dptr(da.idx), B, it.dst.C,
+                            it.dst.C, 0, None, None, L.dptr(da.idx), B, it.dst.C,
                             sa.dims[0], sa.dims[1], sa.dims[2], da.dims[0], da.dims[1], da.dims[2], geom.c(0),
                             None, None, 0)
                 self.keep.append(pl)
@@ -541,11 +514,10 @@ class Plan:
                                   L.dptr(a.mean), L.dptr(a.rstd), it.C)
                 # BatchNorm finalize is fused into the apply+split launch
                 res = acts[it.residual.index].pl if it.residual is not None else None
-                self.fwd.append(split_op(a.data, a.pl, a.M, it.C, None, None, it.relu, a.plw, bn=bf, res=res))
+                self.fwd.append(split_op(a.data, a.pl, a.M, it.C, None, None, it.relu, bn=bf, res=res))
                 if it.gates:
                     # S3D-G feature gating of the block output: the planes written above are scaled in place by
                     # sigmoid(fc(mean_thw)) per clip and channel (csrc/gating.cu)
-                    assert a.plw is None or a.plw is a.pl
                     Pn = a.dims[0] * a.dims[1] * a.dims[2]
                     a.gmean = torch.empty(B, it.C, dtype=torch.float32, device=dev)
                     a.gate = torch.empty(B, it.C, dtype=torch.float32, device=dev)
@@ -631,18 +603,10 @@ class Plan:
                 convs_into.setdefault(it.dst.index, []).append(it)
             elif kind == "pool":
                 pool_into[it.dst.index] = it
-        # reverse forward order: a tensor is handled at its BatchNorm / pool item, i.e. after every consumer.
-        # bwd_split: position in the list after which >= 75 % of the parameters have their final gradient -- the flat
-        # gradient is all-reduced in two parts, the first one while the rest of the backward pass still runs (the
-        # reference gets this overlap from DistributedDataParallel's bucketed reducer, main_nce.py:172)
-        total_params = sum(n for _, (o, n, _) in st.offsets.items())
-        done_params = sum(st.offsets[k][1] for k in ("2.weight", "2.bias", "4.weight", "4.bias") if k in st.offsets)
-        self.bwd_split, self.bwd_split_conv_off, self.bwd_split_bn_off = None, None, None
+        # reverse forward order: a tensor is handled at its BatchNorm / pool item, i.e. after every consumer
         for kind_r, it_r in reversed(g.items):
             if kind_r == "conv":
                 continue
-            if self.bwd_split is None and done_params >= 0.75 * total_params and len(bw) > 0:
-                self.bwd_split = len(bw)
             t = it_r if kind_r == "bn" else it_r.dst
             a = acts[t.index]
             if not a.grad_written:
@@ -680,21 +644,13 @@ class Plan:
                 oscale = None if gbf else a.dy_scale[1:]
                 self.keep.append(bb)
                 bw.append((lib.coclr_bn_bwd, (C.byref(bb), nsm)))
-                if self.bwd_split is None:
-                    done_params += 2 * t.C
-                    self.bwd_split_bn_off = goff            # gammas of this tensor: first BN parameter done so far
                 for it in convs_into[t.index]:
-                    if self.bwd_split is None:
-                        names = [n + ".weight" for n in it.weight_names]
-                        done_params += sum(st.offsets[n][1] for n in names)
-                        off0 = st.offsets[names[0]][0]
-                        self.bwd_split_conv_off = off0 if self.bwd_split_conv_off is None else min(self.bwd_split_conv_off, off0)
                     sa = acts[it.src.index]
                     geom = ops.Geometry(it.k_eff, it.s_eff, it.p_eff)
                     dy = a.dy.src(it.dst_coff, _round8(it.cout), a.dims[0], a.dims[1], a.dims[2])
                     kreal = geom.taps * it.src_C
                     splits = 1   # one fp32 add per dW element: reproducible
-                    wsrc = sa.plw.src(it.src_coff, it.src_C, sa.dims[0], sa.dims[1], src_w(sa))
+                    wsrc = src_of(sa, it)
                     if it.s2d:
                         # the weight gradient is produced in the space-to-depth layout, then scattered back
                         dw_eff = eng.s2d[it.name]["dw_eff"]
@@ -724,13 +680,11 @@ class Plan:
                             L.dptr(a.grad), L.dptr(sa.grad), int(grad_seen(sa)))
                 self.keep.append(pl)
                 bw.append((lib.coclr_maxpool_bwd, (C.byref(pl),)))
-        if any(t.gates for t in g.tensors):
-            self.bwd_split = None   # gating parameters sit behind the BatchNorm region: one all-reduce at the end
         # one workspace for the weight-gradient launches (they run one after the other on the side stream): per-CTA
         # partial sums are written with plain stores and reduced by a second launch instead of fp32 atomics into dW
         need = max([int(lib.coclr_wgrad_ws_floats(C.byref(w))) for w in self.wgrads] + [0])
         self.wg_ws = None
-        if need > 0 and EncoderEngine.wgrad_workspace:
+        if need > 0:
             self.wg_ws = torch.empty(need, dtype=torch.float32, device=dev)
             for w in self.wgrads:
                 w.ws, w.ws_floats = L.dptr(self.wg_ws).value, need
@@ -860,10 +814,6 @@ class EncoderEngine:
             self.plans[key] = p
         return p
 
-    overlap_wgrad = True  # run the weight-gradient GEMMs on a side stream, concurrently with the dgrad chain
-
-    overlap_branches = True  # run the four Inception branches of a block on four streams (forward)
-
     def _run_lanes(self, oplist, lanes):
         """Forward launch list with fork/join: ops tagged lane 1..3 run on side streams that wait for the fork
         point (an event on the main stream recorded before the block's first op); the JOIN op first waits for them."""
@@ -901,7 +851,7 @@ class EncoderEngine:
         main = torch.cuda.current_stream()
         stream = C.c_void_p(main.cuda_stream)
         prof = EncoderEngine.profile
-        use_side = side_fn is not None and prof is None and EncoderEngine.overlap_wgrad
+        use_side = side_fn is not None and prof is None
         if use_side:
             if getattr(self, "_side", None) is None:
                 self._side = torch.cuda.Stream()
@@ -948,20 +898,18 @@ class EncoderEngine:
             assert batch_index.dtype == torch.long and batch_index.is_cuda and batch_index.numel() == B
         p = self.plan(B, T, H, W, training, with_backward)
         lib = L.load()
-        tw = p.input.plw if (p.input.plw is not None and p.input.plw is not p.input.pl) else None
         peer_ptr, cpp = (C.c_void_p(int(peers[0])), int(peers[1])) if peers is not None else (None, 0)
         assert peers is None or batch_index is not None
         # the clip pointer / shuffle index change from call to call, so packing stays outside the captured graph
         if self.graph.stem_s2d:
             assert H % 2 == 0 and W % 2 == 0, "the space-to-depth stem needs even H, W"
             L.check(lib.coclr_pack_input_s2d(L.dptr(x), x.stride(0), x.stride(1), Cin, L.dptr(p.input.pl.hi),
-                                             L.dptr(p.input.pl.lo), L.dptr(tw.hi) if tw else None,
-                                             L.dptr(tw.lo) if tw else None, B, T, H, W, S2D_PAD, L.dptr(batch_index),
-                                             peer_ptr, cpp, nm, ns, L.stream_ptr()), "coclr_pack_input_s2d")
+                                             L.dptr(p.input.pl.lo), None, None, B, T, H, W, S2D_PAD,
+                                             L.dptr(batch_index), peer_ptr, cpp, nm, ns, L.stream_ptr()),
+                    "coclr_pack_input_s2d")
         else:
             L.check(lib.coclr_pack_input(L.dptr(x), x.stride(0), x.stride(1), Cin, L.dptr(p.input.pl.hi),
-                                         L.dptr(p.input.pl.lo), L.dptr(tw.hi) if tw else None,
-                                         L.dptr(tw.lo) if tw else None, B, T * H * W, L.dptr(batch_index),
+                                         L.dptr(p.input.pl.lo), None, None, B, T * H * W, L.dptr(batch_index),
                                          peer_ptr, cpp, nm, ns, L.stream_ptr()), "coclr_pack_input")
 
         def body():
@@ -970,15 +918,14 @@ class EncoderEngine:
             if training:
                 p.stats.zero_()
                 self.store.nbt += 1
-            if EncoderEngine.overlap_branches and EncoderEngine.profile is None:
+            if EncoderEngine.profile is None:
                 self._run_lanes(p.fwd, p.fwd_lane)
             else:
                 self._run(p.fwd)
         self._graphed(p, "fwd" + ("_repack" if repack else ""), body)
         return p
 
-    use_graphs = os.environ.get("COCLR_GRAPHS", "1") != "0"
-    wgrad_workspace = os.environ.get("COCLR_WGRAD_WS", "1") != "0"
+    use_graphs = True   # capture every launch list into a CUDA graph after its first eager run
 
     def _graphed(self, p, key, body):
         """Every launch of `body` has fixed pointers and shapes: after one eager run (which also performs the
@@ -1002,31 +949,11 @@ class EncoderEngine:
             state[0].replay()
             L.LAUNCHES += state[1]
 
-    def grad_ranges(self, p):
-        """[(lo, hi)] element ranges of the flat gradient that are final after the first backward segment, and the
-        complementary ranges (final at the end): conv weights, BatchNorm parameters and the head are three regions of
-        the flat buffer, each filled back to front by the backward pass."""
-        st = self.store
-        conv_end = min(o for k, (o, n, _) in st.offsets.items() if not k.endswith(".weight") or len(st.offsets[k][2]) == 1)
-        c0, b0 = p.bwd_split_conv_off, p.bwd_split_bn_off
-        first = [(c0, conv_end), (b0, st.numel)]
-        rest = [(0, c0), (conv_end, b0)]
-        return [r for r in first if r[1] > r[0]], [r for r in rest if r[1] > r[0]]
-
-    def backward(self, p, dq, mid_hook=None):
-        """dq: gradient w.r.t. the normalised features [B, dim]; accumulates into store.grad.  mid_hook (optional) is
-        called between the two segments of the launch list with the ranges of the flat gradient that are final."""
+    def backward(self, p, dq):
+        """dq: gradient w.r.t. the normalised features [B, dim]; accumulates into store.grad."""
         p.dq.copy_(dq)
         wg = L.load().coclr_conv_wgrad
-        if mid_hook is None or p.bwd_split is None or p.bwd_split_conv_off is None or p.bwd_split_bn_off is None:
-            self._graphed(p, "bwd", lambda: self._run(p.bwd, side_fn=wg))
-            return False
-        first, rest = self.grad_ranges(p)
-        self._graphed(p, "bwd0", lambda: self._run(p.bwd[:p.bwd_split], side_fn=wg))
-        mid_hook(first)
-        self._graphed(p, "bwd1", lambda: self._run(p.bwd[p.bwd_split:], side_fn=wg))
-        mid_hook(rest)
-        return True
+        self._graphed(p, "bwd", lambda: self._run(p.bwd, side_fn=wg))
 
     def backbone_output_ncdhw(self, p):
         return p.backbone_out.pl.value().permute(0, 4, 1, 2, 3).contiguous()

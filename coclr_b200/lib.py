@@ -123,11 +123,13 @@ KERNELS_PER_CALL = {"coclr_bn_bwd": 2, "coclr_l2norm_bwd": 2, "coclr_conv_packed
 
 def kernels_of(fn, args):
     """Kernels one call of `fn` launches (bench.py reports the per-step total).  A weight gradient on the TMA-staged
-    kernel with a workspace is two launches: partial sums, then the reduction over the pixel splits."""
+    kernel (a shape it takes, with a large enough workspace) is two launches: partial sums, then the reduction over
+    the pixel splits."""
     name = fn.__name__
     if name == "coclr_conv_wgrad" and args and hasattr(args[0], "_obj"):
         wg = args[0]._obj
-        if wg.ws and load().coclr_wgrad_tma_plan(args[0], None) == 1:
+        need = load().coclr_wgrad_ws_floats(args[0]) if wg.ws else 0
+        if need > 0 and wg.ws_floats >= need:
             return 2
     return KERNELS_PER_CALL.get(name, 1)
 

@@ -9,7 +9,6 @@
 """
 import ctypes as C
 import math
-import os
 
 import torch
 import torch.distributed as dist
@@ -19,9 +18,6 @@ from . import lib as L
 from .engine import Graph, ParamStore, EncoderEngine
 from .s3d_spec import S3D_FEATURE_SIZE
 
-
-# Split all-reduce started in the middle of backward (see _EncodeFn.backward); COCLR_OVERLAP_ALLREDUCE=1 enables it.
-OVERLAP_ALLREDUCE = os.environ.get("COCLR_OVERLAP_ALLREDUCE", "0") == "1"
 
 # Per-phase timeline of a step (bench.py --timeline): CUDA events on whatever stream the phase runs on; off by default.
 TIMELINE = None
@@ -94,21 +90,8 @@ class _EncodeFn(torch.autograd.Function):
             raise L.CoclrError("backward of an encoder pass whose saved activations were overwritten by a later forward "
                                "of the same shape (one outstanding training forward per encoder and input shape)")
         enc._prepare_grads()
-        st = enc._engine.store
-        world, _ = _world()
-        hook = None
-        if world > 1 and OVERLAP_ALLREDUCE:
-            if getattr(st, "pending_reduce", None):
-                raise L.CoclrError("a second backward before optimizer.step() with the overlapped gradient all-reduce "
-                                   "(gradient accumulation): set COCLR_OVERLAP_ALLREDUCE=0")
-            st.pending_reduce = []
-
-            def hook(ranges):      # async all-reduce on the process group's stream; FlatAdam.step() waits for them
-                for lo, hi in ranges:
-                    st.pending_reduce.append(dist.all_reduce(st.grad[lo:hi], async_op=True))
         mark("bwd:start")
-        if not enc._engine.backward(ctx.plan, dq.contiguous(), mid_hook=hook) and hook is not None:
-            st.pending_reduce = None      # un-split launch list: FlatAdam.step() reduces the whole buffer
+        enc._engine.backward(ctx.plan, dq.contiguous())
         mark("bwd:end")
         return None, None, None, None
 
@@ -291,26 +274,15 @@ class FlatAdam:
         return st
 
     def zero_grad(self, set_to_none=False):
-        st = self._state()
-        pending = getattr(st, "pending_reduce", None)
-        if pending:                        # a backward whose gradients are dropped without a step
-            for work in pending:
-                work.wait()
-            st.pending_reduce = None
-        st.grad.zero_()
+        self._state().grad.zero_()
 
     @torch.no_grad()
     def step(self):
         st = self._state()
         world, _ = _world()
-        pending = getattr(st, "pending_reduce", None)
         mark("opt:allreduce_wait")
-        if pending:
-            for work in pending:          # the ranges were all-reduced while the backward pass was still running
-                work.wait()
-        elif world > 1:
+        if world > 1:
             dist.all_reduce(st.grad)
-        st.pending_reduce = None
         mark("opt:allreduce_done")
         g = self.param_groups[0]
         self.step_count += 1

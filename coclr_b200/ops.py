@@ -105,9 +105,10 @@ def conv_igemm(src, a_bf16, geom_c, B, dst_dims, pw, dst, dst_coff=0, accumulate
 
 
 def conv_wgrad(src, src_bf16, geom_c, dy_src, dy_bf16, B, dst_dims, Cout, Cin_real, dw, npass=3, splits=1,
-               out_scale=None, workspace=None):
-    """workspace: optional fp32 tensor (see coclr_wgrad_ws_floats) -- partial sums by plain stores + one reduction
-    launch instead of fp32 atomics; True allocates one of the size the shape asks for."""
+               out_scale=None, workspace=True):
+    """workspace: fp32 tensor of at least coclr_wgrad_ws_floats floats, which the TMA-staged kernel needs (partial sums
+    by plain stores + one reduction launch); True allocates one of the size the shape asks for, None runs the call on
+    the gather kernel."""
     Td, Hd, Wd = dst_dims
     p = L.Wgrad(src, geom_c, dy_src, B, Td, Hd, Wd, Cout, Cin_real, L.dptr(dw), npass, int(dy_bf16), int(src_bf16),
                 splits, L.dptr(out_scale))

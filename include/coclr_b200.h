@@ -80,14 +80,15 @@ size_t coclr_conv_packed_bytes(int N, int Kreal, int* BN_out, int* n_tiles_out);
  * the taps of one dimension, resident or streamed weight tiles, bulk-tensor store / add-reduce epilogue) and everything
  * else on the cp.async gather kernel.  coclr_conv_tma_plan reports (without a GPU) whether a launch takes the TMA
  * kernel: returns 1 and fills info[8] = {A slots, B slots, weights resident, staging buffers, shared-memory bytes,
- * tiles, slab bytes per plane, slab types}, else 0.  coclr_set_conv_tma(0) forces the gather kernel (tests, A/B
- * timing; also COCLR_TMA=0 in the environment). */
+ * tiles, slab bytes per plane, slab types}, else 0.  coclr_set_conv_tma(0) forces the gather kernel (tests compare
+ * the two kernels with it). */
 int coclr_conv_tma_plan(const coclr_conv_t* p, int* info);
 void coclr_set_conv_tma(int enabled);
 
 /* ---- weight-gradient -----------------------------------------------------------------------
  * replaces cuDNN wgrad.  dW[n, c, tap] += sum_m dY[m, n] * A[m, (tap, c)] into the PyTorch weight
- * layout [Cout, Cin_real, kt, kh, kw] (fp32 atomics; zero dW first). */
+ * layout [Cout, Cin_real, kt, kh, kw] (zero dW first).  With a large enough workspace the TMA-staged kernel writes
+ * partial sums there and adds them to dW in one reduction launch; the gather kernel adds with fp32 atomics. */
 typedef struct {
   coclr_src_t src;   /* conv input planes (as the forward pass consumed them) */
   coclr_geom_t g;    /* forward geometry (transposed = 0) */
@@ -99,21 +100,22 @@ typedef struct {
   int dy_bf16, src_bf16;
   int splits;        /* pixel-range splits (>= 1) */
   const float* out_scale; /* device scalar multiplied into the result before it is added to dw, or NULL */
-  float* ws;         /* optional workspace (16-byte aligned) of ws_floats floats, see coclr_wgrad_ws_floats; NULL: none */
+  float* ws;         /* workspace (16-byte aligned) of ws_floats floats, see coclr_wgrad_ws_floats; NULL: gather kernel */
   long ws_floats;
 } coclr_wgrad_t;
 int coclr_conv_wgrad(const coclr_wgrad_t* p, coclr_stream_t stream);
 /* coclr_conv_wgrad runs stride-1 "same" (1,k,k) / (k,1,1) / 1x1x1 shapes on the TMA-staged kernel (csrc/wgrad_tma.cu:
- * dY tiles and X halo slabs by cp.async.bulk.tensor, the taps of the reuse dimension as the N blocks of one MMA) and
- * everything else (strided convs, the space-to-depth stem) on the cp.async gather kernel.  Tests / tuning can force the
- * gather kernel with coclr_set_wgrad_tma(0) or COCLR_WGRAD_TMA=0; `splits` only steers the gather kernel. */
+ * dY tiles and X halo slabs by cp.async.bulk.tensor, the taps of the reuse dimension as the N blocks of one MMA) when
+ * ws is 16-byte aligned and holds at least coclr_wgrad_ws_floats(p) floats.  Every other call (strided convs, no or a
+ * too small workspace) runs on the cp.async gather kernel.  coclr_set_wgrad_tma(0) forces the gather kernel (tests
+ * compare the two kernels with it); `splits` only steers the gather kernel. */
 void coclr_set_wgrad_tma(int enabled);
-/* 1 when the shape runs on the TMA-staged kernel; info[8] (may be NULL) = {tile extent dims 0..2, columns per MMA,
- * 64-cout blocks per work item, pipeline stages, pixel splits, work items} */
+/* 1 when the TMA-staged kernel's planner accepts the shape (whatever ws is); info[8] (may be NULL) = {tile extent
+ * dims 0..2, columns per MMA, 64-cout blocks per work item, pipeline stages, pixel splits, work items} */
 int coclr_wgrad_tma_plan(const coclr_wgrad_t* p, int* info);
-/* floats of workspace with which the TMA-staged kernel writes its per-CTA partial sums with plain stores and adds them
- * to dw in one reduction launch (no fp32 atomics: deterministic, and ~2x faster on the many small layers); 0 for shapes
- * on the gather kernel.  The workspace may be shared by launches on the same stream. */
+/* floats of workspace the TMA-staged kernel needs for this shape: it writes its per-CTA partial sums there with plain
+ * stores and adds them to dw in one reduction launch (no fp32 atomics: deterministic); 0 for shapes on the gather
+ * kernel.  The workspace may be shared by launches on the same stream. */
 long coclr_wgrad_ws_floats(const coclr_wgrad_t* p);
 
 /* ---- weight packing -------------------------------------------------------------------------

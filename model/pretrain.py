@@ -14,8 +14,6 @@ What changed under the surface (see DESIGN.md):
   * logits + temperature + cross-entropy by-products come from one kernel (:175-182);
   * queue_ptr is mirrored on the host, so there is no `int(self.queue_ptr)` device sync per step (:89).
 """
-import os
-
 import numpy as np
 import torch
 import torch.nn as nn
@@ -155,11 +153,11 @@ class InfoNCE(nn.Module):
         moco.mark("key:gathered")
         return k_global[rank * B:(rank + 1) * B], k_global
 
-    peer_shuffle = os.environ.get("COCLR_PEER_SHUFFLE", "1") != "0"
+    peer_shuffle = True   # exchange the key clips through peer memory where it can be set up
 
     def _peer_exchange(self, x2):
         """PeerClips for this clip shape, or None (-> all-gather path) when peer memory cannot be set up (no NVLink /
-        P2P between the ranks, non-NCCL backend) or is switched off with COCLR_PEER_SHUFFLE=0."""
+        P2P between the ranks, non-NCCL backend) or peer_shuffle is off."""
         if not InfoNCE.peer_shuffle or not x2.is_cuda or dist.get_backend() != "nccl":
             return None
         key = tuple(x2.shape)

@@ -47,9 +47,6 @@ def _worker(rank, world, port, out):
     loss = moco.nce_cross_entropy(logits, labels)
     opt.zero_grad()
     loss.backward()
-    # the flat gradient is all-reduced in two parts while backward is still running (moco._EncodeFn.backward): the
-    # asynchronous works are pending until the optimizer step waits for them
-    overlapped = len(getattr(model.encoder_q._engine.store, "pending_reduce", None) or [])
     opt.step()
     torch.cuda.synchronize()
     # ---- oracle: the same 2-rank world simulated on this GPU in float64 ----
@@ -75,7 +72,6 @@ def _worker(rank, world, port, out):
         errs.append(float((g_new.double() - sdd[k].grad).norm() / sdd[k].grad.norm().clamp_min(1e-30)))
     errs.sort()
     res["grad_median"], res["grad_max"] = errs[len(errs) // 2], errs[-1]
-    res["overlapped_allreduce_works"] = overlapped
     # replicas stay identical: compare flat parameters and Adam moments across ranks
     flat = st.flat.clone()
     other = flat.clone()
@@ -86,12 +82,6 @@ def _worker(rank, world, port, out):
     res["queue_identical"] = bool(torch.equal(qk, model.queue))
     torch.save(res, os.path.join(out, "rank%d.pt" % rank))
     dist.destroy_process_group()
-
-
-def moco_overlap():
-    sys.path.insert(0, ROOT)
-    from coclr_b200 import moco
-    return moco.OVERLAP_ALLREDUCE
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
@@ -106,5 +96,4 @@ def test_infonce_step_world2_nccl(tmp_path, diag):
         assert x["queue_err"] < 1e-3 and x["ptr"] == x["ptr_ref"] == PTR + 2 * B
         assert abs(x["loss"] - x["loss_ref"]) < 1e-3 * max(1.0, abs(x["loss_ref"]))
         assert x["replica_identical"] and x["queue_identical"]
-        assert x["overlapped_allreduce_works"] >= 2 or not moco_overlap(), x    # the overlapped path was the one tested
         assert x["grad_median"] < 0.15 and x["grad_max"] < 0.5, x

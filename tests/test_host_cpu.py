@@ -101,7 +101,6 @@ def test_s3dg_graph_and_plan_dry_run():
         for i, n in enumerate(bw):
             if n == "coclr_gate_bwd_reduce":
                 assert bw[i + 1:i + 7] == ["coclr_gate_fc_bwd"] * 4 + ["coclr_gate_bwd_apply", "coclr_bn_bwd"]
-        assert p.bwd_split is None       # the gating parameters are reduced with everything else at the end
         # every gating parameter's gradient is written by exactly one launch
         base = st.grad.data_ptr()
         offs = sorted((a[4].value - base) // 4 for fn, a in p.bwd if fn.__name__ == "coclr_gate_fc_bwd")
@@ -152,12 +151,27 @@ def test_oracle_not_imported_by_product():
     assert out.stdout.strip() == ""
 
 
+def test_library_reads_no_environment():
+    """The library's behaviour is set by its code and its callers, never by environment variables: no getenv in the
+    CUDA sources, no os.environ in the Python package (except the nvcc path of the build) or the model."""
+    csrc = os.path.join(ROOT, "coclr_b200", "csrc")
+    for f in sorted(os.listdir(csrc)):
+        assert "getenv" not in open(os.path.join(csrc, f)).read(), f
+    for d in ("coclr_b200", "model"):
+        for dirpath, _, files in os.walk(os.path.join(ROOT, d)):
+            for f in files:
+                path = os.path.join(dirpath, f)
+                if f.endswith(".py") and path != os.path.join(ROOT, "coclr_b200", "build.py"):
+                    assert "os.environ" not in open(path).read(), path
+
+
 def test_launch_plans_build_on_cpu_dry_run():
     """Structure of the forward/backward launch lists (built over CPU tensors, never run): every tensor gets
     a gradient, op counts match the architecture, first-writer/accumulate flags are consistent."""
     from coclr_b200 import lib as L
     from coclr_b200.engine import Graph, ParamStore, EncoderEngine
     from coclr_b200.s3d_spec import s3d_stages
+    from oracle import coclr_oracle as O
     L.DRY_RUN = True
     try:
         g = Graph(s3d_stages(3), 3, head_dim=128, bb_prefix="0.")
@@ -165,7 +179,7 @@ def test_launch_plans_build_on_cpu_dry_run():
         eng = EncoderEngine(st, g, "parity")
         p = eng.plan(2, 8, 64, 64, True, True)
         names = [fn.__name__ for fn, _ in p.fwd]
-        fused = 9 if g.fuse_b12 else 0    # per SepInception: branch1.0 + branch2.0 1x1 convs run as one conv, one BN pass
+        fused = 9    # per SepInception: branch1.0 + branch2.0 1x1 convs run as one conv, one BN pass
         assert names.count("coclr_conv_igemm") == 77 - fused + 2
         assert names.count("coclr_maxpool_fwd") == 13
         assert names.count("coclr_affine_split") == (77 - 9 * 3) - fused + 2   # one fused BN-finalize+apply+split per tensor (concat tensors hold 4 BNs) + 2 head splits
@@ -187,8 +201,9 @@ def test_launch_plans_build_on_cpu_dry_run():
                 assert offs == sorted(offs) and offs[-1] - offs[0] == sum(m[2] for m in t.bn_members[:-1]), t.name
         sliced = [it for kind, it in g.items if kind == "conv" and it.src_C != it.src.C and it.src is not g.input]
         assert len(sliced) == 2 * fused and all(it.src_coff % 8 == 0 and it.src_C % 8 == 0 for it in sliced)
-        g0 = Graph(s3d_stages(3), 3, head_dim=128, bb_prefix="0.", fuse_b12=False)
-        assert [n for n, _ in g0.param_layout()] != [] and sorted(n for n, _ in g0.param_layout()) == sorted(n for n, _ in g.param_layout())
+        want = {k[len("encoder_q."):]: tuple(v) for k, v in O.infonce_shapes(128, 128).items()
+                if k.startswith("encoder_q.") and (k.endswith(".weight") or k.endswith(".bias"))}
+        assert {k: tuple(v[2]) for k, v in st.offsets.items()} == want
         # inference plan has no gradient buffers
         p2 = eng.plan(2, 8, 64, 64, True, False)
         assert not p2.bwd and all(a.grad is None for a in p2.acts.values())
@@ -462,7 +477,7 @@ def test_weight_gradient_workspaces_dry_run():
         st = E.ParamStore(g, "cpu")
         eng = E.EncoderEngine(st, g, "parity")
         p = eng.plan(2, 8, 64, 64, True, True)
-        assert len(p.wgrads) + len(p.s2d_wgrads) == 77 - (9 if g.fuse_b12 else 0) + 2 and len(p.s2d_wgrads) == 1
+        assert len(p.wgrads) + len(p.s2d_wgrads) == 77 - 9 + 2 and len(p.s2d_wgrads) == 1
         shared = {w.ws for w in p.wgrads}
         assert len(shared) == 1 and p.wg_ws is not None and shared == {p.wg_ws.data_ptr()}
         need = [int(lib.coclr_wgrad_ws_floats(C.byref(w))) for w in p.wgrads]
@@ -474,53 +489,5 @@ def test_weight_gradient_workspaces_dry_run():
         # launch accounting: a weight gradient with a workspace is two kernels
         wl = [(fn, a) for fn, a in p.bwd if fn.__name__ == "coclr_conv_wgrad"]
         assert sum(L.kernels_of(fn, a) for fn, a in wl) == len(wl) + sum(1 for n in need if n > 0)
-    finally:
-        L.DRY_RUN = False
-
-
-def test_overlapped_allreduce_ranges_are_final_when_reduced():
-    """The flat gradient is all-reduced in two parts (moco._EncodeFn.backward): the first part while the second segment
-    of the backward launch list still runs.  Host logic, checked on the dry-run plan: the two range sets partition the
-    buffer, and no launch of the second segment writes a gradient that the first all-reduce has already taken."""
-    import ctypes as C
-    from coclr_b200 import lib as L, engine as E
-    from coclr_b200.s3d_spec import s3d_stages
-    from coclr_b200.r50_spec import r50_stages
-    L.DRY_RUN = True
-    try:
-        for stages, fs in ((s3d_stages(3), 1024), (r50_stages(3), 2048)):
-            g = E.Graph(stages, 3, head_dim=128, feature_size=fs, bb_prefix="0.")
-            st = E.ParamStore(g, "cpu")
-            eng = E.EncoderEngine(st, g, "parity")
-            p = eng.plan(2, 8, 64, 64, True, True)
-            assert p.bwd_split is not None and 0 < p.bwd_split < len(p.bwd)
-            first, rest = eng.grad_ranges(p)
-            cover = sorted(first + rest)
-            assert cover[0][0] == 0 and cover[-1][1] == st.numel
-            assert all(a[1] == b[0] for a, b in zip(cover, cover[1:])), cover
-            assert sum(hi - lo for lo, hi in first) >= 0.7 * st.numel
-            base = st.grad.data_ptr()
-
-            def written(fn, args):
-                """element offsets of the flat gradient this launch writes"""
-                o = args[0]._obj if (args and hasattr(args[0], "_obj")) else None
-                name = fn.__name__
-                out = []
-                if name == "coclr_conv_wgrad":
-                    out.append(o.dw)
-                elif name == "coclr_conv_wgrad_s2d":
-                    out.append(eng.s2d[[k for k in eng.s2d][0]]["dw"].data_ptr())
-                elif name == "coclr_bn_bwd":
-                    out += [o.dgamma, o.dbeta]
-                elif name == "coclr_l2norm_bwd":
-                    out.append(args[4].value)
-                elif name == "coclr_bias_relu_bwd":
-                    out.append(args[3].value)
-                return [(ptr - base) // 4 for ptr in out if ptr]
-            late = [off for fn, args in p.bwd[p.bwd_split:] for off in written(fn, args)]
-            early = [off for fn, args in p.bwd[:p.bwd_split] for off in written(fn, args)]
-            assert late and early
-            assert all(any(lo <= off < hi for lo, hi in rest) for off in late), "a late launch writes an early range"
-            assert all(any(lo <= off < hi for lo, hi in first) for off in early), "an early launch writes a late range"
     finally:
         L.DRY_RUN = False

@@ -49,7 +49,7 @@ else:
     dy.hi.normal_(); dy.lo.normal_(0, 1e-3)
     dw = torch.zeros_like(w)
     splits = int(os.environ.get("SPLITS", "50"))
-    ws = [True if os.environ.get("WS") else None]     # WS=1: workspace epilogue of the TMA-staged kernel
+    ws = [True]     # allocated by the first call, reused afterwards
 
     def run():
         ws[0] = ops.conv_wgrad(x.src(0, r8(Cin), T, H, W), 1, geom.c(0), dy.src(0, r8(Cout), To, Ho, Wo), 1, B,

@@ -30,7 +30,7 @@ def launches(src, dst):
         n += 1
     total = sum(v[1] for v in tot.values())
     with open(dst, "w") as f:
-        f.write("# ncu launch list of `COCLR_GRAPHS=0 python bench.py --steps 1 --warmup 1 --no-cpu-baseline --no-e2e`\n"
+        f.write("# ncu launch list of `python bench.py --steps 1 --warmup 1 --no-cpu-baseline --no-e2e`\n"
                 "# (1 warm-up + 1 timed + 1 per-launch-profiled training step), `ncu --metrics gpu__time_duration.sum\n"
                 "# --clock-control none`; per-launch times are cold-cache and serialised: compare SHARES, not absolutes.\n"
                 "# %d launches, %.1f ms total\n# kernel | launches | total us | share\n" % (n, total / 1e3))
