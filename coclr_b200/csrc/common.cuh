@@ -175,57 +175,57 @@ COCLR_DEVINL void wgmma_n32(float* d, uint64_t a, uint64_t b, uint32_t scale_d) 
   }
 }
 
-// m64 x n{96,128} x k16, fp32 accumulate, both operands K-major.
-template <bool kBf16>
-COCLR_DEVINL void wgmma_n96_kmaj(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+// m64 x n{96,128} x k16, fp32 accumulate; kTA / kTB as for wgmma_n64.
+template <bool kBf16, int kTA, int kTB>
+COCLR_DEVINL void wgmma_n96(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
   if constexpr (kBf16) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, 0, 0;\n\t}"
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, %51, %52;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
-        : "l"(a), "l"(b), "r"(scale_d));
+        : "l"(a), "l"(b), "r"(scale_d), "n"(kTA), "n"(kTB));
   } else {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, 0, 0;\n\t}"
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, %51, %52;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
-        : "l"(a), "l"(b), "r"(scale_d));
+        : "l"(a), "l"(b), "r"(scale_d), "n"(kTA), "n"(kTB));
   }
 }
-template <bool kBf16>
-COCLR_DEVINL void wgmma_n128_kmaj(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+template <bool kBf16, int kTA, int kTB>
+COCLR_DEVINL void wgmma_n128(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
   if constexpr (kBf16) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "l"(a), "l"(b), "r"(scale_d));
+        : "l"(a), "l"(b), "r"(scale_d), "n"(kTA), "n"(kTB));
   } else {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "l"(a), "l"(b), "r"(scale_d));
+        : "l"(a), "l"(b), "r"(scale_d), "n"(kTA), "n"(kTB));
   }
 }
 
-// m64 x kN x k16 with both operands K-major; the width and the 16-bit format are fixed at compile time, so a run of
-// these issues back to back with no branch between them.
-template <int kN, bool kBf16>
-COCLR_DEVINL void wgmma_kmaj(float (&d)[kN / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
-  static_assert(kN == 32 || kN == 64 || kN == 96 || kN == 128, "wgmma_kmaj: N is 32, 64, 96 or 128");
-  if constexpr (kN == 32) wgmma_n32<kBf16, 0, 0>(d, a, b, scale_d);
-  else if constexpr (kN == 64) wgmma_n64<kBf16, 0, 0>(d, a, b, scale_d);
-  else if constexpr (kN == 96) wgmma_n96_kmaj<kBf16>(d, a, b, scale_d);
-  else wgmma_n128_kmaj<kBf16>(d, a, b, scale_d);
+// m64 x kN x k16; the width, the 16-bit format and the operand majors (kTA / kTB = 1: MN-major) are fixed at compile
+// time, so a run of these issues back to back with no branch between them.
+template <int kN, bool kBf16, int kTA, int kTB>
+COCLR_DEVINL void wgmma_mma(float (&d)[kN / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
+  static_assert(kN == 32 || kN == 64 || kN == 96 || kN == 128, "wgmma_mma: N is 32, 64, 96 or 128");
+  if constexpr (kN == 32) wgmma_n32<kBf16, kTA, kTB>(d, a, b, scale_d);
+  else if constexpr (kN == 64) wgmma_n64<kBf16, kTA, kTB>(d, a, b, scale_d);
+  else if constexpr (kN == 96) wgmma_n96<kBf16, kTA, kTB>(d, a, b, scale_d);
+  else wgmma_n128<kBf16, kTA, kTB>(d, a, b, scale_d);
 }
 
 // Issues one pipeline stage into the fresh block t and commits it as one wgmma group, without waiting: t = sum over
 // the kNProd (<= 3) operand pairs (ad[p], bd[p]), in that order, of 4 K = 16 steps (descriptor increments a_inc /
 // b_inc), one full-width instruction per (pair, step); scale_d = 0 on the first.  The caller waits for the group and
 // adds t into its accumulator with fp32 adds, as wgmma_stage does per 64-column block: t[i] has the register layout
-// of wgmma_stage's acc[i].
-template <int kN, bool kBf16, int kNProd>
+// of wgmma_stage's acc[i].  kTA / kTB = 1: the operand is MN-major.
+template <int kN, bool kBf16, int kNProd, int kTA = 0, int kTB = 0>
 COCLR_DEVINL void wgmma_stage_issue(float (&t)[kN / 2], const uint64_t (&ad)[3], const uint64_t (&bd)[3], uint32_t a_inc,
                                     uint32_t b_inc) {
   acc_fence(t);
@@ -233,7 +233,8 @@ COCLR_DEVINL void wgmma_stage_issue(float (&t)[kN / 2], const uint64_t (&ad)[3],
 #pragma unroll
   for (int p = 0; p < kNProd; ++p) {
 #pragma unroll
-    for (uint32_t k = 0; k < 4; ++k) wgmma_kmaj<kN, kBf16>(t, ad[p] + k * a_inc, bd[p] + k * b_inc, (p | (int)k) != 0);
+    for (uint32_t k = 0; k < 4; ++k)
+      wgmma_mma<kN, kBf16, kTA, kTB>(t, ad[p] + k * a_inc, bd[p] + k * b_inc, (p | (int)k) != 0);
   }
   wgmma_commit();
   acc_fence(t);

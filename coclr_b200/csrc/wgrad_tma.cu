@@ -24,9 +24,13 @@
 //  * the pixel range is split over CTAs; every CTA ends with plain stores of its [cout, columns] register
 //    accumulator into the workspace, and one reduction launch sums the splits into dW (no atomics).
 //
-// Warp roles (288 threads): 0-7 two MMA warpgroups (64-cout block wg of the item each) + epilogue, 8 loader.
+// Warp roles (384 threads, three warpgroups): 0 loader, 1-3 idle (warpgroup 0 gives its registers to the consumers),
+// 4-11 two MMA warpgroups (64-cout block wg of the item each) + epilogue.
 #include <cuda.h>
 #include <string.h>
+
+#include <type_traits>
+#include <utility>
 
 #include "common.cuh"
 #include "coclr_b200.h"
@@ -34,9 +38,9 @@
 
 namespace coclr {
 
-static constexpr int kWgMmaWarps = 8;
-static constexpr int kWgThreads = (kWgMmaWarps + 1) * 32;
-static constexpr int kWgAccChunks = 8;               // N <= 256: 128 fp32 accumulator registers per thread
+static constexpr int kWgThreads = 12 * 32;
+static constexpr int kWgFirstMmaWarp = 4;            // warpgroup 0 loads, warpgroups 1-2 compute
+static constexpr uint32_t kWgLoaderRegs = 40, kWgMmaRegs = 232;   // 128 x 40 + 256 x 232 <= 64 Ki registers
 static constexpr int kWgTilePx = 64;                 // pixels per pipeline stage (4 K steps of 16)
 static constexpr int kWgBlockBytes = kWgTilePx * 128;  // one [64 px][64 ch] operand block
 static constexpr int kWgMaxStages = 4;
@@ -101,6 +105,29 @@ COCLR_DEVINL WgCol wg_col(const WgPlan& L, const WgType& T, int cg, int col) {
   return r;
 }
 
+// An item's kN columns are multiplied in sub-blocks, one wgmma group each; a sub-block starts on a 64-column block
+// boundary (an MN-major operand has no other column offsets).  Widths: 64 for kN = 64 (one group per stage, not
+// pipelined), 2 x 64 for kN = 128, 128 + 64 for kN = 192 and 4 x 64 for kN = 256.  The pipelined forms have an even
+// number of sub-blocks, so each keeps its fresh block from stage to stage, and the accumulator (kN / 2 registers) plus
+// the two fresh blocks stay within 192 registers per thread.
+__host__ __device__ constexpr int wg_nsub(int n) { return n == 64 ? 1 : (n == 256 ? 4 : 2); }
+__host__ __device__ constexpr int wg_sub_cols(int n, int j) { return n == 192 && j == 0 ? 128 : 64; }
+__host__ __device__ constexpr int wg_sub_col0(int n, int j) { return j == 0 ? 0 : wg_sub_col0(n, j - 1) + wg_sub_cols(n, j - 1); }
+
+template <int P, class A, class B>
+COCLR_DEVINL auto& wg_pick(A& a, B& b) {
+  if constexpr (P == 0) return a;
+  else return b;
+}
+// f(0) && f(1) && ... with compile-time arguments
+template <class F, int... Q>
+COCLR_DEVINL bool wg_static_all(F&& f, std::integer_sequence<int, Q...>) {
+  return (f(std::integral_constant<int, Q>{}) && ...);
+}
+
+// kN = the plan's L.N (64, 128, 192 or 256); kNProd = products per K step: 1 (single pass), 2 (Cout <= 64, hi / lo dY
+// planes stacked over the two warpgroups), 3 (three passes); kBf16 = the 16-bit format of the planes.
+template <int kN, int kNProd, bool kBf16>
 __global__ void __launch_bounds__(kWgThreads, 1)
 wgrad_tma_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid_constant__ CUtensorMap map_dy_lo,
                  const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__ CUtensorMap map_x_lo,
@@ -108,7 +135,7 @@ wgrad_tma_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid_con
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const WgPlan& L = P.plan;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);   // provably warp-uniform role branches for ptxas
 
   // work item: column group fastest (items that share a dY tile run at the same time: L2 hits), then cout group, split
   int w = blockIdx.x;
@@ -129,19 +156,19 @@ wgrad_tma_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid_con
   if (threadIdx.x == 0) {
     for (int s = 0; s < kWgMaxStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kWgMmaWarps);   // one arrival per consumer warp
+      mbar_init(&empty_bar[s], 128u * (uint32_t)L.mb);   // one arrival per thread of every consumer warpgroup with work
     }
     mbar_fence_init();
   }
   __syncthreads();
   const WgType& T = L.type[type_i];
-  const int Nt = L.nload > 1 ? L.N : 64 * T.nblk;     // columns of this item's MMAs
   const uint32_t dy_plane_bytes = (uint32_t)L.mb * kWgBlockBytes;
   const uint32_t x_plane_bytes = (uint32_t)L.nload * (uint32_t)L.slab_bytes;
 
-  if (warp == kWgMmaWarps) {
+  if (warp < kWgFirstMmaWarp) {
+    setmaxnreg_dec<kWgLoaderRegs>();   // warpgroup 0: the loader warp 0, and warps 1-3 idle
     // ===================== loader =====================
-    if (elect_one()) {
+    if (warp == 0 && elect_one()) {
       tma_prefetch_desc(&map_dy_hi);
       tma_prefetch_desc(&map_x_hi);
       if (L.planes > 1) {
@@ -188,55 +215,120 @@ wgrad_tma_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid_con
       }
     }
   } else {
+    setmaxnreg_inc<kWgMmaRegs>();
     // ===================== MMA: warpgroup wg multiplies dY block wg (stacked: plane wg) with the X slab =====================
-    const int wg = warp >> 2;
+    const int wg = (warp - kWgFirstMmaWarp) >> 2;
+    // L.mb == 1 (one 64-cout block, not stacked): warpgroup 2 has no rows; the empty barriers count only warpgroup 1
+    if (wg >= L.mb) return;
     const int tw = threadIdx.x & 127;
-    const bool active = L.stacked || wg < L.mb;
-    const bool bf16 = P.dy_bf16 != 0;
-    float acc[16 * kWgAccChunks];
+    constexpr int kNSub = wg_nsub(kN);                  // sub-blocks (wgmma groups) per stage
+    static_assert(kNSub == 1 || kNSub % 2 == 0, "a sub-block keeps its fresh block from stage to stage");
+    constexpr int kT0 = wg_sub_cols(kN, 0) / 2, kT1 = wg_sub_cols(kN, kNSub == 1 ? 0 : 1) / 2;
+    const uint32_t smem_base = smem_u32(smem);
+    float acc[kN / 2];
 #pragma unroll
-    for (int i = 0; i < 16 * kWgAccChunks; ++i) acc[i] = 0.f;
-    uint32_t stage = 0, phase = 0;
-    for (int it = 0; it < ntile; ++it) {
-      mbar_wait_spin(&full_bar[stage], phase);
-      if (active) {
-        const uint32_t s_dy = smem_u32(smem + stage * L.stage_bytes);
-        const uint32_t s_x = s_dy + L.off_x;
-        // MN-major: LBO = stride between 64-element MN blocks, SBO = stride between 8-pixel groups (one swizzle atom);
-        // one K = 16 step = 16 pixels = 2048 bytes = +128 descriptor units
-        const uint64_t b_hi = make_smem_desc(s_x, (uint32_t)L.lbo_bytes, 1024);
-        const uint64_t b_lo = make_smem_desc(s_x + x_plane_bytes, (uint32_t)L.lbo_bytes, 1024);
-        const uint32_t b_step = (uint32_t)L.lbo_bytes >> 4;
-        const uint64_t a_hi = make_smem_desc(s_dy + (uint32_t)wg * kWgBlockBytes, kWgBlockBytes, 1024);
+    for (int i = 0; i < kN / 2; ++i) acc[i] = 0.f;
+    float t0[kT0], t1[kT1];
+    // Issues sub-block j of the tile in stage slot s into t.  The products and their order per column are those of one
+    // full-width stage: dY_hi X_lo, dY_lo X_hi, dY_hi X_hi (stacked: this warpgroup's plane X_lo, X_hi), 4 K steps each.
+    auto issue = [&](auto jc, uint32_t s, auto& t) {
+      constexpr int j = decltype(jc)::value;
+      const uint32_t s_dy = smem_base + s * L.stage_bytes;
+      // MN-major: LBO = stride between 64-element MN blocks, SBO = stride between 8-pixel groups (one swizzle atom);
+      // one K = 16 step = 16 pixels = 2048 bytes = +128 descriptor units
+      const uint32_t s_x = s_dy + L.off_x + (uint32_t)(wg_sub_col0(kN, j) / 64) * (uint32_t)L.lbo_bytes;
+      const uint64_t b_hi = make_smem_desc(s_x, (uint32_t)L.lbo_bytes, 1024);
+      const uint64_t b_lo = make_smem_desc(s_x + x_plane_bytes, (uint32_t)L.lbo_bytes, 1024);
+      const uint64_t a_hi = make_smem_desc(s_dy + (uint32_t)wg * kWgBlockBytes, kWgBlockBytes, 1024);
+      if constexpr (kNProd == 1) {
+        const uint64_t ad[3] = {a_hi, a_hi, a_hi}, bd[3] = {b_hi, b_hi, b_hi};
+        wgmma_stage_issue<wg_sub_cols(kN, j), kBf16, 1, 1, 1>(t, ad, bd, 128u, 128u);
+      } else if constexpr (kNProd == 2) {
+        const uint64_t ad[3] = {a_hi, a_hi, a_hi}, bd[3] = {b_lo, b_hi, b_hi};
+        wgmma_stage_issue<wg_sub_cols(kN, j), kBf16, 2, 1, 1>(t, ad, bd, 128u, 128u);
+      } else {
         const uint64_t a_lo = make_smem_desc(s_dy + dy_plane_bytes + (uint32_t)wg * kWgBlockBytes, kWgBlockBytes, 1024);
-        if (L.planes == 1) {
-          const uint64_t ad[3] = {a_hi, a_hi, a_hi}, bd[3] = {b_hi, b_hi, b_hi};
-          wgmma_stage<kWgAccChunks, 1, 1>(acc, ad, bd, 1, 128u, 128u, b_step, Nt, bf16);
-        } else if (L.stacked) {
-          const uint64_t ad[3] = {a_hi, a_hi, a_hi}, bd[3] = {b_lo, b_hi, b_hi};
-          wgmma_stage<kWgAccChunks, 1, 1>(acc, ad, bd, 2, 128u, 128u, b_step, Nt, bf16);
-        } else {
-          const uint64_t ad[3] = {a_hi, a_lo, a_hi}, bd[3] = {b_lo, b_hi, b_hi};   // small products first
-          wgmma_stage<kWgAccChunks, 1, 1>(acc, ad, bd, 3, 128u, 128u, b_step, Nt, bf16);
-        }
+        const uint64_t ad[3] = {a_hi, a_lo, a_hi}, bd[3] = {b_lo, b_hi, b_hi};   // small products first
+        wgmma_stage_issue<wg_sub_cols(kN, j), kBf16, 3, 1, 1>(t, ad, bd, 128u, 128u);
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[stage]);
-      if (++stage == (uint32_t)L.stages) { stage = 0; phase ^= 1u; }
+    };
+    // Adds a completed sub-block j into the accumulator (once per stage and column: the precision contract)
+    auto fold = [&](auto jc, auto& t) {
+      constexpr int j = decltype(jc)::value;
+      constexpr int c0 = wg_sub_col0(kN, j) / 2;
+      acc_fence(t);
+#pragma unroll
+      for (int i = 0; i < wg_sub_cols(kN, j) / 2; ++i) acc[c0 + i] += t[i];
+    };
+    // Group q + 1 is issued before group q is waited for and folded, so one group is always in flight while a
+    // warpgroup folds, releases a stage and waits on the next full barrier.  A stage is released after its last
+    // sub-block has been folded; every consumer thread arrives (an arrival under `lane == 0` would be a
+    // thread-dependent branch inside the wgmma pipeline, which ptxas answers by serialising every wgmma).
+    uint32_t stage = 0, phase = 0;   // the stage being folded
+    // Waits for the stage after the one being folded and issues its first sub-block into t
+    auto issue_next_tile = [&](auto& t) {
+      uint32_t ns = stage + 1, np = phase;
+      if (ns == (uint32_t)L.stages) { ns = 0; np ^= 1u; }
+      mbar_wait_spin(&full_bar[ns], np);
+      issue(std::integral_constant<int, 0>{}, ns, t);
+    };
+    // Folds sub-block j and, after the stage's last one, releases the stage
+    auto retire = [&](auto qc) {
+      constexpr int j = decltype(qc)::value;
+      fold(qc, wg_pick<j & 1>(t0, t1));
+      if constexpr (j == kNSub - 1) {
+        mbar_arrive(&empty_bar[stage]);
+        if (++stage == (uint32_t)L.stages) { stage = 0; phase ^= 1u; }
+      }
+    };
+    // Sub-block q of a stage: issues the group after it, waits for it and retires it.  Only a stage's last sub-block can
+    // be the item's last group: the loop ends there, in a branch that waits for everything (ptxas has to see that no
+    // group is left in flight on any path).
+    int tiles_left = ntile - 1;   // tiles whose first group is not issued yet
+    auto step = [&](auto qc) -> bool {
+      constexpr int q = decltype(qc)::value;
+      if constexpr (q + 1 < kNSub) {
+        issue(std::integral_constant<int, q + 1>{}, stage, wg_pick<(q + 1) & 1>(t0, t1));
+      } else {
+        if (tiles_left == 0) {
+          wgmma_wait<0>();
+          retire(qc);
+          return false;
+        }
+        issue_next_tile(wg_pick<(q + 1) & 1>(t0, t1));
+        --tiles_left;
+      }
+      wgmma_wait<1>();
+      retire(qc);
+      return true;
+    };
+    if constexpr (kNSub == 1) {
+      for (int it = 0; it < ntile; ++it) {
+        mbar_wait_spin(&full_bar[stage], phase);
+        issue(std::integral_constant<int, 0>{}, stage, t0);
+        wgmma_wait<0>();
+        retire(std::integral_constant<int, 0>{});
+      }
+    } else if (ntile > 0) {
+      mbar_wait_spin(&full_bar[0], 0);
+      issue(std::integral_constant<int, 0>{}, 0u, t0);
+      while (wg_static_all(step, std::make_integer_sequence<int, kNSub>{})) {
+      }
     }
     // ===================== epilogue =====================
     // the accumulator goes to ws[item][column][row] with plain stores; wgrad_reduce_kernel sums the pixel splits into dW
+    // (and drops the columns of taps an item does not have: the 3-tap parity of the temporally strided stem conv runs
+    // at the 4-tap width kN; its 4th block reads frames inside the slab, which is sized for 4 taps)
     const int R = 128;
     const int row0 = 64 * wg + 16 * (tw >> 5) + ((tw & 31) >> 2);
     const int col0 = 2 * (tw & 3);
 #pragma unroll
-    for (int c = 0; c < kWgAccChunks; ++c) {
-      if (c * 32 >= Nt) break;
+    for (int c = 0; c < kN / 32; ++c) {
 #pragma unroll
       for (int r = 0; r < 16; ++r) {
         const int row = row0 + 8 * ((r >> 1) & 1);      // row of the item's M = 128 tile
         const int col = c * 32 + col0 + 8 * (r >> 2) + (r & 1);
-        P.ws[((size_t)blockIdx.x * L.N + col) * R + row] = acc[16 * c + r];
+        P.ws[((size_t)blockIdx.x * kN + col) * R + row] = acc[16 * c + r];
       }
     }
   }
@@ -509,6 +601,30 @@ static bool wgrad_tma_plan(const coclr_wgrad_t& P, WgPlan& L, MapSpec& DY, MapSp
 
 static bool g_wgrad_tma = true;
 
+template <int kN, int kNProd, bool kBf16>
+static int wgrad_tma_launch_n(int grid, const CUtensorMap& dy_hi, const CUtensorMap& dy_lo, const CUtensorMap& x_hi,
+                              const CUtensorMap& x_lo, const WgArgs& args, cudaStream_t stream) {
+  const cudaError_t e = cudaFuncSetAttribute(wgrad_tma_kernel<kN, kNProd, kBf16>,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)args.plan.total);
+  if (e != cudaSuccess) return COCLR_E_LAUNCH;
+  wgrad_tma_kernel<kN, kNProd, kBf16><<<grid, kWgThreads, args.plan.total, stream>>>(dy_hi, dy_lo, x_hi, x_lo, args);
+  return COCLR_OK;
+}
+
+// One kernel instance per (columns, products per K step, 16-bit format): the wgmma shapes and type are compile-time
+// constants.
+template <int kNProd, bool kBf16>
+static int wgrad_tma_launch(int grid, const CUtensorMap& dy_hi, const CUtensorMap& dy_lo, const CUtensorMap& x_hi,
+                            const CUtensorMap& x_lo, const WgArgs& args, cudaStream_t stream) {
+  switch (args.plan.N) {
+    case 64: return wgrad_tma_launch_n<64, kNProd, kBf16>(grid, dy_hi, dy_lo, x_hi, x_lo, args, stream);
+    case 128: return wgrad_tma_launch_n<128, kNProd, kBf16>(grid, dy_hi, dy_lo, x_hi, x_lo, args, stream);
+    case 192: return wgrad_tma_launch_n<192, kNProd, kBf16>(grid, dy_hi, dy_lo, x_hi, x_lo, args, stream);
+    case 256: return wgrad_tma_launch_n<256, kNProd, kBf16>(grid, dy_hi, dy_lo, x_hi, x_lo, args, stream);
+    default: return COCLR_E_ARG;
+  }
+}
+
 int wgrad_tma_try(const coclr_wgrad_t& P, cudaStream_t stream) {
   if (!g_wgrad_tma || P.ws == nullptr || ((uintptr_t)P.ws & 15)) return 1;
   WgArgs args;
@@ -528,10 +644,16 @@ int wgrad_tma_try(const coclr_wgrad_t& P, cudaStream_t stream) {
   args.out_scale = P.out_scale;
   args.dy_bf16 = P.dy_bf16;
   args.src_bf16 = P.src_bf16;
-  cudaError_t e = cudaFuncSetAttribute(wgrad_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total);
-  if (e != cudaSuccess) return COCLR_E_LAUNCH;
   const int grid = L.n_types * L.n_cgroups * L.m_groups * L.splits;
-  wgrad_tma_kernel<<<grid, kWgThreads, L.total, stream>>>(m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, args);
+  const int nprod = L.planes == 1 ? 1 : (L.stacked ? 2 : 3);
+  int rc;
+  if (nprod == 1) rc = args.dy_bf16 ? wgrad_tma_launch<1, true>(grid, m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, args, stream)
+                                    : wgrad_tma_launch<1, false>(grid, m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, args, stream);
+  else if (nprod == 2) rc = args.dy_bf16 ? wgrad_tma_launch<2, true>(grid, m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, args, stream)
+                                         : wgrad_tma_launch<2, false>(grid, m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, args, stream);
+  else rc = args.dy_bf16 ? wgrad_tma_launch<3, true>(grid, m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, args, stream)
+                         : wgrad_tma_launch<3, false>(grid, m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, args, stream);
+  if (rc != COCLR_OK) return rc;
   const int rows = L.stacked ? 64 : L.mb * 64;
   const dim3 rgrid((L.N * rows + 255) / 256, L.n_types * L.n_cgroups * L.m_groups);
   wgrad_reduce_kernel<<<rgrid, 256, 0, stream>>>(args);
