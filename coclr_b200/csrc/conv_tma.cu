@@ -17,15 +17,17 @@
 //  * two consumer warpgroups (64 tile rows each) accumulate in registers with wgmma: one m64 x BN x k16 instruction
 //    per product and K step, BN fixed at compile time.  Each 64-deep K chunk (a pipeline stage) is summed in a fresh
 //    register block and added to the accumulator in fp32; the next stage's instructions are issued before that add,
-//    so the tensor cores are not idle while a stage is folded and its shared-memory slots are released.  The
-//    accumulator goes through a [128][33] fp32 transpose tile 32 columns at a time, from which warps 4-7 (32 rows
-//    each) fill a swizzled staging row block, accumulate the BatchNorm statistics from it, and write it with ONE
-//    cp.async.bulk.tensor store (or add-reduction, for gradient accumulation) per 32 rows x 32 channels: edge
-//    clipping, channel slices of concat buffers and the strided frame order of the transposed stem conv are
-//    properties of the output tensor map, not code.
+//    so the tensor cores are not idle while a stage is folded and its shared-memory slots are released.
+//  * epilogue: each consumer thread scales its accumulator fragment in registers and writes it, 32 columns at a time,
+//    into a 128B-swizzled staging block of 32 tile rows (two warps per block, which take alternate chunks for the
+//    rest).  A chunk's warp accumulates the BatchNorm statistics from it and writes it with ONE cp.async.bulk.tensor
+//    store (or add-reduction, for gradient accumulation) per 32 rows x 32 channels: edge clipping, channel slices of
+//    concat buffers and the strided frame order of the transposed stem conv are properties of the output tensor map,
+//    not code.  The two warpgroups share no barrier, so one's epilogue runs while the other's MMAs keep the tensor
+//    cores busy.
 //
 // Warp roles (384 threads, three warpgroups): 0 A loader, 1 weight loader, 2-3 idle (warpgroup 0 gives its registers to
-// the consumers), 4-11 MMA (warpgroups 1 and 2), 4-7 also the epilogue.
+// the consumers), 4-11 MMA and epilogue (warpgroups 1 and 2).
 #include <cuda.h>
 #include <string.h>
 
@@ -40,11 +42,14 @@ static constexpr int kTmaMmaWarps = 8;
 static constexpr int kTmaFirstMmaWarp = 4;     // warpgroup 0 loads, warpgroups 1-2 compute
 static constexpr int kTmaMaxBN = 128;          // 64 fp32 accumulator registers per thread
 static constexpr uint32_t kTmaLoaderRegs = 40, kTmaMmaRegs = 232;   // 128 x 40 + 256 x 232 <= 64 Ki registers
-static constexpr int kXPitch = 33;             // floats per row of the accumulator transpose tile
-static constexpr uint32_t kXTileBytes = 128u * kXPitch * 4u;
 static constexpr int kTmaMaxASlots = 4;
 static constexpr int kTmaMaxBSlots = 4;
-static constexpr uint32_t kStageBytes = 4096;  // 32 rows x 32 fp32 columns per epilogue warp and buffer
+static constexpr uint32_t kStageBytes = 4096;  // 32 rows x 32 fp32 columns per staging block and buffer
+static constexpr uint32_t kEpiBarEnd = 5;      // named barriers 1-4: the warp pairs of staging blocks 0-3
+// Shared memory the planner leaves unused: what the earlier epilogue's transpose tile and scale table took.  Handing it to
+// the rings would move the temporally strided stem conv to another tile shape, and with it the summation order of its
+// BatchNorm statistics; kept so that every launch runs on the tile plan it had.
+static constexpr int kPlanKeepBytes = 1024 + 128 * 33 * 4;
 
 struct TmaTile {
   int idx[4];
@@ -89,8 +94,6 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
   const uint32_t a_base = smem_base;
   const uint32_t b_base = smem_base + L.off_b;
   const uint32_t stage_base = smem_base + L.off_stage;
-  float* xtile = reinterpret_cast<float*>(smem + L.off_misc + 1024u);   // [128][kXPitch] accumulator transpose tile
-  float* unscale_tab = reinterpret_cast<float*>(smem + L.off_misc);
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + L.off_bars);
   uint64_t* a_empty = a_full + kTmaMaxASlots;
   uint64_t* b_full = a_empty + kTmaMaxASlots;
@@ -113,8 +116,6 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
     }
     mbar_fence_init();
   }
-  for (int i = threadIdx.x; i < 256; i += kTmaThreads)
-    unscale_tab[i] = 1.f;  // per tile the epilogue reads n_tile*BN + c; filled below when there is a table
   __syncthreads();
 
   if (warp < kTmaFirstMmaWarp) {
@@ -183,13 +184,17 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
     }
   } else {
     setmaxnreg_inc<kTmaMmaRegs>();
-    // ===================== MMA (warps 4-11: two warpgroups of 64 rows), then the epilogue (warps 4-7) =====================
+    // ===================== consumers (warps 4-11: two warpgroups of 64 rows): MMA and epilogue =====================
     const int cwarp = warp - kTmaFirstMmaWarp;               // warp index among the consumers
     const int ct = (int)threadIdx.x - kTmaFirstMmaWarp * 32;  // thread index among the consumers
     const int wg = cwarp >> 2;
-    const int tid_wg = threadIdx.x & 127;
-    const bool epi = cwarp < 4;
     const uint32_t a_row_off = (uint32_t)wg * 64u * 128u;   // this warpgroup's 64 rows of the slab window
+    // Staging block blk holds tile rows 32 blk .. 32 blk + 31: warps 2 blk and 2 blk + 1 (the same warpgroup) write 16
+    // rows each and share its stores and statistics.  The pair meets at its own named barrier, so neither warpgroup
+    // waits for the other between tiles.
+    const int blk = cwarp >> 1;
+    const uint32_t pair_bar = 1u + (uint32_t)blk;
+    const uint32_t frow = 16u * (uint32_t)(cwarp & 1) + ((uint32_t)lane >> 2);   // this thread's first row in the block
     float acc[kBN / 2];
     uint32_t aslot = 0, aphase = 0, bslot = 0, bphase = 0;
     if (L.b_resident) mbar_wait_spin(&b_full[0], 0);
@@ -199,14 +204,9 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
     // per-thread state): elected once (elect.sync is deterministic for a given member mask)
     const bool leader = elect_one();
     const float oscale = P.out_scale != nullptr ? __ldg(P.out_scale) : 1.f;
-    if (epi && (P.wunscale != nullptr || P.out_scale != nullptr) && L.n_tiles_n == 1) {
-      for (int i = ct; i < kBN; i += 128)
-        unscale_tab[i] = (P.wunscale != nullptr ? __ldg(P.wunscale + i) : 1.f) * oscale;
-    }
-    if (epi) named_bar_sync(1, 128);
-    const uint32_t my_stage = stage_base + (uint32_t)(cwarp & 3) * (uint32_t)L.stage_bufs * kStageBytes;
-    // BatchNorm statistics: per column, sum and sum of squares of d = x - x0 in fp32, where x0 is the first value of
-    // the column this CTA sees; converted exactly in double when they leave the CTA:
+    const uint32_t my_stage = stage_base + (uint32_t)blk * (uint32_t)L.stage_bufs * kStageBytes;
+    // BatchNorm statistics (chunk c: warp 2 blk + (c & 1)): per column, sum and sum of squares of d = x - x0 in fp32,
+    // where x0 is the first value of the column this warp sees; converted exactly in double when they leave the CTA:
     //   sum x = sum d + n x0,  sum x^2 = sum d^2 + 2 x0 sum d + n x0^2,
     // so that var = E[x^2] - mean^2 (formed in double by the finalize step) does not lose the variance of channels whose
     // spread is small against their mean to fp32 rounding of the raw sums (nn.BatchNorm3d is two-pass)
@@ -215,18 +215,6 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
     int nrows = 0;
 #pragma unroll
     for (int i = 0; i < kChunks; ++i) s1[i] = s2[i] = x0[i] = 0.f;
-    // box-relative position of this lane's row (rows are in box order, dim 1 fastest)
-    int ri[4];
-    {
-      int r = (cwarp & 3) * 32 + lane;
-#pragma unroll
-      for (int d = 0; d < 3; ++d) {
-        ri[d] = r % L.obox[d];
-        r /= L.obox[d];
-      }
-      ri[3] = r;
-    }
-    uint32_t nstore = 0;
     for (int item = first_item; item < n_items; item += item_stride) {
       const TmaTile t = tma_decode(L, item);
       const int ty0 = tma_first_type(L, t);
@@ -306,85 +294,96 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
           retire(t1, rel_a1, rel_b1);
         }
       }
-      // ---- epilogue ----
+      // ---- epilogue: scale, stage, store, statistics ----
+      // Chunks go through the block's staging buffers in rounds: with two buffers a round holds two chunks, one per
+      // buffer, else one.  Both warps of the pair write every chunk of the round; then chunk c is stored and summed by
+      // warp 2 blk + (c & 1), so the two warps take the statistics of a round's two chunks at the same time.
       bool valid = true;
       int oc[4];
+      int r = blk * 32 + lane;   // row r of the tile: box-relative position (rows are in box order, dim 1 fastest)
 #pragma unroll
       for (int d = 0; d < 4; ++d) {
+        const int ri = d < 3 ? r % L.obox[d] : r;
+        if (d < 3) r /= L.obox[d];
         const int o = t.idx[d] * L.o_mul[d];
-        valid = valid && (o + ri[d] < L.oext[d]);
-        oc[d] = o + L.sub[cwarp & 3][d];
+        valid = valid && (o + ri < L.oext[d]);
+        oc[d] = o + L.sub[blk][d];
       }
       const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
-      if (epi && (P.wunscale != nullptr || P.out_scale != nullptr) && L.n_tiles_n > 1) {
-        named_bar_sync(1, 128);   // previous tile's readers are done with the table
-        for (int i = ct; i < kBN; i += 128)
-          unscale_tab[i] = (P.wunscale != nullptr ? __ldg(P.wunscale + t.n_tile * kBN + i) : 1.f) * oscale;
-        named_bar_sync(1, 128);
-      }
 #pragma unroll
       for (int kq = 0; kq < kChunks; ++kq) {
-        const int c0 = kq * 32;
-        const int col0 = t.n_tile * kBN + c0;
+        const int col0 = t.n_tile * kBN + kq * 32;
         if (col0 < L.N) {
-          named_bar_sync(2, kTmaMmaWarps * 32);   // the previous chunk's readers are done with the transpose tile
-          acc_chunk_to_smem<kChunks>(acc, kq, xtile, kXPitch, wg, tid_wg);
-          named_bar_sync(2, kTmaMmaWarps * 32);
-          if (!epi) continue;
-          const float* xrow = xtile + (cwarp * 32 + lane) * kXPitch;
-          const uint32_t buf = my_stage + (L.stage_bufs == 2 ? (nstore & 1u) : 0u) * kStageBytes;
-          if (leader) {
-            // the bulk store that last read this buffer must have finished reading it
-            if (L.stage_bufs == 2) bulk_wait_group_read<1>(); else bulk_wait_group_read<0>();
+          const uint32_t h = L.stage_bufs == 2 ? (uint32_t)kq & 1u : 0u;   // this chunk's buffer
+          if (h == 0u) {
+            // a round starts: the stores of the last round have read both buffers (each warp waits for its own) and
+            // both warps are done with its statistics
+            if (leader) bulk_wait_group_read<0>();
+            named_bar_sync(pair_bar, 64);
           }
-          __syncwarp();
-          const uint32_t rowaddr = buf + (uint32_t)lane * 128u;
+          const uint32_t buf = my_stage + h * kStageBytes;
+          // this thread's part of the chunk, scaled by the column's weight unscale and the output scale:
+          // acc[16 kq + 4 g + 2 h + e] = row frow + 8 h, column 8 g + 2 (lane % 4) + e
 #pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const float4 u = *reinterpret_cast<const float4*>(unscale_tab + c0 + 4 * q);
-            st_shared_v4(rowaddr + (((uint32_t)q ^ ((uint32_t)lane & 7u)) << 4),
-                         xrow[4 * q + 0] * u.x, xrow[4 * q + 1] * u.y, xrow[4 * q + 2] * u.z, xrow[4 * q + 3] * u.w);
+          for (int g = 0; g < 4; ++g) {
+            const uint32_t cl = 8u * (uint32_t)g + 2u * ((uint32_t)lane & 3u);
+            float f0 = oscale, f1 = oscale;
+            if (P.wunscale != nullptr) {
+              f0 = __ldg(P.wunscale + col0 + cl) * oscale;
+              f1 = __ldg(P.wunscale + col0 + cl + 1) * oscale;
+            }
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+              const uint32_t row = frow + 8u * (uint32_t)hr;
+              st_shared_v2(buf + row * 128u + ((((cl >> 2) ^ row) & 7u) << 4) + ((cl & 3u) << 2),
+                           acc[16 * kq + 4 * g + 2 * hr] * f0, acc[16 * kq + 4 * g + 2 * hr + 1] * f1);
+            }
           }
+          const bool round_end = h == 1u || L.stage_bufs == 1 || kq + 1 == kChunks || col0 + 32 >= L.N;
+          if (!round_end) continue;
           fence_proxy_async_smem();
-          __syncwarp();
-          if (leader) {
-            if (P.accumulate) tma_reduce_add_5d(&map_out, buf, col0, oc[0], oc[1], oc[2], oc[3]);
-            else tma_store_5d(&map_out, buf, col0, oc[0], oc[1], oc[2], oc[3]);
-            bulk_commit_group();
-          }
-          ++nstore;
-          if (want_stats) {
-            // lane c sums column c over the warp's valid rows, reading the swizzled block back (conflict-free)
-            if (vmask != 0u) {
+          named_bar_sync(pair_bar, 64);
+#pragma unroll
+          for (int c = 0; c < kChunks; ++c) {
+            // the round's chunks: kq, and kq - 1 when kq went into the second buffer; chunk c belongs to warp c & 1
+            if (!(c == kq || (c == kq - 1 && h == 1u)) || (c & 1) != (cwarp & 1)) continue;
+            const uint32_t cbuf = my_stage + (L.stage_bufs == 2 ? (uint32_t)c & 1u : 0u) * kStageBytes;
+            const int ccol0 = t.n_tile * kBN + c * 32;
+            if (leader) {
+              if (P.accumulate) tma_reduce_add_5d(&map_out, cbuf, ccol0, oc[0], oc[1], oc[2], oc[3]);
+              else tma_store_5d(&map_out, cbuf, ccol0, oc[0], oc[1], oc[2], oc[3]);
+              bulk_commit_group();
+            }
+            if (want_stats && vmask != 0u) {
+              // lane j sums column j over the block's valid rows, reading the swizzled block back (conflict-free)
               float a = 0.f, b = 0.f;
               const uint32_t cchunk = (uint32_t)lane >> 2, cword = ((uint32_t)lane & 3u) << 2;
-              if (!((x0_set >> kq) & 1u)) {
+              if (!((x0_set >> c) & 1u)) {
                 const uint32_t r0 = (uint32_t)__ffs((int)vmask) - 1u;
-                x0[kq] = ld_shared_f32(buf + r0 * 128u + ((cchunk ^ (r0 & 7u)) << 4) + cword);
-                x0_set |= 1u << kq;
+                x0[c] = ld_shared_f32(cbuf + r0 * 128u + ((cchunk ^ (r0 & 7u)) << 4) + cword);
+                x0_set |= 1u << c;
               }
-              const float xs = x0[kq];
+              const float xs = x0[c];
 #pragma unroll 8
               for (uint32_t r = 0; r < 32; ++r) {
                 if ((vmask >> r) & 1u) {
-                  const float d = ld_shared_f32(buf + r * 128u + ((cchunk ^ (r & 7u)) << 4) + cword) - xs;
+                  const float d = ld_shared_f32(cbuf + r * 128u + ((cchunk ^ (r & 7u)) << 4) + cword) - xs;
                   a += d;
                   b = fmaf(d, d, b);
                 }
               }
-              s1[kq] += a;
-              s2[kq] += b;
+              s1[c] += a;
+              s2[c] += b;
             }
           }
         }
       }
-      if (!epi) continue;
       nrows += __popc(vmask);
       if (want_stats && L.n_tiles_n > 1) {
 #pragma unroll
         for (int kq = 0; kq < kChunks; ++kq) {
           const int col = t.n_tile * kBN + kq * 32 + lane;
-          if (col < L.N) {
+          if ((kq & 1) == (cwarp & 1) && col < L.N) {
             const double n = (double)nrows, xd = (double)x0[kq];
             atomicAdd(&P.stats_sum[col], (double)s1[kq] + n * xd);
             atomicAdd(&P.stats_sq[col], (double)s2[kq] + xd * (2.0 * (double)s1[kq] + n * xd));
@@ -395,34 +394,32 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
         nrows = 0;
       }
     }
-    if (epi) {
-      if (leader) bulk_wait_group_read<0>();
-      __syncwarp();
-      if (want_stats && L.n_tiles_n == 1) {
-        // combine the four warps' column sums in shared memory (the staging blocks are free now), one fp64 atomic per
-        // channel and CTA
-        double* tab = reinterpret_cast<double*>(smem + L.off_stage);   // [4 warps][2][128] = 8 KB of the staging blocks
-        named_bar_sync(1, 128);
+    if (leader) bulk_wait_group_read<0>();
+    if (want_stats && L.n_tiles_n == 1) {
+      // combine the four blocks' column sums in shared memory (the staging blocks are free now), one fp64 atomic per
+      // channel and CTA
+      double* tab = reinterpret_cast<double*>(smem + L.off_stage);   // [4 blocks][2][128] = 8 KB of the staging blocks
+      named_bar_sync(kEpiBarEnd, kTmaMmaWarps * 32);
 #pragma unroll
-        for (int kq = 0; kq < kChunks; ++kq) {
-          const double n = (double)nrows, xd = (double)x0[kq];
-          tab[(cwarp * 2 + 0) * 128 + kq * 32 + lane] = (double)s1[kq] + n * xd;
-          tab[(cwarp * 2 + 1) * 128 + kq * 32 + lane] = (double)s2[kq] + xd * (2.0 * (double)s1[kq] + n * xd);
-        }
-        named_bar_sync(1, 128);
-        for (int c = ct; c < L.N; c += 128) {
-          double a = 0.0, b = 0.0;
-#pragma unroll
-          for (int w = 0; w < 4; ++w) {
-            a += tab[(w * 2 + 0) * 128 + c];
-            b += tab[(w * 2 + 1) * 128 + c];
-          }
-          atomicAdd(&P.stats_sum[c], a);
-          atomicAdd(&P.stats_sq[c], b);
-        }
+      for (int kq = 0; kq < kChunks; ++kq) {
+        if ((kq & 1) != (cwarp & 1)) continue;
+        const double n = (double)nrows, xd = (double)x0[kq];
+        tab[(blk * 2 + 0) * 128 + kq * 32 + lane] = (double)s1[kq] + n * xd;
+        tab[(blk * 2 + 1) * 128 + kq * 32 + lane] = (double)s2[kq] + xd * (2.0 * (double)s1[kq] + n * xd);
       }
-      if (leader) bulk_wait_group<0>();   // all global writes of this thread's bulk stores are complete
+      named_bar_sync(kEpiBarEnd, kTmaMmaWarps * 32);
+      for (int c = ct; c < L.N; c += kTmaMmaWarps * 32) {
+        double a = 0.0, b = 0.0;
+#pragma unroll
+        for (int w = 0; w < 4; ++w) {
+          a += tab[(w * 2 + 0) * 128 + c];
+          b += tab[(w * 2 + 1) * 128 + c];
+        }
+        atomicAdd(&P.stats_sum[c], a);
+        atomicAdd(&P.stats_sq[c], b);
+      }
     }
+    if (leader) bulk_wait_group<0>();   // all global writes of this thread's bulk stores are complete
   }
 }
 
@@ -712,7 +709,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
   L.plane_stride = (L.slab_bytes + 1023) & ~1023;
   L.a_slot_bytes = planes * L.plane_stride;
   L.b_tile_bytes = planes * L.BN * 128;
-  const int budget = 227 * 1024 - 1024 /*alignment slack*/ - 1024 /*unscale table*/ - (int)kXTileBytes - 256 /*barriers*/;
+  const int budget = 227 * 1024 - 1024 /*alignment slack*/ - kPlanKeepBytes - 256 /*barriers*/;
   const int stage1 = 4 * (int)kStageBytes, stage2 = 8 * (int)kStageBytes;
   const long tiles_per_cta = ((long)L.total_tiles + 131) / 132;   // one wave over the 132 SMs of an H100 SXM
   L.b_resident = 0;
@@ -752,8 +749,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
     L.off_stage = L.off_b + (uint32_t)(L.b_slots * L.b_tile_bytes);
   }
   L.off_stage = (L.off_stage + 1023u) & ~1023u;
-  L.off_misc = L.off_stage + (uint32_t)(L.stage_bufs == 2 ? stage2 : stage1);
-  L.off_bars = L.off_misc + 1024u + kXTileBytes;
+  L.off_bars = L.off_stage + (uint32_t)(L.stage_bufs == 2 ? stage2 : stage1);
   L.total = L.off_bars + 256u + 1024u;
   if (L.total > 227u * 1024u) return false;
   if (L.stage_bufs == 1 && P.stats_sum != nullptr) {

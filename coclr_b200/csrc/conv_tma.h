@@ -38,7 +38,7 @@ struct TmaPlan {
   int stage_bufs;
   int sub[4][4];       // output coordinate offsets of each epilogue warp's 32-row sub-box
   int BN, N;
-  uint32_t off_b, off_stage, off_misc, off_bars, total;
+  uint32_t off_b, off_stage, off_bars, total;
 };
 
 struct TmaArgs {
