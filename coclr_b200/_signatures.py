@@ -43,6 +43,8 @@ EXPORTS = {
     "coclr_gate_bwd_reduce": (I, [P, I, P, P, I, P, I, I, I, I, P, P]),
     "coclr_gate_fc_bwd": (I, [P, P, P, P, P, P, P, I, I, I, I, P]),
     "coclr_gate_bwd_apply": (I, [P, I, P, P, I, I, I, P]),
+    "coclr_cls_head_fwd": (I, [P, P]),
+    "coclr_cls_head_bwd": (I, [P, P]),
 }
 
 

@@ -93,7 +93,11 @@ class Graph:
     """Shape-independent description of the encoder: tensors, convs, pools in forward order."""
 
     def __init__(self, stages, first_channel=3, head_dim=None, feature_size=S3D_FEATURE_SIZE, bb_prefix="",
-                 stem_s2d=True):
+                 stem_s2d=True, pooled=False):
+        """pooled (only without a head): the pass ends with the average-pooled feature [B, feature_size] and its
+        backward starts from that feature's gradient (LinearClassifier's backbone)."""
+        assert not (pooled and head_dim is not None)
+        self.pooled = pooled
         self.tensors, self.items = [], _LaneList(self)   # items: ("conv", ConvSpec) | ("pool", PoolSpec) | ("bn", TensorSpec)
         self.item_lane, self.item_flag = [], []   # per item: stream lane (Inception branches run concurrently) and FORK/JOIN
         self.cur_lane, self.next_flag = 0, 0
@@ -563,6 +567,11 @@ class Plan:
             self.fwd.append(split_op(self.h1, self.h1_pl, B, fs, self.ones, b2, True, self.h1_plw))   # bias + ReLU
             self.fwd.append((lib.coclr_conv_igemm, (C.byref(c2), nsm)))
             self.fwd.append((lib.coclr_l2norm_fwd, (L.dptr(self.h2), L.dptr(b4), L.dptr(self.q), L.dptr(self.inv_norm), B, hd)))
+        elif g.pooled:
+            fs, Pn = g.feature_size, out.dims[0] * out.dims[1] * out.dims[2]
+            self.feat = torch.empty(B, fs, dtype=torch.float32, device=dev)
+            self.fwd.append((lib.coclr_avgpool_fwd, (L.dptr(out.pl.hi), L.dptr(out.pl.lo), out.pl.bf16, out.spec.C, 0,
+                                                     L.dptr(self.feat), B, Pn, fs)))
         if not with_backward:
             return
         # ---- backward ----
@@ -595,6 +604,10 @@ class Plan:
             bw.append(split_op(self.dh1, self.dh1_pl, B, fs, None, None, False))
             bw.append((lib.coclr_conv_wgrad, (C.byref(wg1),)))
             bw.append((lib.coclr_conv_igemm, (C.byref(dg1), nsm)))
+            bw.append((lib.coclr_avgpool_bwd, (L.dptr(self.dfeat), L.dptr(out.grad), out.spec.C, 0, B, Pn, fs)))
+            grad_seen(out)
+        elif g.pooled:
+            self.dfeat = torch.empty(B, fs, dtype=torch.float32, device=dev)
             bw.append((lib.coclr_avgpool_bwd, (L.dptr(self.dfeat), L.dptr(out.grad), out.spec.C, 0, B, Pn, fs)))
             grad_seen(out)
         convs_into, pool_into = {}, {}
@@ -952,6 +965,13 @@ class EncoderEngine:
     def backward(self, p, dq):
         """dq: gradient w.r.t. the normalised features [B, dim]; accumulates into store.grad."""
         p.dq.copy_(dq)
+        wg = L.load().coclr_conv_wgrad
+        self._graphed(p, "bwd", lambda: self._run(p.bwd, side_fn=wg))
+
+    def backward_feat(self, p, dfeat):
+        """dfeat: gradient w.r.t. the pooled feature [B, feature_size] of a `pooled` graph; accumulates into
+        store.grad."""
+        p.dfeat.copy_(dfeat)
         wg = L.load().coclr_conv_wgrad
         self._graphed(p, "bwd", lambda: self._run(p.bwd, side_fn=wg))
 

@@ -97,6 +97,20 @@ class Adam(C.Structure):
                 ("step_size", C.c_float), ("bc2_sqrt", C.c_float)]
 
 
+class ClsHead(C.Structure):
+    _fields_ = [("B", C.c_int), ("fs", C.c_int), ("ncls", C.c_int),
+                ("l2norm", C.c_int), ("bn", C.c_int), ("bn_training", C.c_int), ("dropout", C.c_int),
+                ("p", C.c_float), ("momentum", C.c_float), ("eps", C.c_float),
+                ("seed", C.c_ulonglong), ("offset", C.c_ulonglong),
+                ("feat", C.c_void_p), ("xn", C.c_void_p), ("inv_norm", C.c_void_p),
+                ("xb", C.c_void_p), ("mean", C.c_void_p), ("rstd", C.c_void_p),
+                ("gamma", C.c_void_p), ("beta", C.c_void_p), ("running_mean", C.c_void_p), ("running_var", C.c_void_p),
+                ("mask", C.c_void_p), ("xd", C.c_void_p),
+                ("W", C.c_void_p), ("bias", C.c_void_p), ("logits", C.c_void_p),
+                ("dlogits", C.c_void_p), ("dW", C.c_void_p), ("dbias", C.c_void_p), ("dgamma", C.c_void_p),
+                ("dbeta", C.c_void_p), ("dx", C.c_void_p), ("dfeat", C.c_void_p)]
+
+
 def library_path():
     return _LIB_PATH
 

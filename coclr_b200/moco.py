@@ -5,7 +5,8 @@
 * nce_logits    -- autograd op: fused [q.k, q.queue]/T (+ cross-entropy by-products);
 * nce_cross_entropy -- nn.CrossEntropyLoss-compatible criterion that reuses those by-products;
 * momentum_update / enqueue / concat_all_gather helpers;
-* FlatAdam      -- torch.optim.Adam semantics (main_nce.py:190-200) as one fused launch over the flat buffer.
+* FlatAdam      -- torch.optim.Adam semantics (main_nce.py:190-200) as one fused launch over the flat buffer;
+* SpanAdam      -- the same with one param group (own lr) per flat span (eval/main_classifier.py:134-141).
 """
 import ctypes as C
 import math
@@ -255,6 +256,16 @@ def nce_cross_entropy(logits, labels=None):
     return torch.nn.functional.cross_entropy(logits, labels)
 
 
+def _adam_step(param, grad, exp_avg, exp_avg_sq, grad_scale, group, step):
+    """One coclr_adam_step launch over a flat span: torch.optim.Adam with coupled L2, hyper-parameters of `group`."""
+    b1, b2 = group["betas"]
+    bc1 = 1.0 - b1 ** step
+    bc2 = 1.0 - b2 ** step
+    p = L.Adam(L.dptr(param), L.dptr(grad), L.dptr(exp_avg), L.dptr(exp_avg_sq), param.numel(), grad_scale, b1, b2,
+               group["eps"], group["weight_decay"], group["lr"] / bc1, math.sqrt(bc2))
+    L.check(L.load().coclr_adam_step(C.byref(p), L.num_sms(param.device), L.stream_ptr()), "coclr_adam_step")
+
+
 class FlatAdam:
     """torch.optim.Adam(lr, betas, eps, weight_decay) with coupled L2 over the flat parameter buffer of one
     MoCoEncoder (main_nce.py:190-200 builds one param group per tensor with identical hyper-parameters,
@@ -284,14 +295,8 @@ class FlatAdam:
         if world > 1:
             dist.all_reduce(st.grad)
         mark("opt:allreduce_done")
-        g = self.param_groups[0]
         self.step_count += 1
-        b1, b2 = g["betas"]
-        bc1 = 1.0 - b1 ** self.step_count
-        bc2 = 1.0 - b2 ** self.step_count
-        p = L.Adam(L.dptr(st.flat), L.dptr(st.grad), L.dptr(self.exp_avg), L.dptr(self.exp_avg_sq), st.numel,
-                   1.0 / world, b1, b2, g["eps"], g["weight_decay"], g["lr"] / bc1, math.sqrt(bc2))
-        L.check(L.load().coclr_adam_step(C.byref(p), L.num_sms(st.flat.device), L.stream_ptr()), "coclr_adam_step")
+        _adam_step(st.flat, st.grad, self.exp_avg, self.exp_avg_sq, 1.0 / world, self.param_groups[0], self.step_count)
         mark("opt:adam_done")
 
     def state_dict(self):
@@ -302,3 +307,42 @@ class FlatAdam:
         self.step_count = sd["step"]
         self.exp_avg, self.exp_avg_sq = sd["exp_avg"], sd["exp_avg_sq"]
         self.param_groups = sd["param_groups"]
+
+
+class SpanAdam:
+    """torch.optim.Adam (coupled L2) with one param group per flat span (params, grad): e.g. a fine-tuned backbone at
+    lr / 10 next to the classifier head at lr (eval/main_classifier.py:134-141 builds one group per tensor with those
+    learning rates, which is equivalent).  One coclr_adam_step launch per group; single process (no all-reduce).
+    groups: [{'name': str, 'params': flat fp32 tensor, 'grad': tensor of the same size, 'lr': float}]."""
+
+    def __init__(self, groups, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0):
+        self.param_groups = [{"name": g["name"], "lr": g["lr"], "betas": betas, "eps": eps, "weight_decay": weight_decay}
+                             for g in groups]
+        self.spans = [(g["params"], g["grad"]) for g in groups]
+        self.step_count = 0
+        self.exp_avg = [torch.zeros_like(p) for p, _ in self.spans]
+        self.exp_avg_sq = [torch.zeros_like(p) for p, _ in self.spans]
+
+    def zero_grad(self, set_to_none=False):
+        for _, g in self.spans:
+            g.zero_()
+
+    @torch.no_grad()
+    def step(self):
+        self.step_count += 1
+        for (p, g), m, v, grp in zip(self.spans, self.exp_avg, self.exp_avg_sq, self.param_groups):
+            _adam_step(p, g, m, v, 1.0, grp, self.step_count)
+
+    def state_dict(self):
+        return {"step": self.step_count, "exp_avg": self.exp_avg, "exp_avg_sq": self.exp_avg_sq,
+                "param_groups": self.param_groups}
+
+    def load_state_dict(self, sd):
+        if [g["name"] for g in sd["param_groups"]] != [g["name"] for g in self.param_groups]:
+            raise ValueError("optimizer state has groups %s, expected %s"
+                             % ([g["name"] for g in sd["param_groups"]], [g["name"] for g in self.param_groups]))
+        with torch.no_grad():
+            for dst, src in zip(self.exp_avg + self.exp_avg_sq, list(sd["exp_avg"]) + list(sd["exp_avg_sq"])):
+                dst.copy_(src)
+        self.step_count = sd["step"]
+        self.param_groups = [dict(g) for g in sd["param_groups"]]

@@ -1,0 +1,294 @@
+#!/usr/bin/env python
+"""Fine-tuning / linear-probe driver -- same command line as the reference's eval/main_classifier.py (:37-77) for the
+train / validate loop, on the engine's LinearClassifier (model/classifier.py), plus:
+
+  --synthetic            random clips [B, 3, seq_len, img_dim, img_dim] with labels in [0, num_class) instead of the
+                         LMDB loaders (without it a dataset name raises, as in main_nce.py)
+  --precision MODE       parity | mixed | fast (see DESIGN.md)
+  --steps-per-epoch N    length of a synthetic epoch (the validation pass takes the same number of steps)
+
+--train_what last (linear probe: l2norm + final BN, no dropout, frozen eval-mode backbone), ft (backbone at lr / 10)
+and all (everything at lr) select the parameters and learning rates as the reference does (:102-147); the optimizer is
+Adam with coupled L2 (--wd) as one launch per group over flat buffers (coclr_b200.moco.SpanAdam).  Accuracy and loss are
+accumulated on the device and read back every --print_freq steps.  --test / --retrieval / the multi-crop tests need
+the per-video LMDB datasets, --optim sgd and more than one GPU (the reference's nn.DataParallel) are not available:
+they raise.
+"""
+import argparse
+import os
+import random
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+import torch.nn as nn  # noqa: E402
+
+from model.classifier import LinearClassifier  # noqa: E402
+from coclr_b200 import moco  # noqa: E402
+
+NUM_CLASS = {'ucf101': 101, 'hmdb51': 51, 'k400': 400, 'ucf101-f': 101, 'hmdb51-f': 51, 'k400-f': 400}   # :98-100
+
+
+def parse_args(argv=None):
+    p = argparse.ArgumentParser()
+    p.add_argument('--net', default='s3d', type=str)
+    p.add_argument('--model', default='lincls', type=str)
+    p.add_argument('--dataset', default='ucf101', type=str)
+    p.add_argument('--which_split', default=1, type=int)
+    p.add_argument('--seq_len', default=32, type=int, help='number of frames in each video block')
+    p.add_argument('--num_seq', default=1, type=int, help='number of video blocks')
+    p.add_argument('--num_fc', default=1, type=int, help='number of fc')
+    p.add_argument('--ds', default=1, type=int, help='frame down sampling rate')
+    p.add_argument('--batch_size', default=32, type=int, help='batch size per GPU')
+    p.add_argument('--optim', default='adam', type=str)
+    p.add_argument('--lr', default=1e-3, type=float, help='learning rate')
+    p.add_argument('--schedule', default=[60, 80], nargs='*', type=int, help='epochs at which lr drops 10x')
+    p.add_argument('--wd', default=1e-3, type=float, help='weight decay')
+    p.add_argument('--dropout', default=0.9, type=float, help='dropout')
+    p.add_argument('--epochs', default=10, type=int, help='number of total epochs to run')
+    p.add_argument('--start_epoch', default=0, type=int, help='manual epoch number (useful on restarts)')
+    p.add_argument('--gpu', default=None, type=str)
+    p.add_argument('--train_what', default='last', type=str)
+    p.add_argument('--img_dim', default=128, type=int)
+    p.add_argument('--print_freq', default=5, type=int, help='frequency of printing output during training')
+    p.add_argument('--eval_freq', default=1, type=int)
+    p.add_argument('--reset_lr', action='store_true', help='Reset learning rate when resume training?')
+    p.add_argument('--prefix', default='linclr', type=str)
+    p.add_argument('-j', '--workers', default=8, type=int)
+    p.add_argument('--cos', action='store_true', help='use cosine lr schedule')
+    p.add_argument('--resume', default='', type=str, help='path of model to resume')
+    p.add_argument('--pretrain', default='', type=str, help='path of pretrained model')
+    p.add_argument('--test', default='', type=str, help='path of model to load and pause')
+    p.add_argument('--retrieval', action='store_true', help='path of model to ucf retrieval')
+    p.add_argument('--dirname', default=None, type=str, help='dirname for feature')
+    p.add_argument('--center_crop', action='store_true')
+    p.add_argument('--five_crop', action='store_true')
+    p.add_argument('--ten_crop', action='store_true')
+    # additions
+    p.add_argument('--synthetic', action='store_true')
+    p.add_argument('--precision', default='parity', choices=['parity', 'mixed', 'fast'])
+    p.add_argument('--steps-per-epoch', default=20, type=int)
+    return p.parse_args(argv)
+
+
+def check_supported(args):
+    """Raise for what this driver does not run (see the module docstring)."""
+    for flag in ('test', 'retrieval', 'center_crop', 'five_crop', 'ten_crop'):
+        if getattr(args, flag):
+            raise NotImplementedError("--%s needs the per-video LMDB test datasets of the reference (dataset/), which are "
+                                      "not part of this repository" % flag)
+    if args.optim != 'adam':
+        raise NotImplementedError("--optim %s: only Adam is available (--optim adam)" % args.optim)
+    if args.model != 'lincls':
+        raise NotImplementedError("--model %s" % args.model)
+    if args.train_what not in ('last', 'ft', 'all'):
+        raise ValueError("--train_what must be last, ft or all")
+    if args.gpu is not None and len(str(args.gpu).split(',')) > 1:
+        raise NotImplementedError("--gpu %s: multi-GPU fine-tuning (the reference's nn.DataParallel) is not available; "
+                                  "use one GPU" % args.gpu)
+    if args.dataset not in NUM_CLASS:
+        raise NotImplementedError("dataset %r" % args.dataset)
+
+
+def build_model(args):
+    """LinearClassifier in the configuration of --train_what (:102-118) and the parameters it trains (:125-147)."""
+    last = args.train_what == 'last'
+    args.final_bn, args.final_norm, args.use_dropout = last, last, not last
+    model = LinearClassifier(network=args.net, num_class=args.num_class, dropout=args.dropout,
+                             use_dropout=args.use_dropout, use_final_bn=args.final_bn, use_l2_norm=args.final_norm,
+                             precision=args.precision)
+    if last:
+        for p in model.backbone.parameters():
+            p.requires_grad = False
+    return model
+
+
+def build_optimizer(model, args):
+    """Adam groups (:125-161): the head at lr, plus the backbone at lr / 10 (ft) or lr (all); none for it with last."""
+    spans = model.flat_spans()
+    groups = [dict(name='head', params=spans['head'][0], grad=spans['head'][1], lr=args.lr)]
+    if args.train_what != 'last':
+        groups.insert(0, dict(name='backbone', params=spans['backbone'][0], grad=spans['backbone'][1],
+                              lr=args.lr / 10 if args.train_what == 'ft' else args.lr))
+    return moco.SpanAdam(groups, weight_decay=args.wd)
+
+
+def map_pretrained(state_dict):
+    """Pre-training checkpoint keys -> classifier keys: encoder_q.0. -> backbone. (:251-255); the DistributedDataParallel
+    prefix of the reference's pre-training checkpoints is dropped first."""
+    out = {}
+    for k, v in state_dict.items():
+        if k.startswith('module.'):
+            k = k[len('module.'):]
+        out[k.replace('encoder_q.0.', 'backbone.')] = v
+    return out
+
+
+def load_pretrained(model, state_dict):
+    """Non-strict load of the backbone part; returns the classifier keys that the checkpoint did not provide."""
+    sd = {k: v for k, v in map_pretrained(state_dict).items() if k in model.state_dict()}
+    return model.load_state_dict(sd, strict=False).missing_keys
+
+
+def adjust_learning_rate(optimizer, epoch, args):
+    """Every group's lr x 0.1 at an epoch listed in --schedule (:721-726); unlike main_nce.py, the drop is applied to
+    the current lr at that epoch, not recomputed from the base lr."""
+    ratio = 0.1 if epoch in args.schedule else 1.
+    for g in optimizer.param_groups:
+        g['lr'] = g['lr'] * ratio
+
+
+class SyntheticClips:
+    """Stand-in for the classification datasets after the GPU-side transform: [B, 3, seq_len, H, W] fp32 N(0, 1) and
+    labels in [0, num_class)."""
+
+    def __init__(self, args, device, seed):
+        self.args, self.device = args, device
+        self.gen = torch.Generator(device=device).manual_seed(seed)
+
+    def __iter__(self):
+        a = self.args
+        for _ in range(a.steps_per_epoch):
+            x = torch.randn(a.batch_size, 3, a.seq_len, a.img_dim, a.img_dim, device=self.device, generator=self.gen)
+            y = torch.randint(0, a.num_class, (a.batch_size,), device=self.device, generator=self.gen)
+            yield x, y
+
+    def __len__(self):
+        return self.args.steps_per_epoch
+
+
+def get_data(args, device, mode):
+    if not args.synthetic:
+        raise NotImplementedError(
+            "dataset %r: the LMDB loaders and PIL augmentations of the reference (dataset/, utils/augmentation.py) are "
+            "outside the accelerated hot path; run with --synthetic, or feed [B,3,T,H,W] float tensors from your own "
+            "loader" % args.dataset)
+    return SyntheticClips(args, device, seed=args.seed_base + (0 if mode == 'train' else 1))
+
+
+def set_path(args):
+    if args.resume:
+        exp_path = os.path.dirname(os.path.dirname(args.resume))
+    else:
+        exp_path = 'log-eval-{a.prefix}/{a.dataset}-{a.img_dim}_sp{a.which_split}_{a.model}_{a.net}_Adam_bs{a.batch_size}_' \
+                   'lr{a.lr}_dp{a.dropout}_wd{a.wd}_seq{a.num_seq}_len{a.seq_len}_ds{a.ds}_train-{a.train_what}{pt}'.format(
+                       a=args, pt='_pt=%s' % args.pretrain.replace('/', '-') if args.pretrain else '')
+    model_path = os.path.join(exp_path, 'model')
+    os.makedirs(model_path, exist_ok=True)
+    return model_path
+
+
+def _accumulate(stat, logit, target, loss):
+    with torch.no_grad():
+        top5 = logit.topk(min(5, logit.shape[1]), dim=1).indices
+        hit = top5 == target.unsqueeze(1)
+        stat[0] += loss.detach()
+        stat[1] += hit[:, 0].float().mean()
+        stat[2] += hit.any(1).float().mean()
+        stat[3] += 1
+
+
+def train_one_epoch(loader, model, criterion, optimizer, epoch, args):
+    if args.train_what == 'last':
+        model.eval()                     # frozen backbone BN (:319-320)
+    else:
+        model.train()
+    if args.final_bn:
+        model.final_bn.train()           # :324-325
+    stat = torch.zeros(4, device=torch.device('cuda'))   # loss sum, top1 sum, top5 sum, steps
+    tic = time.time()
+    for idx, (input_seq, target) in enumerate(loader):
+        logit, _ = model(input_seq)
+        loss = criterion(logit, target)
+        _accumulate(stat, logit, target, loss)
+        optimizer.zero_grad()
+        loss.backward()
+        optimizer.step()
+        if idx % args.print_freq == 0:
+            s = stat.tolist()
+            n = max(s[3], 1.0)
+            dt = (time.time() - tic) / n
+            print('Epoch: [%d][%d/%d] loss %.4f acc@1 %.4f acc@5 %.4f  %.1f ms/step  %.0f clips/s'
+                  % (epoch, idx, len(loader), s[0] / n, s[1] / n, s[2] / n, dt * 1e3, args.batch_size / dt))
+        args.iteration += 1
+    s = stat.tolist()
+    n = max(s[3], 1.0)
+    return s[0] / n, s[1] / n
+
+
+def validate(loader, model, criterion, epoch, args):
+    model.eval()
+    stat = torch.zeros(4, device=torch.device('cuda'))
+    with torch.no_grad():
+        for input_seq, target in loader:
+            logit, _ = model(input_seq)
+            _accumulate(stat, logit, target, criterion(logit, target))
+    s = stat.tolist()
+    n = max(s[3], 1.0)
+    print('Epoch: [%d]\tLoss: %.4f Acc@1: %.4f Acc@5: %.4f' % (epoch, s[0] / n, s[1] / n, s[2] / n))
+    return s[0] / n, s[1] / n
+
+
+def main(args):
+    check_supported(args)
+    if args.gpu is not None:
+        torch.cuda.set_device(int(args.gpu))
+    device = torch.device('cuda')
+    torch.manual_seed(0)
+    np.random.seed(0)
+    random.seed(0)
+    args.seed_base = 0
+    args.num_class = NUM_CLASS[args.dataset]
+    model = build_model(args).to(device)
+    optimizer = build_optimizer(model, args)
+    criterion = nn.CrossEntropyLoss()
+    args.iteration = 1
+    best_acc = 0.0
+    if args.resume:
+        ckpt = torch.load(args.resume, map_location='cpu')
+        args.start_epoch = ckpt['epoch'] + 1
+        args.iteration = ckpt['iteration']
+        best_acc = ckpt['best_acc']
+        model.load_state_dict(ckpt['state_dict'])
+        if not args.reset_lr:
+            optimizer.load_state_dict(ckpt['optimizer'])
+        print("=> load resumed checkpoint '%s' (epoch %d)" % (args.resume, ckpt['epoch']))
+    elif args.pretrain:
+        ckpt = torch.load(args.pretrain, map_location='cpu')
+        missing = load_pretrained(model, ckpt['state_dict'])
+        print("=> loaded pretrained checkpoint '%s' (epoch %s); keys not in it: %s"
+              % (args.pretrain, ckpt.get('epoch'), missing))
+    else:
+        print("=> train from scratch")
+    model_path = set_path(args)
+    args.seed_base = args.start_epoch * 2
+    train_loader = get_data(args, device, 'train')
+    val_loader = get_data(args, device, 'val')
+    for epoch in range(args.start_epoch, args.epochs):
+        np.random.seed(epoch)
+        random.seed(epoch)
+        adjust_learning_rate(optimizer, epoch, args)
+        train_one_epoch(train_loader, model, criterion, optimizer, epoch, args)
+        if epoch % args.eval_freq == 0:
+            _, val_acc = validate(val_loader, model, criterion, epoch, args)
+            is_best = val_acc > best_acc
+            best_acc = max(val_acc, best_acc)
+            state = {'epoch': epoch, 'state_dict': model.state_dict(), 'best_acc': best_acc,
+                     'optimizer': optimizer.state_dict(), 'iteration': args.iteration}
+            torch.save(state, os.path.join(model_path, 'epoch%d.pth.tar' % epoch))
+            prev = os.path.join(model_path, 'epoch%d.pth.tar' % (epoch - 1))
+            if os.path.exists(prev):
+                os.remove(prev)
+            if is_best:
+                torch.save(state, os.path.join(model_path, 'model_best.pth.tar'))
+    print('Training from ep %d to ep %d finished' % (args.start_epoch, args.epochs))
+    return model
+
+
+if __name__ == '__main__':
+    main(parse_args())

@@ -348,6 +348,36 @@ int coclr_gate_fc_bwd(const float* dgate, const float* gate, const float* mean, 
                       float* dmean, int B /* <= 256 */, int C, int coff, int n, coclr_stream_t stream);
 int coclr_gate_bwd_apply(float* dout, int ldd, const float* gate, const float* dmean, int B, int P, int C, coclr_stream_t stream);
 
+/* ---- Classifier head of LinearClassifier (model/classifier.py:47-61 of the reference):
+ *   feat [B, fs] -> F.normalize (l2norm) -> BatchNorm1d (bn) -> Dropout (dropout) -> Linear -> logits [B, ncls]
+ * Each stage is optional; a stage that is off passes its input through, and its buffers may be NULL.  fp32
+ * throughout, every sum in a fixed order (no float atomics): results are bit-identical from run to run.
+ *   forward : xn = feat / max(||feat||, 1e-12) (inv_norm[b] = 1 / that denominator);
+ *             bn_training: batch mean / biased variance, running stats updated with momentum and the unbiased
+ *             variance (needs B >= 2); else the running stats.  mean / rstd receive the statistics used;
+ *             dropout: keep element i when a Philox4x32-10 uniform (seed, subsequence i / 4, offset) is < 1 - p,
+ *             mask[i] = keep, xd = keep * x / (1 - p);
+ *             logits = fc_in . W^T + bias with fc_in the output of the last stage that is on.
+ *   backward: from dlogits: dW / dbias / dgamma / dbeta accumulate (+=); dx is a [B, fs] scratch buffer;
+ *             dfeat (may be NULL: no gradient to the backbone) receives d/dfeat. */
+typedef struct {
+  int B, fs, ncls;
+  int l2norm, bn, bn_training, dropout;
+  float p, momentum, eps;
+  unsigned long long seed, offset;
+  const float* feat;                                    /* [B, fs] */
+  float* xn; float* inv_norm;                           /* [B, fs], [B] */
+  float* xb; float* mean; float* rstd;                  /* [B, fs], [fs], [fs] */
+  const float* gamma; const float* beta; float* running_mean; float* running_var;   /* [fs] */
+  unsigned char* mask; float* xd;                       /* [B, fs] */
+  const float* W; const float* bias; float* logits;     /* [ncls, fs] (nn.Linear.weight), [ncls], [B, ncls] */
+  const float* dlogits;                                 /* [B, ncls] */
+  float* dW; float* dbias; float* dgamma; float* dbeta; /* accumulated */
+  float* dx; float* dfeat;                              /* [B, fs] */
+} coclr_cls_head_t;
+int coclr_cls_head_fwd(const coclr_cls_head_t* h, coclr_stream_t stream);
+int coclr_cls_head_bwd(const coclr_cls_head_t* h, coclr_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
