@@ -285,23 +285,6 @@ COCLR_DEVINL void wgmma_stage(float (&acc)[16 * kChunks], const uint64_t (&ad)[3
   }
 }
 
-// Writes 32-column chunk c of a warpgroup's accumulator into rows [64 wg, 64 wg + 64) of a [128][pitch] fp32 tile, so
-// that lane i of warp w can afterwards read row 32 w + i (the row-per-lane view the epilogues work on).
-template <int kChunks>
-COCLR_DEVINL void acc_chunk_to_smem(const float (&acc)[16 * kChunks], int c, float* tile, int pitch, int wg,
-                                    int tid_in_wg) {
-  const int row0 = 64 * wg + 16 * (tid_in_wg >> 5) + ((tid_in_wg & 31) >> 2);
-  const int col0 = 2 * (tid_in_wg & 3);
-#pragma unroll
-  for (int cc = 0; cc < kChunks; ++cc) {
-    if (cc == c) {
-#pragma unroll
-      for (int r = 0; r < 16; ++r)
-        tile[(row0 + 8 * ((r >> 1) & 1)) * pitch + col0 + 8 * (r >> 2) + (r & 1)] = acc[16 * cc + r];
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------------
 // misc
 // ---------------------------------------------------------------------------------------------

@@ -12,11 +12,15 @@
 //  * producer warps only generate addresses: 16-byte cp.async (LDGSTS) copies with hardware zero-fill for
 //    padding land 128 pixels x 64 K-elements straight in 128B-swizzled shared-memory tiles; weights arrive
 //    pre-split and pre-swizzled through one bulk (TMA-engine) copy per stage;
-//  * two consumer warpgroups (64 pixel rows each) issue wgmma (M=64, N<=128, K=16) for the three products
-//    hi*lo, lo*hi, hi*hi into one fp32 register accumulator (fp32-equivalent result), or hi*hi only in
-//    single-pass mode;
-//  * the accumulator goes through shared memory 32 columns at a time; four of the consumer warps then make
-//    coalesced stores and accumulate the per-channel sum / sum-of-squares that train-mode BatchNorm needs.
+//  * two consumer warpgroups (64 pixel rows each) issue one wgmma m64 x BN x k16 (BN fixed at compile time) per product
+//    and K step for the three products hi*lo, lo*hi, hi*hi (fp32-equivalent result), or hi*hi only in single-pass
+//    mode.  Each 64-deep K chunk (a pipeline stage) is summed in a fresh register block and added to the fp32
+//    accumulator; the next stage is issued before that add, so one stage is always in flight;
+//  * the epilogue is the TMA kernel's (ConvEpilogue, conv_tma.h): the output tile is 128 consecutive flat rows of a
+//    2-D output tensor map [N, M], stored with bulk-tensor stores; the per-channel sum / sum-of-squares that
+//    train-mode BatchNorm needs are summed from the staged tile into per-block fp32 column tables (kStatTable).
+#include <string.h>
+
 #include "common.cuh"
 #include "coclr_b200.h"
 #include "conv_tma.h"
@@ -28,13 +32,18 @@ static constexpr int kChunkK = 64;      // K elements per pipeline stage (one 12
 static constexpr int kProducerWarps = 8;       // weight-gradient kernel: 256 threads gather 64 rows x 2 operands
 static constexpr int kFwdProducerWarps = 4;    // forward / dgrad kernel: 128 threads gather 128 rows
 static constexpr int kMmaWarps = 8;     // two consumer warpgroups: MMA, then the epilogue
-static constexpr int kEpiWarps = 4;     // consumer warps that store a tile (32 rows each)
 static constexpr int kMaxBN = 128;      // output columns per tile (register accumulator: 64 fp32 per thread)
 static constexpr int kAccChunks = kMaxBN / 32;
-// warp roles: [0,8) MMA + epilogue, [8,12) producers, 12 weight loader
-static constexpr int kThreads = (kMmaWarps + kFwdProducerWarps + 1) * 32;
+// forward / dgrad kernel, three warpgroups: 0 producers (gather, and one elected thread also copies the weights),
+// 1-2 MMA + epilogue
+static constexpr int kThreads = (kFwdProducerWarps + kMmaWarps) * 32;
 static constexpr int kWgradThreads = (kMmaWarps + kProducerWarps) * 32;
-static constexpr int kStagePitch = 33;  // floats per staged row (conflict-free transpose)
+// 128 x 40 + 256 x 232 = 384 x 168, the registers the CTA is given (setmaxnreg only moves them between warpgroups): a
+// BN = 128 consumer holds the accumulator and two fresh blocks (3 x 64); the producers read their 8 rows' coordinates
+// from shared memory (RowsShared)
+static constexpr uint32_t kProducerRegs = 40, kMmaRegs = 232;
+static_assert(kFwdProducerWarps * 32 * kProducerRegs + kMmaWarps * 32 * kMmaRegs <= 384 * 168, "register budget");
+static constexpr uint32_t kRowsBar = kConvEpiBarEnd + 1;   // named barrier of the producer warpgroup
 static constexpr int kMaxStages = 6;
 
 // Decompose destination pixel m into the source-space base coordinates used by the gather.
@@ -108,10 +117,30 @@ COCLR_DEVINL void tap_advance(TapPos& p, const coclr_src_t& S, const coclr_geom_
   }
 }
 
-template <bool kLo, int NI, int kRowStride = 32>
+// Source-space base coordinates (b, t, y, x) of the gathered rows, b < 0 for rows past the end: four registers per row, or
+// one shared-memory table entry per row with two 16-bit fields per word (t:b, y:x), filled once per tile.
+struct RowsPlain {
+  const int *b, *t, *y, *x;
+  COCLR_DEVINL void get(int i, int& bi, int& ti, int& yi, int& xi) const { bi = b[i]; ti = t[i]; yi = y[i]; xi = x[i]; }
+};
+template <int kStride>
+struct RowsShared {
+  const int2* tab;   // this thread's first row; row i at tab[kStride * i]
+  COCLR_DEVINL static int2 pack(int b, int t, int y, int x) {
+    return make_int2((int)(((uint32_t)t << 16) | ((uint32_t)b & 0xffffu)), (int)(((uint32_t)y << 16) | ((uint32_t)x & 0xffffu)));
+  }
+  COCLR_DEVINL void get(int i, int& bi, int& ti, int& yi, int& xi) const {
+    const int2 v = tab[kStride * i];
+    bi = (v.x << 16) >> 16;   // arithmetic shifts sign-extend both fields
+    ti = v.x >> 16;
+    yi = v.y >> 16;
+    xi = (v.y << 16) >> 16;
+  }
+};
+
+template <bool kLo, int NI, int kRowStride = 32, class Rows>
 COCLR_DEVINL void gather_block_async(const coclr_src_t& S, const coclr_geom_t& G, int Kreal, const TapPos& tp, int ck,
-                                     int r0, const int* rb, const int* rt, const int* ry, const int* rx,
-                                     uint32_t blk_hi, uint32_t blk_lo) {
+                                     int r0, const Rows& rows, uint32_t blk_hi, uint32_t blk_lo) {
   // This runs once per (row, K chunk) in warps that share their issue slots with everything else on the SM: for
   // narrow layers (N <= 64) the MMAs of a chunk take ~600 cycles, so the address arithmetic is kept to 32-bit pixel
   // indices (host side guarantees B*T*H*W < 2^31) and one widening multiply per row.
@@ -122,22 +151,24 @@ COCLR_DEVINL void gather_block_async(const coclr_src_t& S, const coclr_geom_t& G
   const int HW = S.H * S.W;
 #pragma unroll
   for (int i = 0; i < NI; ++i) {
-    bool in = kvalid && rb[i] >= 0;
+    int rb, rt, ry, rx;
+    rows.get(i, rb, rt, ry, rx);
+    bool in = kvalid && rb >= 0;
     int ts, ys, xs;
     if (!G.transposed) {
-      ts = rt[i] + ta;
-      ys = ry[i] + ya;
-      xs = rx[i] + xa;
+      ts = rt + ta;
+      ys = ry + ya;
+      xs = rx + xa;
     } else {
-      ts = rt[i] - ta;
-      ys = ry[i] - ya;
-      xs = rx[i] - xa;
+      ts = rt - ta;
+      ys = ry - ya;
+      xs = rx - xa;
       if (G.st == 2) { in = in && !(ts & 1); ts >>= 1; }   // arithmetic shifts keep negatives negative
       if (G.sh == 2) { in = in && !(ys & 1); ys >>= 1; }
       if (G.sw == 2) { in = in && !(xs & 1); xs >>= 1; }
     }
     in = in && ((unsigned)ts < (unsigned)S.T) && ((unsigned)ys < (unsigned)S.H) && ((unsigned)xs < (unsigned)S.W);
-    const int pix = in ? (rb[i] * S.T + ts) * HW + ys * S.W + xs : 0;
+    const int pix = in ? (rb * S.T + ts) * HW + ys * S.W + xs : 0;
     const size_t off = (size_t)(unsigned)pix * (unsigned)S.ld;
     const uint32_t dst = swz128_offset((uint32_t)(r0 + kRowStride * i), (uint32_t)ck);
     const uint32_t nbytes = in ? 16u : 0u;
@@ -154,35 +185,33 @@ struct ConvSmemLayout {
   uint32_t b_bytes;      // per copy
   uint32_t stage_bytes;  // all copies of A and B of one stage
   uint32_t stages;
-  uint32_t off_stage;    // [128 rows][kStagePitch] fp32: one 32-column chunk of the accumulator for the epilogue
-  uint32_t off_stats;    // float [epilogue warps][2][n_tiles*BN + 4]: per-warp BN-statistic partial sums
+  uint32_t stage_bufs;   // epilogue staging buffers per 32-row block (ConvOut::stage_bufs)
+  uint32_t off_stage;    // epilogue staging: 4 blocks x stage_bufs x kConvStageBytes
+  uint32_t off_stats;    // float [4 blocks][2][stat_table_cols + 4]: per-block BN-statistic column sums (ConvEpilogue)
   uint32_t off_bars;
+  uint32_t off_rows;     // int2 [128]: packed source coordinates of the tile's rows (producers)
   uint32_t total;
 };
-
-// per-warp BatchNorm statistic tables cover all output channels when those are few (flushed once per CTA), else one
-// N-tile (flushed after every tile: wide layers -- ResNet2d3d-50 has up to 2048 channels -- have few pixel tiles)
-static constexpr int kStatTableMaxCols = 512;
-__host__ __device__ inline int stat_table_cols(int BN, int n_tiles) {
-  return n_tiles * BN <= kStatTableMaxCols ? n_tiles * BN : BN;
-}
 
 __host__ __device__ inline ConvSmemLayout conv_smem_layout(int BN, int n_tiles, int npass, int want_stats) {
   ConvSmemLayout L;
   const uint32_t copies = npass > 1 ? 2u : 1u;
   L.a_bytes = kTileM * 128u;
   L.b_bytes = (uint32_t)BN * 128u;
-  L.stage_bytes = copies * (L.a_bytes + L.b_bytes);
-  const uint32_t stat_bytes = want_stats ? kEpiWarps * 2u * (uint32_t)(stat_table_cols(BN, n_tiles) + 4) * 4u : 0u;
-  const uint32_t fixed = kEpiWarps * 32u * kStagePitch * 4u + stat_bytes + 256u;
-  const uint32_t budget = 227u * 1024u - 1024u /*alignment slack*/ - fixed;
-  uint32_t st = budget / L.stage_bytes;
-  if (st > (uint32_t)kMaxStages) st = kMaxStages;
-  L.stages = st;
+  L.stage_bytes = copies * (L.a_bytes + L.b_bytes);   // a multiple of 1024: every stage starts on a swizzle atom
+  const uint32_t stat_bytes = want_stats ? 4u * 2u * (uint32_t)(stat_table_cols(BN, n_tiles) + 4) * 4u : 0u;
+  const uint32_t budget =
+      227u * 1024u - 1024u /*alignment slack*/ - 256u /*barriers*/ - kTileM * 8u /*rows*/ - ((stat_bytes + 15u) & ~15u);
+  // double-buffered staging unless a single buffer buys one more stage
+  const uint32_t st1 = min((budget - 4u * kConvStageBytes) / L.stage_bytes, (uint32_t)kMaxStages);
+  const uint32_t st2 = min((budget - 8u * kConvStageBytes) / L.stage_bytes, (uint32_t)kMaxStages);
+  L.stage_bufs = st1 > st2 ? 1u : 2u;
+  L.stages = st1 > st2 ? st1 : st2;
   L.off_stage = L.stages * L.stage_bytes;
-  L.off_stats = L.off_stage + kEpiWarps * 32u * kStagePitch * 4u;
-  L.off_bars = (L.off_stats + stat_bytes + 15u) & ~15u;
-  L.total = L.off_bars + 256u + 1024u;
+  L.off_stats = L.off_stage + 4u * L.stage_bufs * kConvStageBytes;
+  L.off_bars = L.off_stats + ((stat_bytes + 15u) & ~15u);
+  L.off_rows = L.off_bars + 256u;
+  L.total = L.off_rows + kTileM * 8u + 1024u;
   return L;
 }
 
@@ -205,55 +234,59 @@ COCLR_DEVINL uint64_t zero_chunk_mask(const coclr_conv_t& P, int nkc, int m_tile
   return mask;
 }
 
-template <int kNPass>
-__global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const coclr_conv_t P) {
+template <int kNPass, int kBN, bool kBf16>
+__global__ void __launch_bounds__(kThreads, 1)
+    conv_igemm_kernel(const __grid_constant__ CUtensorMap map_out, const __grid_constant__ coclr_conv_t P,
+                      const __grid_constant__ ConvOut O) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr bool kLo = kNPass > 1;
+  constexpr uint32_t kCopies = kLo ? 2u : 1u;
   const int M = P.B * P.Td * P.Hd * P.Wd;
   const int nkc = (P.Kreal + kChunkK - 1) / kChunkK;
   const int m_tiles = (M + kTileM - 1) / kTileM;
   const int total_tiles = m_tiles * P.n_tiles;
-  const ConvSmemLayout L = conv_smem_layout(P.BN, P.n_tiles, kNPass, P.stats_sum != nullptr);
+  const ConvSmemLayout L = conv_smem_layout(kBN, P.n_tiles, kNPass, P.stats_sum != nullptr);
   const uint32_t nstages = L.stages;
-
-  float* stage_buf = reinterpret_cast<float*>(smem + L.off_stage);
-  float* wstats = reinterpret_cast<float*>(smem + L.off_stats);
-  const bool stats_per_tile = P.n_tiles * P.BN > kStatTableMaxCols;
-  const int stat_cols = stat_table_cols(P.BN, P.n_tiles) + 4;
+  const uint32_t smem_base = smem_u32(smem);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L.off_bars);  // [kMaxStages]
   uint64_t* empty_bar = full_bar + kMaxStages;                           // [kMaxStages]
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);   // provably warp-uniform role branches for ptxas
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kMaxStages; ++s) {
-      mbar_init(&full_bar[s], kFwdProducerWarps * 32 + 1);  // every producer thread (async, via cp.async) + the weight loader
-      mbar_init(&empty_bar[s], kMmaWarps);               // one arrival per consumer warp
+      mbar_init(&full_bar[s], kFwdProducerWarps * 32 + 1);  // every producer thread (async, via cp.async) + the weight copy
+      mbar_init(&empty_bar[s], kMmaWarps * 32);              // one arrival per consumer thread
     }
     mbar_fence_init();
   }
+  float* stat_tab = reinterpret_cast<float*>(smem + L.off_stats);
   if (P.stats_sum != nullptr) {
-    for (int i = threadIdx.x; i < kEpiWarps * 2 * stat_cols; i += kThreads) wstats[i] = 0.f;
+    for (int i = threadIdx.x; i < 4 * 2 * (stat_table_cols(kBN, P.n_tiles) + 4); i += kThreads) stat_tab[i] = 0.f;
   }
   __syncthreads();
 
-  if (warp >= kMmaWarps && warp < kMmaWarps + kFwdProducerWarps) {
-    // ===================== A-operand producers (address generation + cp.async only) =====================
-    const int pt = threadIdx.x - kMmaWarps * 32;  // 0..127
+  if (warp < kFwdProducerWarps) {
+    // ===================== producers: A gather (address generation + cp.async only), weight bulk copy =====================
+    setmaxnreg_dec<kProducerRegs>();
+    const int pt = threadIdx.x;   // 0..127
     const int ck = pt & 7;
     const int r0 = pt >> 3;  // 0..15; rows r0 + 16*i
-    const uint32_t smem_base = smem_u32(smem);
+    int2* rows_tab = reinterpret_cast<int2*>(smem + L.off_rows);
+    const RowsShared<16> rows{rows_tab + r0};
     uint32_t stage = 0, phase = 0;
-    const TapPos tap0 = tap_of(P.src, P.g, ck * 8);  // this thread's K granule in chunk 0 (the only division)
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int m_tile = tile / P.n_tiles;
-      int rb[8], rt[8], ry[8], rx[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-        row_coords(P.g, P.Td, P.Hd, P.Wd, M, m_tile * kTileM + r0 + 16 * i, rb[i], rt[i], ry[i], rx[i]);
-      TapPos tp = tap0;
+      // the tile's row coordinates, one row per producer thread, once every producer is done with the last tile's
+      named_bar_sync(kRowsBar, kFwdProducerWarps * 32);
+      {
+        int b, t, y, x;
+        row_coords(P.g, P.Td, P.Hd, P.Wd, M, m_tile * kTileM + pt, b, t, y, x);
+        rows_tab[pt] = RowsShared<16>::pack(b, t, y, x);
+      }
+      named_bar_sync(kRowsBar, kFwdProducerWarps * 32);
+      TapPos tp = tap_of(P.src, P.g, ck * 8);  // this thread's K granule in chunk 0 (the only division)
       const uint64_t zmask = zero_chunk_mask(P, nkc, m_tile);
       for (int kc = 0; kc < nkc; ++kc) {
         if ((zmask >> kc) & 1ull) {
@@ -262,186 +295,97 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const coclr_con
         }
         mbar_wait(&empty_bar[stage], phase ^ 1u);
         const uint32_t sa = smem_base + stage * L.stage_bytes;
-        gather_block_async<kLo, 8, 16>(P.src, P.g, P.Kreal, tp, ck, r0, rb, rt, ry, rx, sa, sa + L.a_bytes);
+        if (warp == 0 && elect_one()) {
+          const int n_tile = tile - m_tile * P.n_tiles;
+          const uint8_t* src =
+              reinterpret_cast<const uint8_t*>(P.wpk) + ((size_t)n_tile * nkc + kc) * (size_t)(2u * L.b_bytes);
+          mbar_arrive_expect_tx(&full_bar[stage], kCopies * L.b_bytes);
+          bulk_g2s(smem + stage * L.stage_bytes + kCopies * L.a_bytes, src, kCopies * L.b_bytes, &full_bar[stage]);
+        }
+        gather_block_async<kLo, 8, 16>(P.src, P.g, P.Kreal, tp, ck, r0, rows, sa, sa + L.a_bytes);
         tap_advance(tp, P.src, P.g, kChunkK);
         // asynchronous arrival when this thread's copies have landed: the producer never waits for data
         cp_async_mbar_arrive_noinc(&full_bar[stage]);
         if (++stage == nstages) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp == kMmaWarps + kFwdProducerWarps) {
-    // ===================== weight loader (bulk copies) =====================
-    if (elect_one()) {
-      const uint32_t copies = kLo ? 2u : 1u;
-      const uint32_t bytes = copies * L.b_bytes;
-      uint32_t stage = 0, phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int n_tile = tile % P.n_tiles;
-        const uint64_t zmask = zero_chunk_mask(P, nkc, tile / P.n_tiles);
-        for (int kc = 0; kc < nkc; ++kc) {
-          if ((zmask >> kc) & 1ull) continue;
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          uint8_t* sb = smem + stage * L.stage_bytes + copies * L.a_bytes;
-          const uint8_t* src =
-              reinterpret_cast<const uint8_t*>(P.wpk) + ((size_t)n_tile * nkc + kc) * (size_t)(2u * L.b_bytes);
-          mbar_arrive_expect_tx(&full_bar[stage], bytes);
-          bulk_g2s(sb, src, bytes, &full_bar[stage]);
-          if (++stage == nstages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp < kMmaWarps) {
-    // ===================== MMA (two warpgroups of 64 rows), then the epilogue =====================
-    const int wg = warp >> 2;
-    const int tid_wg = threadIdx.x & 127;
-    const bool bf16 = P.a_bf16 != 0;
-    const uint32_t a_row_off = (uint32_t)wg * 64u * 128u;   // this warpgroup's 64 rows of the A tile
-    float* my_stage = stage_buf + warp * 32 * kStagePitch;
-    float acc[16 * kAccChunks];
+  } else {
+    setmaxnreg_inc<kMmaRegs>();
+    // ===================== consumers (warpgroups 1-2, 64 rows each): MMA, then the epilogue =====================
+    const int cwarp = warp - kFwdProducerWarps;                 // warp index among the consumers
+    const uint32_t a_row_off = (uint32_t)(cwarp >> 2) * 64u * 128u;   // this warpgroup's 64 rows of the A tile
+    float acc[kBN / 2];
     uint32_t stage = 0, phase = 0;
+    ConvEpilogue<kBN, true> epi(stat_tab);
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int m_tile = tile / P.n_tiles;
-      const int n_tile = tile % P.n_tiles;
+      const int n_tile = tile - m_tile * P.n_tiles;
       const uint64_t zmask = zero_chunk_mask(P, nkc, m_tile);
+      // Stage s + 1 (the next K chunk that zmask keeps) is issued into the other fresh block before stage s is waited
+      // for, added into acc and its slot released, so one stage is always in flight.
 #pragma unroll
-      for (int i = 0; i < 16 * kAccChunks; ++i) acc[i] = 0.f;
-      for (int kc = 0; kc < nkc; ++kc) {
-        if ((zmask >> kc) & 1ull) continue;
+      for (int i = 0; i < kBN / 2; ++i) acc[i] = 0.f;
+      int kc = 0;   // the next K chunk to issue
+      // Waits for the next stage's operands and issues it into t; rel = its slot.  Returns false after the last stage.
+      auto issue = [&](float (&t)[kBN / 2], uint32_t& rel) -> bool {
+        if (zmask != 0ull && kc < nkc) {   // first chunk >= kc that zmask keeps (zmask != 0 only when nkc <= 64)
+          const uint64_t keep = ~zmask & (~0ull << kc);
+          kc = keep != 0ull ? __ffsll((long long)keep) - 1 : nkc;
+        }
+        if (kc >= nkc) return false;
         mbar_wait_spin(&full_bar[stage], phase);
         fence_proxy_async_smem();   // cp.async (generic proxy) data -> wgmma (async proxy)
-        const uint32_t sa = smem_u32(smem + stage * L.stage_bytes);
-        const uint32_t sb = sa + (kLo ? 2u : 1u) * L.a_bytes;
+        const uint32_t sa = smem_base + stage * L.stage_bytes;
+        const uint32_t sb = sa + kCopies * L.a_bytes;
         const uint64_t a_hi = make_smem_desc(sa + a_row_off, 16, 1024);
         const uint64_t b_hi = make_smem_desc(sb, 16, 1024);
         if constexpr (kLo) {
           const uint64_t a_lo = make_smem_desc(sa + L.a_bytes + a_row_off, 16, 1024);
           const uint64_t b_lo = make_smem_desc(sb + L.b_bytes, 16, 1024);
           const uint64_t ad[3] = {a_hi, a_lo, a_hi}, bd[3] = {b_lo, b_hi, b_hi};   // small products first
-          wgmma_stage<kAccChunks, 0, 0>(acc, ad, bd, 3, 2u, 2u, 512u, P.BN, bf16);
+          wgmma_stage_issue<kBN, kBf16, 3>(t, ad, bd, 2u, 2u);
         } else {
           const uint64_t ad[3] = {a_hi, a_hi, a_hi}, bd[3] = {b_hi, b_hi, b_hi};
-          wgmma_stage<kAccChunks, 0, 0>(acc, ad, bd, 1, 2u, 2u, 512u, P.BN, bf16);
+          wgmma_stage_issue<kBN, kBf16, 1>(t, ad, bd, 2u, 2u);
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[stage]);   // this warp's reads of the stage are complete
+        rel = stage;
         if (++stage == nstages) { stage = 0; phase ^= 1u; }
+        ++kc;
+        return true;
+      };
+      // Adds a completed stage into acc and releases its slot.
+      auto retire = [&](float (&t)[kBN / 2], uint32_t rel) {
+        acc_fence(t);
+#pragma unroll
+        for (int i = 0; i < kBN / 2; ++i) acc[i] += t[i];
+        // every consumer thread arrives: an arrival under `lane == 0` would be a thread-dependent branch inside the
+        // wgmma pipeline, which ptxas answers by serialising every wgmma of the kernel
+        mbar_arrive(&empty_bar[rel]);
+      };
+      float t0[kBN / 2], t1[kBN / 2];
+      uint32_t rel0, rel1;
+      if (issue(t0, rel0)) {
+        while (true) {
+          if (!issue(t1, rel1)) {
+            wgmma_wait<0>();
+            retire(t0, rel0);
+            break;
+          }
+          wgmma_wait<1>();
+          retire(t0, rel0);
+          if (!issue(t0, rel0)) {
+            wgmma_wait<0>();
+            retire(t1, rel1);
+            break;
+          }
+          wgmma_wait<1>();
+          retire(t1, rel1);
+        }
       }
-      const int row_base = m_tile * kTileM + warp * 32;
-      const int rows_here = min(32, M - row_base);
-      // store mapping after the transpose: lane = (row group rg, column quad cq); one 16-byte store per lane covers
-      // 4 rows x 128 B per warp instruction
-      const int rg = lane >> 3, cq = lane & 7;
-#pragma unroll
-      for (int c = 0; c < kAccChunks; ++c) {
-        const int c0 = c * 32;
-        if (c0 >= P.BN) break;
-        named_bar_sync(2, kMmaWarps * 32);   // the previous chunk's readers are done with the staging tile
-        acc_chunk_to_smem<kAccChunks>(acc, c, stage_buf, kStagePitch, wg, tid_wg);
-        named_bar_sync(2, kMmaWarps * 32);
-        if (warp >= kEpiWarps) continue;
-        const int colq = n_tile * P.BN + c0 + cq * 4;  // first of this lane's 4 output channels
-        float us[4] = {1.f, 1.f, 1.f, 1.f};
-        if (P.wunscale != nullptr) {
-          const float4 u4 = __ldg(reinterpret_cast<const float4*>(P.wunscale + n_tile * P.BN + c0 + cq * 4));
-          us[0] = u4.x; us[1] = u4.y; us[2] = u4.z; us[3] = u4.w;
-        }
-        if (P.out_scale != nullptr) {
-          const float os = __ldg(P.out_scale);
-          us[0] *= os; us[1] *= os; us[2] *= os; us[3] *= os;
-        }
-        float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
-        const bool full_quad = colq + 3 < P.N;
-        if (colq < P.N) {
-          // read-modify-write destinations: issue all 8 loads of this chunk before the first store (the compiler
-          // must otherwise keep each load behind the previous store)
-          float4 old[8];
-          if (P.accumulate && full_quad) {
-#pragma unroll
-            for (int it = 0; it < 8; ++it) {
-              const int r = it * 4 + rg;
-              old[it] = (r < rows_here)
-                            ? *reinterpret_cast<const float4*>(P.dst + (size_t)(row_base + r) * P.dst_ld + P.dst_coff + colq)
-                            : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-          }
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int r = it * 4 + rg;
-            if (r < rows_here) {
-              const float* sp = my_stage + r * kStagePitch + cq * 4;
-              float4 val = make_float4(sp[0] * us[0], sp[1] * us[1], sp[2] * us[2], sp[3] * us[3]);
-              float* d = P.dst + (size_t)(row_base + r) * P.dst_ld + P.dst_coff + colq;
-              if (full_quad) {
-                if (P.accumulate) {
-                  val.x += old[it].x; val.y += old[it].y; val.z += old[it].z; val.w += old[it].w;
-                }
-                *reinterpret_cast<float4*>(d) = val;
-              } else {
-                const float vv[4] = {val.x, val.y, val.z, val.w};
-                for (int k = 0; k < 4; ++k)
-                  if (colq + k < P.N) d[k] = P.accumulate ? d[k] + vv[k] : vv[k];
-              }
-              s1[0] += val.x; s1[1] += val.y; s1[2] += val.z; s1[3] += val.w;
-              s2[0] = fmaf(val.x, val.x, s2[0]); s2[1] = fmaf(val.y, val.y, s2[1]);
-              s2[2] = fmaf(val.z, val.z, s2[2]); s2[3] = fmaf(val.w, val.w, s2[3]);
-            }
-          }
-        }
-        if (P.stats_sum != nullptr) {
-          // column sums over the warp's 32 rows: combine the 4 row groups, then one owner lane per column quad
-          // accumulates into this warp's private fp32 table (no atomics; flushed in fp64 at the end)
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            s1[k] += __shfl_xor_sync(0xffffffffu, s1[k], 8);
-            s1[k] += __shfl_xor_sync(0xffffffffu, s1[k], 16);
-            s2[k] += __shfl_xor_sync(0xffffffffu, s2[k], 8);
-            s2[k] += __shfl_xor_sync(0xffffffffu, s2[k], 16);
-          }
-          if (rg == 0 && colq < P.N) {
-            float* ws = wstats + (size_t)warp * 2 * stat_cols;
-            const int tc = stats_per_tile ? c0 + cq * 4 : colq;
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              ws[tc + k] += s1[k];
-              ws[stat_cols + tc + k] += s2[k];
-            }
-          }
-        }
-        __syncwarp();
-      }
-      if (warp < kEpiWarps && stats_per_tile && P.stats_sum != nullptr) {
-        named_bar_sync(1, kEpiWarps * 32);
-        for (int c = threadIdx.x; c < P.BN; c += kEpiWarps * 32) {
-          double a = 0.0, b = 0.0;
-#pragma unroll
-          for (int w = 0; w < kEpiWarps; ++w) {
-            float* ws = wstats + (size_t)w * 2 * stat_cols;
-            a += (double)ws[c];
-            b += (double)ws[stat_cols + c];
-            ws[c] = 0.f;
-            ws[stat_cols + c] = 0.f;
-          }
-          if (n_tile * P.BN + c < P.N) {
-            atomicAdd(&P.stats_sum[n_tile * P.BN + c], a);
-            atomicAdd(&P.stats_sq[n_tile * P.BN + c], b);
-          }
-        }
-        named_bar_sync(1, kEpiWarps * 32);
-      }
+      const int idx[4] = {m_tile, 0, 0, 0};
+      epi.tile(P, O, &map_out, smem_base + L.off_stage, acc, idx, n_tile);
     }
-    if (warp < kEpiWarps && P.stats_sum != nullptr && !stats_per_tile) {
-      named_bar_sync(1, kEpiWarps * 32);
-      for (int c = threadIdx.x; c < P.N; c += kEpiWarps * 32) {
-        double a = 0.0, b = 0.0;
-#pragma unroll
-        for (int w = 0; w < kEpiWarps; ++w) {
-          a += (double)wstats[(size_t)w * 2 * stat_cols + c];
-          b += (double)wstats[(size_t)w * 2 * stat_cols + stat_cols + c];
-        }
-        atomicAdd(&P.stats_sum[c], a);
-        atomicAdd(&P.stats_sq[c], b);
-      }
-    }
+    epi.finish(P, O, smem + L.off_stage);
   }
 }
 
@@ -558,18 +502,19 @@ __global__ void __launch_bounds__(kWgradThreads, 1) conv_wgrad_kernel(const cocl
       const uint32_t s_a = s_dy + (kLo ? 2u : 1u) * L.dy_bytes;
       // dY: 2 blocks of 64 output channels (stacked mode: block 0 = hi plane, block 1 = lo plane of channels 0..63)
       if (stack_m) {
-        gather_block_async<kLo, 2>(P.dy, ident, P.dy.C, tp_dy[0], ck, r0, qb, qt, qy, qx, s_dy, s_dy + kWgPx * 128);
+        gather_block_async<kLo, 2>(P.dy, ident, P.dy.C, tp_dy[0], ck, r0, RowsPlain{qb, qt, qy, qx}, s_dy,
+                                   s_dy + kWgPx * 128);
       } else {
 #pragma unroll
         for (int blk = 0; blk < 2; ++blk) {
-          gather_block_async<kLo, 2>(P.dy, ident, P.dy.C, tp_dy[blk], ck, r0, qb, qt, qy, qx,
+          gather_block_async<kLo, 2>(P.dy, ident, P.dy.C, tp_dy[blk], ck, r0, RowsPlain{qb, qt, qy, qx},
                                      s_dy + blk * (kWgPx * 128), s_dy + L.dy_bytes + blk * (kWgPx * 128));
         }
       }
 #pragma unroll
       for (int blk = 0; blk < kMaxBN / 64; ++blk) {
         if (blk < BNk / 64)
-          gather_block_async<kLo, 2>(P.src, P.g, Kreal, tp_a[blk], ck, r0, rb, rt, ry, rx,
+          gather_block_async<kLo, 2>(P.src, P.g, Kreal, tp_a[blk], ck, r0, RowsPlain{rb, rt, ry, rx},
                                      s_a + blk * (kWgPx * 128), s_a + L.a_bytes + blk * (kWgPx * 128));
       }
       cp_async_mbar_arrive_noinc(&full_bar[stage]);
@@ -786,17 +731,65 @@ static bool src_ok(const coclr_src_t& s, int need_lo) {
   return true;
 }
 
-template <int NP>
+template <int kNPass, int kBN, bool kBf16>
+static int launch_conv_bn(const coclr_conv_t& P, const CUtensorMap& m_out, const ConvOut& O, int grid, uint32_t smem,
+                          cudaStream_t s) {
+  const cudaError_t e =
+      cudaFuncSetAttribute(conv_igemm_kernel<kNPass, kBN, kBf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e != cudaSuccess) return COCLR_E_LAUNCH;
+  conv_igemm_kernel<kNPass, kBN, kBf16><<<grid, kThreads, smem, s>>>(m_out, P, O);
+  return COCLR_OK;
+}
+
+// One kernel instance per (pass count, tile width, 16-bit format): the wgmma shape and type are compile-time constants.
+template <int kNPass, bool kBf16>
+static int launch_conv_np(const coclr_conv_t& P, const CUtensorMap& m_out, const ConvOut& O, int grid, uint32_t smem,
+                          cudaStream_t s) {
+  switch (P.BN) {
+    case 32: return launch_conv_bn<kNPass, 32, kBf16>(P, m_out, O, grid, smem, s);
+    case 64: return launch_conv_bn<kNPass, 64, kBf16>(P, m_out, O, grid, smem, s);
+    case 96: return launch_conv_bn<kNPass, 96, kBf16>(P, m_out, O, grid, smem, s);
+    case 128: return launch_conv_bn<kNPass, 128, kBf16>(P, m_out, O, grid, smem, s);
+    default: return COCLR_E_ARG;
+  }
+}
+
 static int launch_conv(const coclr_conv_t& P, int num_sms, cudaStream_t s) {
   const int M = P.B * P.Td * P.Hd * P.Wd;
   const int m_tiles = (M + kTileM - 1) / kTileM;
   const int total = m_tiles * P.n_tiles;
-  const ConvSmemLayout L = conv_smem_layout(P.BN, P.n_tiles, NP, P.stats_sum != nullptr);
+  const ConvSmemLayout L = conv_smem_layout(P.BN, P.n_tiles, P.npass, P.stats_sum != nullptr);
   if (L.stages < 2) return COCLR_E_ARG;
-  cudaError_t e = cudaFuncSetAttribute(conv_igemm_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total);
-  if (e != cudaSuccess) return COCLR_E_LAUNCH;
+  // the output tile is 128 consecutive flat rows: a [N, M] tensor map, rows of dst_ld fp32, 32 x 32 boxes
+  ConvOut O;
+  memset(&O, 0, sizeof(O));
+  for (int d = 0; d < 4; ++d) O.obox[d] = O.o_mul[d] = O.oext[d] = 1;
+  O.obox[0] = O.o_mul[0] = kTileM;
+  O.oext[0] = M;
+  for (int w = 0; w < 4; ++w) O.sub[w][0] = 32 * w;
+  O.n_tiles_n = P.n_tiles;
+  O.BN = P.BN;
+  O.N = P.N;
+  O.stage_bufs = (int)L.stage_bufs;
+  const uint64_t row_bytes = (uint64_t)P.dst_ld * 4u;
+  MapSpec ms;
+  memset(&ms, 0, sizeof(ms));
+  ms.base[0] = P.dst + P.dst_coff;
+  ms.elem_bytes = 4;
+  ms.dims[0] = (uint64_t)P.N; ms.dims[1] = (uint64_t)M; ms.dims[2] = ms.dims[3] = ms.dims[4] = 1;
+  ms.strides[0] = row_bytes; ms.strides[1] = ms.strides[2] = ms.strides[3] = row_bytes * (uint64_t)M;
+  ms.box[0] = 32; ms.box[1] = 32; ms.box[2] = ms.box[3] = ms.box[4] = 1;
+  if (ms.strides[1] >= (1ull << 40)) return COCLR_E_ARG;   // tensor-map stride limit
+  CUtensorMap m_out;
+  if (!encode_map(&m_out, ms, 0, 5, /*swizzle=*/true)) return COCLR_E_LAUNCH;
   const int grid = total < num_sms ? total : num_sms;
-  conv_igemm_kernel<NP><<<grid, kThreads, L.total, s>>>(P);
+  const bool bf16 = P.a_bf16 != 0;
+  int rc;
+  if (P.npass > 1) rc = bf16 ? launch_conv_np<3, true>(P, m_out, O, grid, L.total, s)
+                             : launch_conv_np<3, false>(P, m_out, O, grid, L.total, s);
+  else rc = bf16 ? launch_conv_np<1, true>(P, m_out, O, grid, L.total, s)
+                 : launch_conv_np<1, false>(P, m_out, O, grid, L.total, s);
+  if (rc != COCLR_OK) return rc;
   return cudaGetLastError() == cudaSuccess ? COCLR_OK : COCLR_E_LAUNCH;
 }
 
@@ -811,11 +804,15 @@ extern "C" int coclr_conv_igemm(const coclr_conv_t* p, int num_sms, coclr_stream
     return COCLR_E_ARG;
   if (num_sms <= 0) return COCLR_E_ARG;
   if ((long long)p->B * p->src.T * p->src.H * p->src.W >= (1ll << 31)) return COCLR_E_ARG;  // 32-bit pixel indices
+  // 16-bit row coordinates in the gather producers (RowsShared): |b|, |t|, |y|, |x| < 2^15
+  if (p->B >= (1 << 15) || p->Td >= (1 << 14) || p->Hd >= (1 << 14) || p->Wd >= (1 << 14) || p->g.pt >= (1 << 14) ||
+      p->g.ph >= (1 << 14) || p->g.pw >= (1 << 14) || p->g.pt < 0 || p->g.ph < 0 || p->g.pw < 0)
+    return COCLR_E_ARG;
   cudaStream_t s = (cudaStream_t)stream;
   // TMA-staged kernel first (conv_tma.cu); shapes it does not cover run on the cp.async gather kernel below
   const int rc = coclr::conv_tma_try(*p, num_sms, s);
   if (rc <= 0) return rc;
-  return p->npass > 1 ? launch_conv<3>(*p, num_sms, s) : launch_conv<1>(*p, num_sms, s);
+  return launch_conv(*p, num_sms, s);
 }
 
 template <int NP>

@@ -44,8 +44,6 @@ static constexpr int kTmaMaxBN = 128;          // 64 fp32 accumulator registers 
 static constexpr uint32_t kTmaLoaderRegs = 40, kTmaMmaRegs = 232;   // 128 x 40 + 256 x 232 <= 64 Ki registers
 static constexpr int kTmaMaxASlots = 4;
 static constexpr int kTmaMaxBSlots = 4;
-static constexpr uint32_t kStageBytes = 4096;  // 32 rows x 32 fp32 columns per staging block and buffer
-static constexpr uint32_t kEpiBarEnd = 5;      // named barriers 1-4: the warp pairs of staging blocks 0-3
 // Shared memory the planner leaves unused: what the earlier epilogue's transpose tile and scale table took.  Handing it to
 // the rings would move the temporally strided stem conv to another tile shape, and with it the summation order of its
 // BatchNorm statistics; kept so that every launch runs on the tile plan it had.
@@ -58,8 +56,8 @@ struct TmaTile {
 // Work item -> tile.  Items enumerate (pixel tile, N tile) with the N tile fastest.
 COCLR_DEVINL TmaTile tma_decode(const TmaPlan& L, int item) {
   TmaTile t;
-  t.n_tile = item % L.n_tiles_n;
-  int m = item / L.n_tiles_n;
+  t.n_tile = item % L.out.n_tiles_n;
+  int m = item / L.out.n_tiles_n;
 #pragma unroll
   for (int d = 0; d < 3; ++d) {
     t.idx[d] = m % L.ntiles[d];
@@ -87,20 +85,17 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr bool kLo = kNPass > 1;
   constexpr uint32_t kPlanes = kLo ? 2u : 1u;
-  constexpr int kChunks = kBN / 32;                       // 32-column epilogue chunks
   constexpr uint32_t kBTileBytes = kPlanes * kBN * 128u;  // one K chunk of weights (hi, lo) in shared memory
   const TmaPlan& L = P.plan;
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t a_base = smem_base;
   const uint32_t b_base = smem_base + L.off_b;
-  const uint32_t stage_base = smem_base + L.off_stage;
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + L.off_bars);
   uint64_t* a_empty = a_full + kTmaMaxASlots;
   uint64_t* b_full = a_empty + kTmaMaxASlots;
   uint64_t* b_empty = b_full + kTmaMaxBSlots;
 
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);   // provably warp-uniform role branches for ptxas
-  const int lane = threadIdx.x & 31;
   const int first_item = (int)blockIdx.x;
   const int item_stride = (int)gridDim.x;
   const int n_items = L.total_tiles;
@@ -186,35 +181,12 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
     setmaxnreg_inc<kTmaMmaRegs>();
     // ===================== consumers (warps 4-11: two warpgroups of 64 rows): MMA and epilogue =====================
     const int cwarp = warp - kTmaFirstMmaWarp;               // warp index among the consumers
-    const int ct = (int)threadIdx.x - kTmaFirstMmaWarp * 32;  // thread index among the consumers
     const int wg = cwarp >> 2;
     const uint32_t a_row_off = (uint32_t)wg * 64u * 128u;   // this warpgroup's 64 rows of the slab window
-    // Staging block blk holds tile rows 32 blk .. 32 blk + 31: warps 2 blk and 2 blk + 1 (the same warpgroup) write 16
-    // rows each and share its stores and statistics.  The pair meets at its own named barrier, so neither warpgroup
-    // waits for the other between tiles.
-    const int blk = cwarp >> 1;
-    const uint32_t pair_bar = 1u + (uint32_t)blk;
-    const uint32_t frow = 16u * (uint32_t)(cwarp & 1) + ((uint32_t)lane >> 2);   // this thread's first row in the block
     float acc[kBN / 2];
     uint32_t aslot = 0, aphase = 0, bslot = 0, bphase = 0;
     if (L.b_resident) mbar_wait_spin(&b_full[0], 0);
-
-    const bool want_stats = P.stats_sum != nullptr;
-    // the bulk-tensor stores of a warp are issued, committed and waited for by ONE thread (bulk async-groups are
-    // per-thread state): elected once (elect.sync is deterministic for a given member mask)
-    const bool leader = elect_one();
-    const float oscale = P.out_scale != nullptr ? __ldg(P.out_scale) : 1.f;
-    const uint32_t my_stage = stage_base + (uint32_t)blk * (uint32_t)L.stage_bufs * kStageBytes;
-    // BatchNorm statistics (chunk c: warp 2 blk + (c & 1)): per column, sum and sum of squares of d = x - x0 in fp32,
-    // where x0 is the first value of the column this warp sees; converted exactly in double when they leave the CTA:
-    //   sum x = sum d + n x0,  sum x^2 = sum d^2 + 2 x0 sum d + n x0^2,
-    // so that var = E[x^2] - mean^2 (formed in double by the finalize step) does not lose the variance of channels whose
-    // spread is small against their mean to fp32 rounding of the raw sums (nn.BatchNorm3d is two-pass)
-    float s1[kChunks], s2[kChunks], x0[kChunks];
-    uint32_t x0_set = 0u;
-    int nrows = 0;
-#pragma unroll
-    for (int i = 0; i < kChunks; ++i) s1[i] = s2[i] = x0[i] = 0.f;
+    ConvEpilogue<kBN> epi;
     for (int item = first_item; item < n_items; item += item_stride) {
       const TmaTile t = tma_decode(L, item);
       const int ty0 = tma_first_type(L, t);
@@ -294,132 +266,9 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
           retire(t1, rel_a1, rel_b1);
         }
       }
-      // ---- epilogue: scale, stage, store, statistics ----
-      // Chunks go through the block's staging buffers in rounds: with two buffers a round holds two chunks, one per
-      // buffer, else one.  Both warps of the pair write every chunk of the round; then chunk c is stored and summed by
-      // warp 2 blk + (c & 1), so the two warps take the statistics of a round's two chunks at the same time.
-      bool valid = true;
-      int oc[4];
-      int r = blk * 32 + lane;   // row r of the tile: box-relative position (rows are in box order, dim 1 fastest)
-#pragma unroll
-      for (int d = 0; d < 4; ++d) {
-        const int ri = d < 3 ? r % L.obox[d] : r;
-        if (d < 3) r /= L.obox[d];
-        const int o = t.idx[d] * L.o_mul[d];
-        valid = valid && (o + ri < L.oext[d]);
-        oc[d] = o + L.sub[blk][d];
-      }
-      const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
-#pragma unroll
-      for (int kq = 0; kq < kChunks; ++kq) {
-        const int col0 = t.n_tile * kBN + kq * 32;
-        if (col0 < L.N) {
-          const uint32_t h = L.stage_bufs == 2 ? (uint32_t)kq & 1u : 0u;   // this chunk's buffer
-          if (h == 0u) {
-            // a round starts: the stores of the last round have read both buffers (each warp waits for its own) and
-            // both warps are done with its statistics
-            if (leader) bulk_wait_group_read<0>();
-            named_bar_sync(pair_bar, 64);
-          }
-          const uint32_t buf = my_stage + h * kStageBytes;
-          // this thread's part of the chunk, scaled by the column's weight unscale and the output scale:
-          // acc[16 kq + 4 g + 2 h + e] = row frow + 8 h, column 8 g + 2 (lane % 4) + e
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            const uint32_t cl = 8u * (uint32_t)g + 2u * ((uint32_t)lane & 3u);
-            float f0 = oscale, f1 = oscale;
-            if (P.wunscale != nullptr) {
-              f0 = __ldg(P.wunscale + col0 + cl) * oscale;
-              f1 = __ldg(P.wunscale + col0 + cl + 1) * oscale;
-            }
-#pragma unroll
-            for (int hr = 0; hr < 2; ++hr) {
-              const uint32_t row = frow + 8u * (uint32_t)hr;
-              st_shared_v2(buf + row * 128u + ((((cl >> 2) ^ row) & 7u) << 4) + ((cl & 3u) << 2),
-                           acc[16 * kq + 4 * g + 2 * hr] * f0, acc[16 * kq + 4 * g + 2 * hr + 1] * f1);
-            }
-          }
-          const bool round_end = h == 1u || L.stage_bufs == 1 || kq + 1 == kChunks || col0 + 32 >= L.N;
-          if (!round_end) continue;
-          fence_proxy_async_smem();
-          named_bar_sync(pair_bar, 64);
-#pragma unroll
-          for (int c = 0; c < kChunks; ++c) {
-            // the round's chunks: kq, and kq - 1 when kq went into the second buffer; chunk c belongs to warp c & 1
-            if (!(c == kq || (c == kq - 1 && h == 1u)) || (c & 1) != (cwarp & 1)) continue;
-            const uint32_t cbuf = my_stage + (L.stage_bufs == 2 ? (uint32_t)c & 1u : 0u) * kStageBytes;
-            const int ccol0 = t.n_tile * kBN + c * 32;
-            if (leader) {
-              if (P.accumulate) tma_reduce_add_5d(&map_out, cbuf, ccol0, oc[0], oc[1], oc[2], oc[3]);
-              else tma_store_5d(&map_out, cbuf, ccol0, oc[0], oc[1], oc[2], oc[3]);
-              bulk_commit_group();
-            }
-            if (want_stats && vmask != 0u) {
-              // lane j sums column j over the block's valid rows, reading the swizzled block back (conflict-free)
-              float a = 0.f, b = 0.f;
-              const uint32_t cchunk = (uint32_t)lane >> 2, cword = ((uint32_t)lane & 3u) << 2;
-              if (!((x0_set >> c) & 1u)) {
-                const uint32_t r0 = (uint32_t)__ffs((int)vmask) - 1u;
-                x0[c] = ld_shared_f32(cbuf + r0 * 128u + ((cchunk ^ (r0 & 7u)) << 4) + cword);
-                x0_set |= 1u << c;
-              }
-              const float xs = x0[c];
-#pragma unroll 8
-              for (uint32_t r = 0; r < 32; ++r) {
-                if ((vmask >> r) & 1u) {
-                  const float d = ld_shared_f32(cbuf + r * 128u + ((cchunk ^ (r & 7u)) << 4) + cword) - xs;
-                  a += d;
-                  b = fmaf(d, d, b);
-                }
-              }
-              s1[c] += a;
-              s2[c] += b;
-            }
-          }
-        }
-      }
-      nrows += __popc(vmask);
-      if (want_stats && L.n_tiles_n > 1) {
-#pragma unroll
-        for (int kq = 0; kq < kChunks; ++kq) {
-          const int col = t.n_tile * kBN + kq * 32 + lane;
-          if ((kq & 1) == (cwarp & 1) && col < L.N) {
-            const double n = (double)nrows, xd = (double)x0[kq];
-            atomicAdd(&P.stats_sum[col], (double)s1[kq] + n * xd);
-            atomicAdd(&P.stats_sq[col], (double)s2[kq] + xd * (2.0 * (double)s1[kq] + n * xd));
-          }
-          s1[kq] = s2[kq] = 0.f;
-        }
-        x0_set = 0u;
-        nrows = 0;
-      }
+      epi.tile(P, L.out, &map_out, smem_base + L.off_stage, acc, t.idx, t.n_tile);
     }
-    if (leader) bulk_wait_group_read<0>();
-    if (want_stats && L.n_tiles_n == 1) {
-      // combine the four blocks' column sums in shared memory (the staging blocks are free now), one fp64 atomic per
-      // channel and CTA
-      double* tab = reinterpret_cast<double*>(smem + L.off_stage);   // [4 blocks][2][128] = 8 KB of the staging blocks
-      named_bar_sync(kEpiBarEnd, kTmaMmaWarps * 32);
-#pragma unroll
-      for (int kq = 0; kq < kChunks; ++kq) {
-        if ((kq & 1) != (cwarp & 1)) continue;
-        const double n = (double)nrows, xd = (double)x0[kq];
-        tab[(blk * 2 + 0) * 128 + kq * 32 + lane] = (double)s1[kq] + n * xd;
-        tab[(blk * 2 + 1) * 128 + kq * 32 + lane] = (double)s2[kq] + xd * (2.0 * (double)s1[kq] + n * xd);
-      }
-      named_bar_sync(kEpiBarEnd, kTmaMmaWarps * 32);
-      for (int c = ct; c < L.N; c += kTmaMmaWarps * 32) {
-        double a = 0.0, b = 0.0;
-#pragma unroll
-        for (int w = 0; w < 4; ++w) {
-          a += tab[(w * 2 + 0) * 128 + c];
-          b += tab[(w * 2 + 1) * 128 + c];
-        }
-        atomicAdd(&P.stats_sum[c], a);
-        atomicAdd(&P.stats_sq[c], b);
-      }
-    }
-    if (leader) bulk_wait_group<0>();   // all global writes of this thread's bulk stores are complete
+    epi.finish(P, L.out, smem + L.off_stage);
   }
 }
 
@@ -485,9 +334,9 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
   if (g.sh != 1 || g.sw != 1) return false;
   const int planes = P.npass > 1 ? 2 : 1;
   const long ld2 = (long)S.ld * 2;
-  L.BN = P.BN;
-  L.N = P.N;
-  L.n_tiles_n = P.n_tiles;
+  L.out.BN = P.BN;
+  L.out.N = P.N;
+  L.out.n_tiles_n = P.n_tiles;
   L.nc = window ? 1 : (S.C + 63) / 64;
   L.nkc = window ? g.kh : taps * L.nc;
   L.sel_dim = -1;
@@ -516,7 +365,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
     A.box[0] = 64; A.box[1] = 128; A.box[2] = A.box[3] = A.box[4] = 1;
     O.dims[0] = P.N; O.dims[1] = M; O.dims[2] = O.dims[3] = O.dims[4] = 1;
     O.strides[0] = old4; O.strides[1] = O.strides[2] = O.strides[3] = (uint64_t)old4 * M;
-    L.oext[0] = (int)M; L.oext[1] = L.oext[2] = L.oext[3] = 1;
+    L.out.oext[0] = (int)M; L.out.oext[1] = L.out.oext[2] = L.out.oext[3] = 1;
     L.n_types = 1;
     L.type[0].nshift = 1;
     L.type[0].tap[0] = 0;
@@ -536,7 +385,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
     O.dims[0] = P.N; O.dims[1] = P.Wd; O.dims[2] = P.Hd; O.dims[3] = P.Td; O.dims[4] = P.B;
     O.strides[0] = old4; O.strides[1] = old4 * P.Wd; O.strides[2] = old4 * P.Wd * P.Hd;
     O.strides[3] = old4 * P.Wd * P.Hd * P.Td;
-    L.oext[0] = P.Wd; L.oext[1] = P.Hd; L.oext[2] = P.Td; L.oext[3] = P.B;
+    L.out.oext[0] = P.Wd; L.out.oext[1] = P.Hd; L.out.oext[2] = P.Td; L.out.oext[3] = P.B;
     L.n_types = 1;
     L.a_c0_step = 0;
     L.type[0].d[1] = -g.ph;
@@ -560,7 +409,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
     O.dims[0] = P.N; O.dims[1] = P.Wd; O.dims[2] = P.Hd; O.dims[3] = P.Td; O.dims[4] = P.B;
     O.strides[0] = old4; O.strides[1] = old4 * P.Wd; O.strides[2] = old4 * P.Wd * P.Hd;
     O.strides[3] = old4 * P.Wd * P.Hd * P.Td;
-    L.oext[0] = P.Wd; L.oext[1] = P.Hd; L.oext[2] = P.Td; L.oext[3] = P.B;
+    L.out.oext[0] = P.Wd; L.out.oext[1] = P.Hd; L.out.oext[2] = P.Td; L.out.oext[3] = P.B;
     L.n_types = g.kw;
     for (int xa = 0; xa < g.kw; ++xa) {
       TmaSlabType& t = L.type[xa];
@@ -594,7 +443,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
       A.box[0] = 64; A.box[1] = npx; A.box[2] = 1; A.box[3] = nt + g.kt - 1; A.box[4] = 1;
       O.dims[0] = P.N; O.dims[1] = oHW; O.dims[2] = 1; O.dims[3] = P.Td; O.dims[4] = P.B;
       O.strides[0] = old4; O.strides[1] = old4 * oHW; O.strides[2] = old4 * oHW; O.strides[3] = old4 * oHW * P.Td;
-      L.oext[0] = (int)oHW; L.oext[1] = 1; L.oext[2] = P.Td; L.oext[3] = P.B;
+      L.out.oext[0] = (int)oHW; L.out.oext[1] = 1; L.out.oext[2] = P.Td; L.out.oext[3] = P.B;
       L.n_types = 1;
       TmaSlabType& t = L.type[0];
       t.d[2] = tr ? g.pt - (g.kt - 1) : -g.pt;
@@ -627,7 +476,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
       A.box[0] = 64; A.box[1] = npx; A.box[2] = 1; A.box[3] = nt + maxshift - 1; A.box[4] = 1;
       O.dims[0] = P.N; O.dims[1] = oHW; O.dims[2] = 1; O.dims[3] = P.Td; O.dims[4] = P.B;
       O.strides[0] = old4; O.strides[1] = old4 * oHW; O.strides[2] = old4 * oHW; O.strides[3] = old4 * oHW * P.Td;
-      L.oext[0] = (int)oHW; L.oext[1] = 1; L.oext[2] = P.Td; L.oext[3] = P.B;
+      L.out.oext[0] = (int)oHW; L.out.oext[1] = 1; L.out.oext[2] = P.Td; L.out.oext[3] = P.B;
       L.slab_bytes = npx * (nt + maxshift - 1) * 128;
     } else if (g.st == 2 && tr) {
       // data gradient of the temporally strided conv: output frame t = 2*th + par receives dY[th + sh] * W[dt] with
@@ -657,7 +506,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
       A.box[0] = 64; A.box[1] = npx; A.box[2] = 1; A.box[3] = nt + maxshift - 1; A.box[4] = 1;
       O.dims[0] = P.N; O.dims[1] = oHW; O.dims[2] = 2; O.dims[3] = TH; O.dims[4] = P.B;
       O.strides[0] = old4; O.strides[1] = old4 * oHW; O.strides[2] = old4 * oHW * 2; O.strides[3] = old4 * oHW * P.Td;
-      L.oext[0] = (int)oHW; L.oext[1] = 2; L.oext[2] = TH; L.oext[3] = P.B;
+      L.out.oext[0] = (int)oHW; L.out.oext[1] = 2; L.out.oext[2] = TH; L.out.oext[3] = P.B;
       L.slab_bytes = npx * (nt + maxshift - 1) * 128;
     } else {
       return false;
@@ -668,20 +517,20 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
   }
   if (L.slab_bytes / 128 > 256 * 4) return false;
   for (int d = 0; d < 4; ++d) {
-    L.obox[d] = box[d];
+    L.out.obox[d] = box[d];
     L.a_mul[d] = box[d];
-    L.o_mul[d] = box[d];
+    L.out.o_mul[d] = box[d];
   }
   if (L.sel_dim >= 0) {          // parity dimension: tile index = output parity coordinate, no A coordinate
     L.a_mul[L.sel_dim] = 0;
-    L.o_mul[L.sel_dim] = 1;
+    L.out.o_mul[L.sel_dim] = 1;
   }
-  if (g.st == 2 && !tr && g.kt > 1) L.a_mul[1] = 0, L.o_mul[1] = 0;   // A parity coordinate comes from the slab type
+  if (g.st == 2 && !tr && g.kt > 1) L.a_mul[1] = 0, L.out.o_mul[1] = 0;   // A parity coordinate comes from the slab type
   long mt = 1;
   for (int d = 0; d < 4; ++d) mt *= L.ntiles[d];
-  if (mt * L.n_tiles_n >= (1l << 31)) return false;
+  if (mt * L.out.n_tiles_n >= (1l << 31)) return false;
   L.m_tiles = (int)mt;
-  L.total_tiles = (int)(mt * L.n_tiles_n);
+  L.total_tiles = (int)(mt * L.out.n_tiles_n);
   // epilogue sub-boxes: 32 consecutive tile rows form a rectangular box (all extents are powers of two)
   int sb[4], rem = 32;
   for (int d = 0; d < 4; ++d) {
@@ -694,7 +543,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
   for (int w = 0; w < 4; ++w) {
     int r = 32 * w;
     for (int d = 0; d < 4; ++d) {
-      L.sub[w][d] = r % box[d];
+      L.out.sub[w][d] = r % box[d];
       r /= box[d];
     }
   }
@@ -708,27 +557,27 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
   // ---- shared memory ----
   L.plane_stride = (L.slab_bytes + 1023) & ~1023;
   L.a_slot_bytes = planes * L.plane_stride;
-  L.b_tile_bytes = planes * L.BN * 128;
+  L.b_tile_bytes = planes * L.out.BN * 128;
   const int budget = 227 * 1024 - 1024 /*alignment slack*/ - kPlanKeepBytes - 256 /*barriers*/;
-  const int stage1 = 4 * (int)kStageBytes, stage2 = 8 * (int)kStageBytes;
+  const int stage1 = 4 * (int)kConvStageBytes, stage2 = 8 * (int)kConvStageBytes;
   const long tiles_per_cta = ((long)L.total_tiles + 131) / 132;   // one wave over the 132 SMs of an H100 SXM
   L.b_resident = 0;
   const long resident_bytes = (long)L.nkc * L.b_tile_bytes;
-  if (L.n_tiles_n == 1 && tiles_per_cta >= 2 && resident_bytes + 2l * L.a_slot_bytes + stage1 <= budget) {
+  if (L.out.n_tiles_n == 1 && tiles_per_cta >= 2 && resident_bytes + 2l * L.a_slot_bytes + stage1 <= budget) {
     L.b_resident = 1;
     L.b_slots = 0;
     long left = budget - resident_bytes;
-    L.stage_bufs = (left - stage2 >= 2l * L.a_slot_bytes) ? 2 : 1;
-    left -= L.stage_bufs == 2 ? stage2 : stage1;
+    L.out.stage_bufs = (left - stage2 >= 2l * L.a_slot_bytes) ? 2 : 1;
+    left -= L.out.stage_bufs == 2 ? stage2 : stage1;
     L.a_slots = (int)(left / L.a_slot_bytes);
     if (L.a_slots > kTmaMaxASlots) L.a_slots = kTmaMaxASlots;
     L.off_b = (uint32_t)(L.a_slots * L.a_slot_bytes);
     L.off_stage = L.off_b + (uint32_t)resident_bytes;
   } else {
-    L.stage_bufs = 2;
+    L.out.stage_bufs = 2;
     long left = budget - stage2;
     if (left < 2l * L.a_slot_bytes + 2l * L.b_tile_bytes) {
-      L.stage_bufs = 1;
+      L.out.stage_bufs = 1;
       left = budget - stage1;
       if (left < 2l * L.a_slot_bytes + 2l * L.b_tile_bytes) return false;
     }
@@ -749,12 +598,12 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
     L.off_stage = L.off_b + (uint32_t)(L.b_slots * L.b_tile_bytes);
   }
   L.off_stage = (L.off_stage + 1023u) & ~1023u;
-  L.off_bars = L.off_stage + (uint32_t)(L.stage_bufs == 2 ? stage2 : stage1);
+  L.off_bars = L.off_stage + (uint32_t)(L.out.stage_bufs == 2 ? stage2 : stage1);
   L.total = L.off_bars + 256u + 1024u;
   if (L.total > 227u * 1024u) return false;
-  if (L.stage_bufs == 1 && P.stats_sum != nullptr) {
+  if (L.out.stage_bufs == 1 && P.stats_sum != nullptr) {
     // the end-of-kernel statistics table (4 warps x 2 x 256 floats = 8 KB) lives in the staging area
-    if (4 * (int)kStageBytes < 8192) return false;
+    if (4 * (int)kConvStageBytes < 8192) return false;
   }
   return true;
 }
@@ -769,7 +618,7 @@ bool conv_tma_plan(const coclr_conv_t& P, TmaPlan& L, MapSpec& A, MapSpec& O) {
     MapSpec a, o;
     if (!conv_tma_plan_variant(P, v, l, a, o)) continue;
     const int slots = l.a_slots < 3 ? l.a_slots : 3;
-    const long score = (long)(l.stage_bufs == 2) * (1l << 40) + (long)slots * (1l << 32) + ((1l << 31) - l.slab_bytes);
+    const long score = (long)(l.out.stage_bufs == 2) * (1l << 40) + (long)slots * (1l << 32) + ((1l << 31) - l.slab_bytes);
     if (!have || score > best) {
       have = true;
       best = score;
@@ -795,7 +644,7 @@ extern "C" int coclr_conv_tma_plan(const coclr_conv_t* p, int* info) {
   MapSpec A, O;
   if (!conv_tma_plan(*p, L, A, O)) return 0;
   if (info) {
-    info[0] = L.a_slots; info[1] = L.b_slots; info[2] = L.b_resident; info[3] = L.stage_bufs;
+    info[0] = L.a_slots; info[1] = L.b_slots; info[2] = L.b_resident; info[3] = L.out.stage_bufs;
     info[4] = (int)L.total; info[5] = L.total_tiles; info[6] = L.slab_bytes; info[7] = L.n_types;
   }
   return 1;
@@ -851,10 +700,10 @@ int coclr::conv_tma_try(const coclr_conv_t& P, int num_sms, cudaStream_t stream)
   const int grid = L.total_tiles < num_sms ? L.total_tiles : num_sms;
   const bool bf16 = P.a_bf16 != 0;
   int rc;
-  if (P.npass > 1) rc = bf16 ? conv_tma_launch<3, true>(L.BN, grid, m_hi, m_lo, m_out, args, stream)
-                             : conv_tma_launch<3, false>(L.BN, grid, m_hi, m_lo, m_out, args, stream);
-  else rc = bf16 ? conv_tma_launch<1, true>(L.BN, grid, m_hi, m_lo, m_out, args, stream)
-                 : conv_tma_launch<1, false>(L.BN, grid, m_hi, m_lo, m_out, args, stream);
+  if (P.npass > 1) rc = bf16 ? conv_tma_launch<3, true>(L.out.BN, grid, m_hi, m_lo, m_out, args, stream)
+                             : conv_tma_launch<3, false>(L.out.BN, grid, m_hi, m_lo, m_out, args, stream);
+  else rc = bf16 ? conv_tma_launch<1, true>(L.out.BN, grid, m_hi, m_lo, m_out, args, stream)
+                 : conv_tma_launch<1, false>(L.out.BN, grid, m_hi, m_lo, m_out, args, stream);
   if (rc != COCLR_OK) return rc;
   return cudaGetLastError() == cudaSuccess ? COCLR_OK : COCLR_E_LAUNCH;
 }
