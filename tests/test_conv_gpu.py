@@ -241,7 +241,9 @@ def test_conv_dgrad_accumulate(diag):
 @pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
 @pytest.mark.parametrize("npass,splits", [(3, 1), (3, 5), (1, 2)])
 def test_conv_wgrad(case, npass, splits, diag):
-    """dY as bf16 planes x the bf16 twin of the activation planes (what the training step uses)."""
+    """dY as bf16 planes x the bf16 twin of the activation planes, no out_scale.  The training step's backbone runs its
+    weight gradients on fp16 planes of dY * s with out_scale = 1/s instead: test_wgrad_tma_gpu.py and
+    test_conv_bwd_scaled_gpu.py test that format."""
     ops, geom, x, w = _setup(case, seed=9)
     name, Cin, Cout, k, s, p, B, T, H, W = case
     To, Ho, Wo = geom.out_dims(T, H, W)
