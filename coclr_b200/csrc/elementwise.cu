@@ -51,18 +51,24 @@ COCLR_DEVINL float4 ld_pair4_any(const uint16_t* hi, const uint16_t* lo, size_t 
   return v;
 }
 
+// 4 values -> their (hi, lo) 16-bit pairs, 2 channels per word (the layout of the planes)
 template <bool kBf16>
-COCLR_DEVINL void st_pair4(uint16_t* hi, uint16_t* lo, size_t off, float4 v) {
+COCLR_DEVINL void pack_pair4(float4 v, uint2& h, uint2& l) {
   uint16_t h0, h1, h2, h3, l0, l1, l2, l3;
   split2<kBf16>(v.x, h0, l0);
   split2<kBf16>(v.y, h1, l1);
   split2<kBf16>(v.z, h2, l2);
   split2<kBf16>(v.w, h3, l3);
-  *reinterpret_cast<uint2*>(hi + off) =
-      make_uint2((uint32_t)h0 | ((uint32_t)h1 << 16), (uint32_t)h2 | ((uint32_t)h3 << 16));
-  if (lo != nullptr)
-    *reinterpret_cast<uint2*>(lo + off) =
-        make_uint2((uint32_t)l0 | ((uint32_t)l1 << 16), (uint32_t)l2 | ((uint32_t)l3 << 16));
+  h = make_uint2((uint32_t)h0 | ((uint32_t)h1 << 16), (uint32_t)h2 | ((uint32_t)h3 << 16));
+  l = make_uint2((uint32_t)l0 | ((uint32_t)l1 << 16), (uint32_t)l2 | ((uint32_t)l3 << 16));
+}
+
+template <bool kBf16>
+COCLR_DEVINL void st_pair4(uint16_t* hi, uint16_t* lo, size_t off, float4 v) {
+  uint2 h, l;
+  pack_pair4<kBf16>(v, h, l);
+  *reinterpret_cast<uint2*>(hi + off) = h;
+  if (lo != nullptr) *reinterpret_cast<uint2*>(lo + off) = l;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -458,7 +464,25 @@ COCLR_DEVINL int h_hi_int(uint32_t u) { return __half2int_rn(__ushort_as_half((u
 
 static constexpr uint32_t kNegInf2 = 0xfc00fc00u;  // (-inf, -inf) in fp16
 
-template <int KT, int KH, int KW, int ST, int SH, int SW>
+// Input pairs of a pool.  kBn = false: the fp16 planes x_hi / x_lo.  kBn = true (P.y != NULL): the conv output y, turned
+// into the pairs coclr_affine_split would have stored -- relu?(fma(y, scale, shift)) split by pack_pair4 -- so the
+// comparisons below see the same bits either way and the planes of y are never written.
+COCLR_DEVINL void bn_pair4(const coclr_pool_t& P, size_t off, const float4& sc, const float4& sh, uint2& h, uint2& l) {
+  float4 v = ld4(P.y + off);
+  v.x = fmaf(v.x, sc.x, sh.x);
+  v.y = fmaf(v.y, sc.y, sh.y);
+  v.z = fmaf(v.z, sc.z, sh.z);
+  v.w = fmaf(v.w, sc.w, sh.w);
+  if (P.relu) {
+    v.x = fmaxf(v.x, 0.f);
+    v.y = fmaxf(v.y, 0.f);
+    v.z = fmaxf(v.z, 0.f);
+    v.w = fmaxf(v.w, 0.f);
+  }
+  pack_pair4<false>(v, h, l);
+}
+
+template <bool kBn, int KT, int KH, int KW, int ST, int SH, int SW>
 __global__ void __launch_bounds__(256) maxpool_fwd_kernel(const coclr_pool_t P) {
   const int kt = KT ? KT : P.g.kt, kh = KH ? KH : P.g.kh, kw = KW ? KW : P.g.kw;
   const int st = ST ? ST : P.g.st, sh = SH ? SH : P.g.sh, sw = SW ? SW : P.g.sw;
@@ -476,6 +500,8 @@ __global__ void __launch_bounds__(256) maxpool_fwd_kernel(const coclr_pool_t P) 
     const int to = (int)(r % P.To);
     const int b = (int)(r / P.To);
     const int c = cg * 4;
+    float4 bn_sc, bn_sh;
+    if constexpr (kBn) { bn_sc = ld4(P.scale + c); bn_sh = ld4(P.shift + c); }
     uint32_t bh[2] = {kNegInf2, kNegInf2}, bl[2] = {0u, 0u}, bt[2] = {0u, 0u};  // best hi / lo / tap (2 ch per word)
 #pragma unroll
     for (int a = 0; a < kt; ++a) {
@@ -491,9 +517,13 @@ __global__ void __launch_bounds__(256) maxpool_fwd_kernel(const coclr_pool_t P) 
           if ((unsigned)xi >= (unsigned)P.Wi) continue;
           const uint32_t tap2 = int_h2((a * kh + bb) * kw + cc);
           const size_t off = ((((size_t)b * P.Ti + ti) * P.Hi + yi) * P.Wi + xi) * P.ldx + P.x_coff + c;
-          const uint2 h = *reinterpret_cast<const uint2*>(xh + off);
-          uint2 l = make_uint2(0u, 0u);
-          if (xl != nullptr) l = *reinterpret_cast<const uint2*>(xl + off);
+          uint2 h, l = make_uint2(0u, 0u);
+          if constexpr (kBn) {
+            bn_pair4(P, off, bn_sc, bn_sh, h, l);
+          } else {
+            h = *reinterpret_cast<const uint2*>(xh + off);
+            if (xl != nullptr) l = *reinterpret_cast<const uint2*>(xl + off);
+          }
           const uint32_t hw[2] = {h.x, h.y}, lw[2] = {l.x, l.y};
 #pragma unroll
           for (int p = 0; p < 2; ++p) {
@@ -740,6 +770,7 @@ __global__ void __launch_bounds__(256) maxpool333_smem_kernel(const coclr_pool_t
 // every thread (output row, output column, 8 channels) reduces its 9 taps from shared memory.  An input element leaves
 // L2 ~1.1 times instead of 2.25 times, in 16-byte instead of 8-byte requests.
 static constexpr int kPool133TY = 4;
+template <bool kBn>
 __global__ void __launch_bounds__(256) maxpool133s2_smem_kernel(const coclr_pool_t P) {
   extern __shared__ __align__(16) uint8_t pool_smem[];
   const int W = P.Wi, H = P.Hi, Wo = P.Wo, Ho = P.Ho;
@@ -767,22 +798,44 @@ __global__ void __launch_bounds__(256) maxpool133s2_smem_kernel(const coclr_pool
     *reinterpret_cast<uint4*>(pool_smem + (size_t)(ry * WP) * 32 + part * 16) = make_uint4(kNegInf2, kNegInf2, kNegInf2, kNegInf2);
     *reinterpret_cast<uint4*>(pool_smem + (size_t)plane_px * 32 + (size_t)(ry * WP) * 32 + part * 16) = make_uint4(0u, 0u, 0u, 0u);
   }
-  const int nchunk = rows * W * 4;                          // rows x image columns x (hi0, hi1, lo0, lo1)
-  for (int i = tid; i < nchunk; i += blockDim.x) {
-    const int part = i & 3, px = (i >> 2) % W, ry = (i >> 2) / W;
-    const int yi = yi0 + ry;
-    const uint32_t dst = (part >> 1) * (uint32_t)plane_px * 32u + (uint32_t)(ry * WP + px + 1) * 32u + (part & 1) * 16u;
-    const uint16_t* src = (part >> 1) ? xl : xh;
-    if ((unsigned)yi < (unsigned)H && src != nullptr) {
-      const size_t goff = ((((size_t)b * P.Ti + t) * H + yi) * W + px) * P.ldx + P.x_coff + c0 + (part & 1) * 8;
-      cp_async16(sbase + dst, src + goff, 16u);
-    } else {
-      const uint32_t v = (part >> 1) ? 0u : kNegInf2;
-      *reinterpret_cast<uint4*>(pool_smem + dst) = make_uint4(v, v, v, v);
+  if constexpr (kBn) {
+    // rows x image columns x 2 channel octets: 32 bytes of y -> 16 bytes of hi and 16 of lo
+    const int nchunk = rows * W * 2;
+    for (int i = tid; i < nchunk; i += blockDim.x) {
+      const int part = i & 1, px = (i >> 1) % W, ry = (i >> 1) / W;
+      const int yi = yi0 + ry;
+      const uint32_t dst = (uint32_t)(ry * WP + px + 1) * 32u + part * 16u;
+      uint4 hv = make_uint4(kNegInf2, kNegInf2, kNegInf2, kNegInf2), lv = make_uint4(0u, 0u, 0u, 0u);
+      if ((unsigned)yi < (unsigned)H) {
+        const int c = c0 + part * 8;
+        const size_t goff = ((((size_t)b * P.Ti + t) * H + yi) * W + px) * P.ldx + P.x_coff + c;
+        uint2 h0, l0, h1, l1;
+        bn_pair4(P, goff, ld4(P.scale + c), ld4(P.shift + c), h0, l0);
+        bn_pair4(P, goff + 4, ld4(P.scale + c + 4), ld4(P.shift + c + 4), h1, l1);
+        hv = make_uint4(h0.x, h0.y, h1.x, h1.y);
+        lv = make_uint4(l0.x, l0.y, l1.x, l1.y);
+      }
+      *reinterpret_cast<uint4*>(pool_smem + dst) = hv;
+      *reinterpret_cast<uint4*>(pool_smem + (size_t)plane_px * 32 + dst) = lv;
     }
+  } else {
+    const int nchunk = rows * W * 4;                          // rows x image columns x (hi0, hi1, lo0, lo1)
+    for (int i = tid; i < nchunk; i += blockDim.x) {
+      const int part = i & 3, px = (i >> 2) % W, ry = (i >> 2) / W;
+      const int yi = yi0 + ry;
+      const uint32_t dst = (part >> 1) * (uint32_t)plane_px * 32u + (uint32_t)(ry * WP + px + 1) * 32u + (part & 1) * 16u;
+      const uint16_t* src = (part >> 1) ? xl : xh;
+      if ((unsigned)yi < (unsigned)H && src != nullptr) {
+        const size_t goff = ((((size_t)b * P.Ti + t) * H + yi) * W + px) * P.ldx + P.x_coff + c0 + (part & 1) * 8;
+        cp_async16(sbase + dst, src + goff, 16u);
+      } else {
+        const uint32_t v = (part >> 1) ? 0u : kNegInf2;
+        *reinterpret_cast<uint4*>(pool_smem + dst) = make_uint4(v, v, v, v);
+      }
+    }
+    cp_async_commit();
+    cp_async_wait<0>();
   }
-  cp_async_commit();
-  cp_async_wait<0>();
   __syncthreads();
   const int cq = tid & 1, xo = (tid >> 1) % Wo, yl_ = (tid >> 1) / Wo;     // blockDim = 2 * Wo * kPool133TY
   const int yo = yo0 + yl_;
@@ -1153,7 +1206,8 @@ extern "C" int coclr_bn_finalize(const coclr_bn_finalize_t* p, coclr_stream_t st
 }
 
 extern "C" int coclr_affine_split(const coclr_split_t* p, int num_sms, coclr_stream_t stream) {
-  if (!p || !p->x || !p->hi || p->C % 4 || p->ld % 4 || p->coff % 4 || p->out_ld % 4 || p->out_coff % 4)
+  if (!p || !p->x || (!p->hi && !p->bn.scale) || p->C % 4 || p->ld % 4 || p->coff % 4 || p->out_ld % 4 ||
+      p->out_coff % 4)
     return COCLR_E_ARG;
   if (p->res_hi && (p->res_ld % 4 || p->res_coff % 4)) return COCLR_E_ARG;
   const long total = p->M * (p->C / 4);
@@ -1161,6 +1215,14 @@ extern "C" int coclr_affine_split(const coclr_split_t* p, int num_sms, coclr_str
     const coclr_bn_finalize_t& f = p->bn;
     if (!f.shift || !f.gamma || !f.beta || !f.running_mean || !f.running_var || p->C > kMaxBnC) return COCLR_E_ARG;
     if (f.training && (!f.sum || !f.sumsq || f.count <= 0)) return COCLR_E_ARG;
+    if (!p->hi) {
+      // no planes: the finalize alone, by the same kernel over zero rows, so that scale / shift / the running stats
+      // carry the same bits as when the planes are written
+      coclr_split_t q = *p;
+      q.M = 0;
+      bn_apply_split_kernel<false><<<1, 256, 0, (cudaStream_t)stream>>>(q);
+      return LAUNCH_OK();
+    }
     const int grid = grid_for(total, 256, num_sms * 16);
     if (p->bf16)
       bn_apply_split_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(*p);
@@ -1205,16 +1267,12 @@ extern "C" int coclr_bias_relu_bwd(const float* h, const float* bias, float* dA,
   return LAUNCH_OK();
 }
 
-template <bool kBwd>
-static void launch_pool(const coclr_pool_t& p, long total, cudaStream_t s) {
+static void launch_pool_bwd(const coclr_pool_t& p, long total, cudaStream_t s) {
   const int grid = grid_for(total, 256, 148 * 32);
   const coclr_geom_t& g = p.g;
 #define POOL_CASE(KT, KH, KW, ST, SH, SW)                                                 \
   if (g.kt == KT && g.kh == KH && g.kw == KW && g.st == ST && g.sh == SH && g.sw == SW) { \
-    if (kBwd)                                                                             \
-      maxpool_bwd_kernel<KT, KH, KW, ST, SH, SW><<<grid, 256, 0, s>>>(p);                 \
-    else                                                                                  \
-      maxpool_fwd_kernel<KT, KH, KW, ST, SH, SW><<<grid, 256, 0, s>>>(p);                 \
+    maxpool_bwd_kernel<KT, KH, KW, ST, SH, SW><<<grid, 256, 0, s>>>(p);                   \
     return;                                                                               \
   }
   POOL_CASE(1, 3, 3, 1, 2, 2)
@@ -1222,41 +1280,70 @@ static void launch_pool(const coclr_pool_t& p, long total, cudaStream_t s) {
   POOL_CASE(3, 3, 3, 2, 2, 2)
   POOL_CASE(2, 2, 2, 2, 2, 2)
 #undef POOL_CASE
-  if (kBwd)
-    maxpool_bwd_kernel<0, 0, 0, 0, 0, 0><<<grid, 256, 0, s>>>(p);
-  else
-    maxpool_fwd_kernel<0, 0, 0, 0, 0, 0><<<grid, 256, 0, s>>>(p);
+  maxpool_bwd_kernel<0, 0, 0, 0, 0, 0><<<grid, 256, 0, s>>>(p);
+}
+
+// Windows the conv-output form (P.y) is instantiated for: the stage pools of S3D and the ResNet stem pool,
+// (1,3,3)/(1,2,2), (3,3,3)/2 and (2,2,2)/2 (any padding).
+static bool bn_pool_geometry(const coclr_geom_t& g) {
+  return (g.kt == 1 && g.kh == 3 && g.kw == 3 && g.st == 1 && g.sh == 2 && g.sw == 2) ||
+         (g.kt == 3 && g.kh == 3 && g.kw == 3 && g.st == 2 && g.sh == 2 && g.sw == 2) ||
+         (g.kt == 2 && g.kh == 2 && g.kw == 2 && g.st == 2 && g.sh == 2 && g.sw == 2);
+}
+
+// kBn = false: pool the planes; kBn = true: pool straight from the conv output.  The 3x3x3/s1 kernels serve only the
+// planes (the Inception branch-3 pools, whose input also feeds convolutions).
+template <bool kBn>
+static void launch_pool_fwd(const coclr_pool_t& p, cudaStream_t s) {
+  const coclr_geom_t& g = p.g;
+  const long total = (long)p.B * p.To * p.Ho * p.Wo * (p.C / 4);
+  if (!kBn && g.kt == 3 && g.kh == 3 && g.kw == 3 && g.st == 1 && g.sh == 1 && g.sw == 1 && g.pt == 1 && g.ph == 1 &&
+      g.pw == 1 && (p.Wo % 4) == 0 && p.Wo == p.Wi && p.Ho == p.Hi && p.To == p.Ti) {
+    const int threads = 2 * p.Wi * kPoolTY;
+    if (p.Wi >= 8 && threads <= 256 && p.C % 16 == 0 && p.x_coff % 8 == 0 && p.y_coff % 8 == 0 && p.ldx % 8 == 0 &&
+        p.ldy % 8 == 0) {
+      const size_t smem = (size_t)3 * (kPoolTY + 2) * (p.Wi + 2) * 64;
+      const int grid = p.B * ((p.Hi + kPoolTY - 1) / kPoolTY) * (p.C / 16);
+      maxpool333_smem_kernel<<<grid, threads, smem, s>>>(p);
+      return;
+    }
+    maxpool333_fwd_kernel<<<grid_for(total / 4, 256, 148 * 32), 256, 0, s>>>(p);
+    return;
+  }
+  if (g.kt == 1 && g.kh == 3 && g.kw == 3 && g.st == 1 && g.sh == 2 && g.sw == 2 && g.pt == 0 && g.ph == 1 && g.pw == 1 &&
+      p.To == p.Ti && 2 * p.Ho == p.Hi && 2 * p.Wo == p.Wi && 2 * p.Wo * kPool133TY <= 256 && p.C % 16 == 0 &&
+      p.x_coff % 8 == 0 && p.y_coff % 8 == 0 && p.ldx % 8 == 0 && p.ldy % 8 == 0) {
+    const size_t smem = (size_t)(2 * kPool133TY + 1) * (p.Wi + 1) * 64;
+    const int grid = p.B * p.Ti * ((p.Ho + kPool133TY - 1) / kPool133TY) * (p.C / 16);
+    maxpool133s2_smem_kernel<kBn><<<grid, 2 * p.Wo * kPool133TY, smem, s>>>(p);
+    return;
+  }
+  const int grid = grid_for(total, 256, 148 * 32);
+#define POOL_CASE(KT, KH, KW, ST, SH, SW)                                                 \
+  if (g.kt == KT && g.kh == KH && g.kw == KW && g.st == ST && g.sh == SH && g.sw == SW) { \
+    maxpool_fwd_kernel<kBn, KT, KH, KW, ST, SH, SW><<<grid, 256, 0, s>>>(p);              \
+    return;                                                                               \
+  }
+  POOL_CASE(1, 3, 3, 1, 2, 2)
+  POOL_CASE(3, 3, 3, 2, 2, 2)
+  POOL_CASE(2, 2, 2, 2, 2, 2)
+  if constexpr (!kBn) {   // the conv-output form takes only the windows above (bn_pool_geometry)
+    POOL_CASE(3, 3, 3, 1, 1, 1)
+    maxpool_fwd_kernel<false, 0, 0, 0, 0, 0, 0><<<grid, 256, 0, s>>>(p);
+  }
+#undef POOL_CASE
 }
 
 extern "C" int coclr_maxpool_fwd(const coclr_pool_t* p, coclr_stream_t stream) {
-  if (!p || !p->x_hi || !p->y_hi || p->C % 4 || p->ldx % 4 || p->ldy % 4 || p->x_coff % 4 || p->y_coff % 4)
-    return COCLR_E_ARG;
+  if (!p || !p->y_hi || p->C % 4 || p->ldx % 4 || p->ldy % 4 || p->x_coff % 4 || p->y_coff % 4) return COCLR_E_ARG;
   if (p->g.kt * p->g.kh * p->g.kw > 255) return COCLR_E_ARG;
-  const long total = (long)p->B * p->To * p->Ho * p->Wo * (p->C / 4);
-  const coclr_geom_t& g = p->g;
-  if (g.kt == 3 && g.kh == 3 && g.kw == 3 && g.st == 1 && g.sh == 1 && g.sw == 1 && g.pt == 1 && g.ph == 1 &&
-      g.pw == 1 && (p->Wo % 4) == 0 && p->Wo == p->Wi && p->Ho == p->Hi && p->To == p->Ti) {
-    const int threads = 2 * p->Wi * kPoolTY;
-    if (p->Wi >= 8 && threads <= 256 && p->C % 16 == 0 && p->x_coff % 8 == 0 && p->y_coff % 8 == 0 &&
-        p->ldx % 8 == 0 && p->ldy % 8 == 0) {
-      const size_t smem = (size_t)3 * (kPoolTY + 2) * (p->Wi + 2) * 64;
-      const int grid = p->B * ((p->Hi + kPoolTY - 1) / kPoolTY) * (p->C / 16);
-      maxpool333_smem_kernel<<<grid, threads, smem, (cudaStream_t)stream>>>(*p);
-      return LAUNCH_OK();
-    }
-    maxpool333_fwd_kernel<<<grid_for(total / 4, 256, 148 * 32), 256, 0, (cudaStream_t)stream>>>(*p);
-    return LAUNCH_OK();
+  if (p->y != nullptr) {
+    if (!p->scale || !p->shift || !bn_pool_geometry(p->g)) return COCLR_E_ARG;
+    launch_pool_fwd<true>(*p, (cudaStream_t)stream);
+  } else {
+    if (!p->x_hi) return COCLR_E_ARG;
+    launch_pool_fwd<false>(*p, (cudaStream_t)stream);
   }
-  if (g.kt == 1 && g.kh == 3 && g.kw == 3 && g.st == 1 && g.sh == 2 && g.sw == 2 && g.pt == 0 && g.ph == 1 && g.pw == 1 &&
-      p->To == p->Ti && 2 * p->Ho == p->Hi && 2 * p->Wo == p->Wi &&
-      2 * p->Wo * kPool133TY <= 256 && p->C % 16 == 0 && p->x_coff % 8 == 0 && p->y_coff % 8 == 0 && p->ldx % 8 == 0 &&
-      p->ldy % 8 == 0) {
-    const size_t smem = (size_t)(2 * kPool133TY + 1) * (p->Wi + 1) * 64;
-    const int grid = p->B * p->Ti * ((p->Ho + kPool133TY - 1) / kPool133TY) * (p->C / 16);
-    maxpool133s2_smem_kernel<<<grid, 2 * p->Wo * kPool133TY, smem, (cudaStream_t)stream>>>(*p);
-    return LAUNCH_OK();
-  }
-  launch_pool<false>(*p, total, (cudaStream_t)stream);
   return LAUNCH_OK();
 }
 extern "C" int coclr_maxpool_bwd(const coclr_pool_t* p, coclr_stream_t stream) {
@@ -1275,7 +1362,7 @@ extern "C" int coclr_maxpool_bwd(const coclr_pool_t* p, coclr_stream_t stream) {
     return LAUNCH_OK();
   }
   const long total = (long)p->B * p->Ti * p->Hi * p->Wi * (p->C / 4);
-  launch_pool<true>(*p, total, (cudaStream_t)stream);
+  launch_pool_bwd(*p, total, (cudaStream_t)stream);
   return LAUNCH_OK();
 }
 

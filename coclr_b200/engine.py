@@ -65,6 +65,11 @@ class ConvSpec:
 class PoolSpec:
     def __init__(self, name, src, dst, k, s, p):
         self.name, self.src, self.dst, self.k, self.s, self.p = name, src, dst, k, s, p
+        self.fused = False   # pools straight from its source's conv output (see Graph._fuse_pools)
+
+
+# (kernel, stride) of the pools coclr_maxpool_fwd can run from a conv output (coclr_pool_t.y)
+FUSED_POOL_WINDOWS = {((1, 3, 3), (1, 2, 2)), ((3, 3, 3), (2, 2, 2)), ((2, 2, 2), (2, 2, 2))}
 
 
 def _conv_out(d, k, s, p):
@@ -162,6 +167,25 @@ class Graph:
             else:
                 raise ValueError(kind)
         self.backbone_out = x
+        self._fuse_pools()
+
+    def _fuse_pools(self):
+        """A max-pool whose input is a plain BatchNorm(+ReLU) output -- no gating, no residual -- that nothing else
+        reads pools straight from the conv output: its BatchNorm item only finalizes the statistics and the pool applies
+        BatchNorm + ReLU while it loads, so the input's planes are never written or read.  The Inception branch-3
+        pools stay on the planes: their input also feeds convolutions."""
+        readers = {}
+        for kind, it in self.items:
+            if kind in ("conv", "pool"):
+                readers[it.src.index] = readers.get(it.src.index, 0) + 1
+        for t in self.tensors:
+            if t.residual is not None:
+                readers[t.residual.index] = readers.get(t.residual.index, 0) + 1
+        for kind, it in self.items:
+            if kind == "pool":
+                src = it.src
+                it.fused = (src.pending and not src.gates and src.residual is None and readers[src.index] == 1
+                            and src is not self.backbone_out and (tuple(it.k), tuple(it.s)) in FUSED_POOL_WINDOWS)
 
     # -- helpers --
     def _tensor(self, name, C, dims_fn, pending=True):
@@ -391,6 +415,21 @@ class _Act:
                  "bsums", "grad_written", "M", "dy_scale", "bamax", "gmean", "gate", "dgate", "dmean")
 
 
+class _PoolInputView:
+    """Stands in for the planes of a tensor whose max-pool reads the conv output itself, which are never stored:
+    value() recomputes relu(bn(y)) from the conv output and the published scale / shift, bit-identical to what the
+    pool compared (for inspection; nothing on the training path reads it)."""
+
+    def __init__(self, a):
+        self.a = a
+
+    def value(self):
+        a = self.a
+        pl = ops.Planes(a.data.shape, 0, a.data.device)
+        ops.split_into(a.data, pl, scale=a.scale, shift=a.shift, relu=a.spec.relu)
+        return pl.value()
+
+
 class Plan:
     """Buffers + launch lists for one (B, T, H, W, training) configuration."""
 
@@ -408,6 +447,9 @@ class Plan:
         # by coclr_bn_bwd from the data's range) so that the weight-gradient GEMM pairs it with the forward planes --
         # wgmma wants one 16-bit format for both operands -- instead of a bf16 twin of every activation
         gbf = 1 if fbf else 0
+        # source tensor index -> its max-pool that reads the conv output (fp16 planes only: that pool splits into fp16)
+        fused_pool = {it.src.index: it for kind, it in g.items if kind == "pool" and it.fused and not fbf}
+        self.fused_pools = [it.name for it in fused_pool.values()]
         # ---- activations ----
         acts = {}
         n_stat = sum(t.C for t in g.tensors if t.pending)
@@ -425,7 +467,10 @@ class Plan:
             if padded:
                 shape = (B,) + a.dims[:2] + (a.dims[2] + 2 * S2D_PAD, t.C)
             # what every forward consumer reads, and the weight-gradient GEMM (same 16-bit format as dY)
-            a.pl = ops.Planes(shape, fbf, dev, lo=fnp > 1, zero=padded)
+            if t.index in fused_pool:
+                a.pl = _PoolInputView(a)
+            else:
+                a.pl = ops.Planes(shape, fbf, dev, lo=fnp > 1, zero=padded)
             a.data = a.grad = a.dy = a.idx = a.bsums = a.dy_scale = a.bamax = None
             a.gmean = a.gate = a.dgate = a.dmean = None
             a.grad_written = False
@@ -499,10 +544,13 @@ class Plan:
                 geom = ops.Geometry(it.k, it.s, it.p)
                 if with_backward:
                     da.idx = torch.empty(da.M * it.dst.C, dtype=torch.uint8, device=dev)
-                pl = L.Pool(L.dptr(sa.pl.hi), L.dptr(sa.pl.lo), it.src.C, 0, L.dptr(da.pl.hi), L.dptr(da.pl.lo),
-                            it.dst.C, 0, None, None, L.dptr(da.idx), B, it.dst.C,
+                fused = it.src.index in fused_pool
+                pl = L.Pool(None if fused else L.dptr(sa.pl.hi), None if fused else L.dptr(sa.pl.lo), it.src.C, 0,
+                            L.dptr(da.pl.hi), L.dptr(da.pl.lo), it.dst.C, 0, None, None, L.dptr(da.idx), B, it.dst.C,
                             sa.dims[0], sa.dims[1], sa.dims[2], da.dims[0], da.dims[1], da.dims[2], geom.c(0),
                             None, None, 0)
+                if fused:   # BatchNorm + ReLU applied while loading the conv output
+                    pl.y, pl.scale, pl.shift, pl.relu = L.dptr(sa.data), L.dptr(sa.scale), L.dptr(sa.shift), it.src.relu
                 self.keep.append(pl)
                 self.fwd.append((lib.coclr_maxpool_fwd, (C.byref(pl),)))
             elif kind == "bn":
@@ -516,9 +564,16 @@ class Plan:
                                   L.dptr(st.running_mean[rboff:]), L.dptr(st.running_var[rboff:]),
                                   BN_MOMENTUM, BN_EPS, int(training), L.dptr(a.scale), L.dptr(a.shift),
                                   L.dptr(a.mean), L.dptr(a.rstd), it.C)
-                # BatchNorm finalize is fused into the apply+split launch
-                res = acts[it.residual.index].pl if it.residual is not None else None
-                self.fwd.append(split_op(a.data, a.pl, a.M, it.C, None, None, it.relu, bn=bf, res=res))
+                if it.index in fused_pool:
+                    # the finalize alone: the max-pool that is this tensor's only consumer applies it (no planes)
+                    sp = L.Split(L.dptr(a.data), it.C, 0, it.C, a.M, None, None, it.relu, None, None, it.C, 0, 0,
+                                 None, None, bf)
+                    self.keep.append(sp)
+                    self.fwd.append((lib.coclr_affine_split, (C.byref(sp), nsm)))
+                else:
+                    # BatchNorm finalize is fused into the apply+split launch
+                    res = acts[it.residual.index].pl if it.residual is not None else None
+                    self.fwd.append(split_op(a.data, a.pl, a.M, it.C, None, None, it.relu, bn=bf, res=res))
                 if it.gates:
                     # S3D-G feature gating of the block output: the planes written above are scaled in place by
                     # sigmoid(fc(mean_thw)) per clip and channel (csrc/gating.cu)

@@ -87,7 +87,8 @@ class Pool(C.Structure):
                 ("y2_hi", C.c_void_p), ("y2_lo", C.c_void_p), ("idx", C.c_void_p),
                 ("B", C.c_int), ("C", C.c_int), ("Ti", C.c_int), ("Hi", C.c_int), ("Wi", C.c_int),
                 ("To", C.c_int), ("Ho", C.c_int), ("Wo", C.c_int), ("g", Geom),
-                ("dy", C.c_void_p), ("dx", C.c_void_p), ("accumulate", C.c_int)]
+                ("dy", C.c_void_p), ("dx", C.c_void_p), ("accumulate", C.c_int),
+                ("y", C.c_void_p), ("scale", C.c_void_p), ("shift", C.c_void_p), ("relu", C.c_int)]
 
 
 class Adam(C.Structure):

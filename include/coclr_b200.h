@@ -178,7 +178,10 @@ typedef struct {
   void* lo2; /* two operands must share one 16-bit format (wgmma); NULL to skip */
   /* optional fused BatchNorm finalize (bn.scale != NULL): scale/shift are derived in-kernel from the statistics
    * (bn.training) or the running stats, written to bn.scale/bn.shift/bn.save_* and the running stats are updated
-   * by one block -- saves the separate coclr_bn_finalize launch; `scale`/`shift` above are then ignored */
+   * by one block -- saves the separate coclr_bn_finalize launch; `scale`/`shift` above are then ignored.
+   * hi == NULL with the fused finalize: no planes are written, the call is the finalize alone -- the same kernel over
+   * zero rows, so scale / shift / running stats carry the same bits -- for a tensor whose only consumer, a max-pool,
+   * reads the conv output itself (coclr_pool_t.y) */
   coclr_bn_finalize_t bn;
   /* optional residual branch of a ResNet bottleneck (`out += residual` then ReLU, backbone/resnet_2d3d.py:75-80,
    * 118-123): operand planes of the same 16-bit format as hi/lo, added after the affine and before the ReLU */
@@ -247,6 +250,15 @@ typedef struct {
   const float* dy; /* [B,To,Ho,Wo,C] */
   float* dx;       /* [B,Ti,Hi,Wi,ldx] at x_coff */
   int accumulate;
+  /* forward from the conv output (y != NULL; x_hi / x_lo unused): the input is relu?(scale[c] * y + shift[c]) of the
+   * fp32 conv output y [B,Ti,Hi,Wi,ldx] at x_coff, split into the fp16 (hi, lo) pairs coclr_affine_split would store
+   * and pooled as those planes would be -- the same output planes and idx bit for bit, without writing or reading the
+   * input planes (for a BatchNorm+ReLU output whose only consumer is the pool; scale / shift as published by the
+   * BatchNorm finalize).  Windows (1,3,3)/(1,2,2), (3,3,3)/2 and (2,2,2)/2 only (any padding). */
+  const float* y;
+  const float* scale;
+  const float* shift;
+  int relu;
 } coclr_pool_t;
 int coclr_maxpool_fwd(const coclr_pool_t* p, coclr_stream_t stream);
 int coclr_maxpool_bwd(const coclr_pool_t* p, coclr_stream_t stream);
