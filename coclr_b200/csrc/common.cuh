@@ -223,8 +223,9 @@ COCLR_DEVINL void wgmma_mma(float (&d)[kN / 2], uint64_t a, uint64_t b, uint32_t
 // Issues one pipeline stage into the fresh block t and commits it as one wgmma group, without waiting: t = sum over
 // the kNProd (<= 3) operand pairs (ad[p], bd[p]), in that order, of 4 K = 16 steps (descriptor increments a_inc /
 // b_inc), one full-width instruction per (pair, step); scale_d = 0 on the first.  The caller waits for the group and
-// adds t into its accumulator with fp32 adds, as wgmma_stage does per 64-column block: t[i] has the register layout
-// of wgmma_stage's acc[i].  kTA / kTB = 1: the operand is MN-major.
+// adds t into its accumulator with fp32 adds, so long reductions keep fp32 accuracy.  t[16 c + r] = row
+// 16 (warp % 4) + lane / 4 + 8 ((r >> 1) & 1), column 32 c + 8 (r >> 2) + 2 (lane % 4) + (r & 1) of the warpgroup's
+// 64 rows.  kTA / kTB = 1: the operand is MN-major.
 template <int kN, bool kBf16, int kNProd, int kTA = 0, int kTB = 0>
 COCLR_DEVINL void wgmma_stage_issue(float (&t)[kN / 2], const uint64_t (&ad)[3], const uint64_t (&bd)[3], uint32_t a_inc,
                                     uint32_t b_inc) {
@@ -238,51 +239,6 @@ COCLR_DEVINL void wgmma_stage_issue(float (&t)[kN / 2], const uint64_t (&ad)[3],
   }
   wgmma_commit();
   acc_fence(t);
-}
-
-// One 64- (n64) or 32-column block of a warpgroup's product: t holds 32 (16) accumulator registers.
-template <int kTA, int kTB>
-COCLR_DEVINL void wgmma_blk(float (&t)[32], uint64_t a, uint64_t b, bool n64, bool bf16, uint32_t scale_d) {
-  if (n64) {
-    if (bf16) wgmma_n64<true, kTA, kTB>(t, a, b, scale_d);
-    else wgmma_n64<false, kTA, kTB>(t, a, b, scale_d);
-  } else {
-    if (bf16) wgmma_n32<true, kTA, kTB>(t, a, b, scale_d);
-    else wgmma_n32<false, kTA, kTB>(t, a, b, scale_d);
-  }
-}
-
-// One pipeline stage: acc += sum over the nprod (<= 3) operand pairs (ad[p], bd[p]) of 4 K = 16 steps (descriptor
-// increments a_inc / b_inc), ncols (multiple of 32) columns, b_step64 = descriptor step per 64 B columns.  Each
-// 64-column block is summed by the tensor core in a fresh accumulator and added to acc with fp32 adds: long
-// reductions keep fp32 accuracy.  acc[16 c + r] = row 16 (warp % 4) + lane / 4 + 8 ((r >> 1) & 1), column
-// 32 c + 8 (r >> 2) + 2 (lane % 4) + (r & 1) of the warpgroup's 64 rows.
-template <int kChunks, int kTA, int kTB>
-COCLR_DEVINL void wgmma_stage(float (&acc)[16 * kChunks], const uint64_t (&ad)[3], const uint64_t (&bd)[3], int nprod,
-                              uint32_t a_inc, uint32_t b_inc, uint32_t b_step64, int ncols, bool bf16) {
-#pragma unroll
-  for (int j = 0; j < kChunks / 2; ++j) {
-    if (64 * j < ncols) {
-      const bool n64 = 64 * j + 64 <= ncols;
-      float t[32];
-      wgmma_fence();
-#pragma unroll
-      for (int p = 0; p < 3; ++p) {
-        if (p < nprod) {
-#pragma unroll
-          for (uint32_t k = 0; k < 4; ++k)
-            wgmma_blk<kTA, kTB>(t, ad[p] + k * a_inc, bd[p] + k * b_inc + (uint64_t)j * b_step64, n64, bf16,
-                                (p | (int)k) != 0);
-        }
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      acc_fence(t);
-#pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (n64 || i < 16) acc[32 * j + i] += t[i];
-    }
-  }
 }
 
 // ---------------------------------------------------------------------------------------------

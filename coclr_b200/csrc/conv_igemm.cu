@@ -15,10 +15,14 @@
 //  * two consumer warpgroups (64 pixel rows each) issue one wgmma m64 x BN x k16 (BN fixed at compile time) per product
 //    and K step for the three products hi*lo, lo*hi, hi*hi (fp32-equivalent result), or hi*hi only in single-pass
 //    mode.  Each 64-deep K chunk (a pipeline stage) is summed in a fresh register block and added to the fp32
-//    accumulator; the next stage is issued before that add, so one stage is always in flight;
+//    accumulator; the next stage is issued before that add, so one stage is always in flight (the TMA kernel's stage
+//    driver, run_stages in conv_tma.h);
 //  * the epilogue is the TMA kernel's (ConvEpilogue, conv_tma.h): the output tile is 128 consecutive flat rows of a
 //    2-D output tensor map [N, M], stored with bulk-tensor stores; the per-channel sum / sum-of-squares that
-//    train-mode BatchNorm needs are summed from the staged tile into per-block fp32 column tables (kStatTable).
+//    train-mode BatchNorm needs are summed from the staged tile into per-block fp32 column tables (kStatTable);
+//  * the weight-gradient kernel has the wgmma shape fixed at compile time too (products per K step, K-column tile
+//    width, 16-bit format) and issues one n64 group per 64-column block of a stage, each waited for and added into the
+//    fp32 accumulator before the next.
 #include <string.h>
 
 #include "common.cuh"
@@ -33,7 +37,6 @@ static constexpr int kProducerWarps = 8;       // weight-gradient kernel: 256 th
 static constexpr int kFwdProducerWarps = 4;    // forward / dgrad kernel: 128 threads gather 128 rows
 static constexpr int kMmaWarps = 8;     // two consumer warpgroups: MMA, then the epilogue
 static constexpr int kMaxBN = 128;      // output columns per tile (register accumulator: 64 fp32 per thread)
-static constexpr int kAccChunks = kMaxBN / 32;
 // forward / dgrad kernel, three warpgroups: 0 producers (gather, and one elected thread also copies the weights),
 // 1-2 MMA + epilogue
 static constexpr int kThreads = (kFwdProducerWarps + kMmaWarps) * 32;
@@ -321,12 +324,10 @@ __global__ void __launch_bounds__(kThreads, 1)
       const int m_tile = tile / P.n_tiles;
       const int n_tile = tile - m_tile * P.n_tiles;
       const uint64_t zmask = zero_chunk_mask(P, nkc, m_tile);
-      // Stage s + 1 (the next K chunk that zmask keeps) is issued into the other fresh block before stage s is waited
-      // for, added into acc and its slot released, so one stage is always in flight.
+      // Stages are the K chunks that zmask keeps, one in flight (run_stages); a stage releases its slot.
 #pragma unroll
       for (int i = 0; i < kBN / 2; ++i) acc[i] = 0.f;
       int kc = 0;   // the next K chunk to issue
-      // Waits for the next stage's operands and issues it into t; rel = its slot.  Returns false after the last stage.
       auto issue = [&](float (&t)[kBN / 2], uint32_t& rel) -> bool {
         if (zmask != 0ull && kc < nkc) {   // first chunk >= kc that zmask keeps (zmask != 0 only when nkc <= 64)
           const uint64_t keep = ~zmask & (~0ull << kc);
@@ -353,7 +354,6 @@ __global__ void __launch_bounds__(kThreads, 1)
         ++kc;
         return true;
       };
-      // Adds a completed stage into acc and releases its slot.
       auto retire = [&](float (&t)[kBN / 2], uint32_t rel) {
         acc_fence(t);
 #pragma unroll
@@ -362,26 +362,7 @@ __global__ void __launch_bounds__(kThreads, 1)
         // wgmma pipeline, which ptxas answers by serialising every wgmma of the kernel
         mbar_arrive(&empty_bar[rel]);
       };
-      float t0[kBN / 2], t1[kBN / 2];
-      uint32_t rel0, rel1;
-      if (issue(t0, rel0)) {
-        while (true) {
-          if (!issue(t1, rel1)) {
-            wgmma_wait<0>();
-            retire(t0, rel0);
-            break;
-          }
-          wgmma_wait<1>();
-          retire(t0, rel0);
-          if (!issue(t0, rel0)) {
-            wgmma_wait<0>();
-            retire(t1, rel1);
-            break;
-          }
-          wgmma_wait<1>();
-          retire(t1, rel1);
-        }
-      }
+      run_stages<kBN, uint32_t>(issue, retire);
       const int idx[4] = {m_tile, 0, 0, 0};
       epi.tile(P, O, &map_out, smem_base + L.off_stage, acc, idx, n_tile);
     }
@@ -424,23 +405,24 @@ __host__ __device__ inline int wgrad_bnk(int Kreal) {
   return ((w + 63) / 64) * 64;
 }
 
-template <int kNPass>
+// kNProd: products per K step, 1 (single pass), 2 (stacked, below) or 3; kBNk = wgrad_bnk(Kreal); kBf16: the 16-bit
+// format of both operands.
+template <int kNProd, int kBNk, bool kBf16>
 __global__ void __launch_bounds__(kWgradThreads, 1) conv_wgrad_kernel(const coclr_wgrad_t P) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr bool kLo = kNPass > 1;
+  constexpr bool kLo = kNProd > 1;
   const int M = P.B * P.Td * P.Hd * P.Wd;
   const int taps = P.g.kt * P.g.kh * P.g.kw;
   const int Kreal = taps * P.src.C;
-  const int BNk = wgrad_bnk(Kreal);
-  const int k_tiles = (Kreal + BNk - 1) / BNk;
+  const int k_tiles = (Kreal + kBNk - 1) / kBNk;
   const int c_tiles = (P.Cout + 127) / 128;
-  const WgradSmemLayout L = wgrad_smem_layout(BNk, kNPass);
+  const WgradSmemLayout L = wgrad_smem_layout(kBNk, kNProd);
   const uint32_t nstages = L.stages;
   // Cout <= 64 in split-precision mode: the hi and the lo plane of dY are the two 64-row halves of the M = 128 tile
   // ([dY_hi; dY_lo] x A_hi, then x A_lo: 2 instructions per K step instead of 3 on a half-empty tile, and the lo x lo
   // term comes for free); rows 64..127 hold the dY_lo products of channels 0..63 and are added by the epilogue
-  const bool stack_m = kLo && P.Cout <= 64;
+  constexpr bool stack_m = kNProd == 2;
 
   // work item: (split, c_tile, k_tile)
   int w = blockIdx.x;
@@ -458,11 +440,10 @@ __global__ void __launch_bounds__(kWgradThreads, 1) conv_wgrad_kernel(const cocl
   uint64_t* empty_bar = full_bar + kMaxStages;
 
   const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int s = 0; s < kMaxStages; ++s) {
       mbar_init(&full_bar[s], kProducerWarps * 32);
-      mbar_init(&empty_bar[s], kMmaWarps);
+      mbar_init(&empty_bar[s], kMmaWarps * 32);   // one arrival per consumer thread
     }
     mbar_fence_init();
   }
@@ -480,11 +461,11 @@ __global__ void __launch_bounds__(kWgradThreads, 1) conv_wgrad_kernel(const cocl
     ident.pt = ident.ph = ident.pw = 0;
     ident.transposed = 0;
     // the K granules this thread copies are the same for every pixel chunk: decompose them once
-    TapPos tp_dy[2], tp_a[kMaxBN / 64];
+    TapPos tp_dy[2], tp_a[kBNk / 64];
 #pragma unroll
     for (int blk = 0; blk < 2; ++blk) tp_dy[blk] = tap_of(P.dy, ident, c_tile * 128 + blk * 64 + ck * 8);
 #pragma unroll
-    for (int blk = 0; blk < kMaxBN / 64; ++blk) tp_a[blk] = tap_of(P.src, P.g, k_tile * BNk + blk * 64 + ck * 8);
+    for (int blk = 0; blk < kBNk / 64; ++blk) tp_a[blk] = tap_of(P.src, P.g, k_tile * kBNk + blk * 64 + ck * 8);
     for (int ch = ch_begin; ch < ch_begin + nch; ++ch) {
       int rb[2], rt[2], ry[2], rx[2];    // source-space bases for the activation gather
       int qb[2], qt[2], qy[2], qx[2];    // plain destination coordinates for dY
@@ -501,7 +482,7 @@ __global__ void __launch_bounds__(kWgradThreads, 1) conv_wgrad_kernel(const cocl
       const uint32_t s_dy = smem_base + stage * L.stage_bytes;
       const uint32_t s_a = s_dy + (kLo ? 2u : 1u) * L.dy_bytes;
       // dY: 2 blocks of 64 output channels (stacked mode: block 0 = hi plane, block 1 = lo plane of channels 0..63)
-      if (stack_m) {
+      if constexpr (stack_m) {
         gather_block_async<kLo, 2>(P.dy, ident, P.dy.C, tp_dy[0], ck, r0, RowsPlain{qb, qt, qy, qx}, s_dy,
                                    s_dy + kWgPx * 128);
       } else {
@@ -512,21 +493,18 @@ __global__ void __launch_bounds__(kWgradThreads, 1) conv_wgrad_kernel(const cocl
         }
       }
 #pragma unroll
-      for (int blk = 0; blk < kMaxBN / 64; ++blk) {
-        if (blk < BNk / 64)
-          gather_block_async<kLo, 2>(P.src, P.g, Kreal, tp_a[blk], ck, r0, RowsPlain{rb, rt, ry, rx},
-                                     s_a + blk * (kWgPx * 128), s_a + L.a_bytes + blk * (kWgPx * 128));
-      }
+      for (int blk = 0; blk < kBNk / 64; ++blk)
+        gather_block_async<kLo, 2>(P.src, P.g, Kreal, tp_a[blk], ck, r0, RowsPlain{rb, rt, ry, rx},
+                                   s_a + blk * (kWgPx * 128), s_a + L.a_bytes + blk * (kWgPx * 128));
       cp_async_mbar_arrive_noinc(&full_bar[stage]);
       if (++stage == nstages) { stage = 0; phase ^= 1u; }
     }
   } else {
     // ===================== MMA: warpgroup wg owns cout rows [64 wg, 64 wg + 64) of the tile =====================
     const int wg = warp >> 2;
-    const bool bf16 = P.dy_bf16 != 0;
-    float acc[16 * kAccChunks];
+    float acc[kBNk / 2];
 #pragma unroll
-    for (int i = 0; i < 16 * kAccChunks; ++i) acc[i] = 0.f;
+    for (int i = 0; i < kBNk / 2; ++i) acc[i] = 0.f;
     uint32_t stage = 0, phase = 0;
     for (int ch = 0; ch < nch; ++ch) {
       mbar_wait_spin(&full_bar[stage], phase);
@@ -536,34 +514,38 @@ __global__ void __launch_bounds__(kWgradThreads, 1) conv_wgrad_kernel(const cocl
       // MN-major: LBO = stride between 64-element MN blocks (64 px * 128 B), SBO = 8-pixel group stride
       const uint64_t a_hi = make_smem_desc(s_dy, kWgPx * 128, 1024);
       const uint64_t b_hi = make_smem_desc(s_a, kWgPx * 128, 1024);
-      const uint32_t b_step = (kWgPx * 128) >> 4;
-      // one K=16 step = 16 pixels = 2 swizzle atoms = 2048 B -> +128 in descriptor units
-      if constexpr (kLo) {
-        const uint64_t a_lo = make_smem_desc(s_dy + L.dy_bytes, kWgPx * 128, 1024);
-        const uint64_t b_lo = make_smem_desc(s_a + L.a_bytes, kWgPx * 128, 1024);
-        const uint64_t ad[3] = {a_hi, stack_m ? a_hi : a_lo, a_hi}, bd[3] = {b_lo, b_hi, b_hi};
-        wgmma_stage<kAccChunks, 1, 1>(acc, ad, bd, stack_m ? 2 : 3, 128u, 128u, b_step, BNk, bf16);
-      } else {
-        const uint64_t ad[3] = {a_hi, a_hi, a_hi}, bd[3] = {b_hi, b_hi, b_hi};
-        wgmma_stage<kAccChunks, 1, 1>(acc, ad, bd, 1, 128u, 128u, b_step, BNk, bf16);
+      const uint64_t a_lo = kLo ? make_smem_desc(s_dy + L.dy_bytes, kWgPx * 128, 1024) : a_hi;
+      const uint64_t b_lo = kLo ? make_smem_desc(s_a + L.a_bytes, kWgPx * 128, 1024) : b_hi;
+      // Each 64-column block of the stage is summed by the tensor core in the fresh block t and added into acc with fp32
+      // adds: long reductions keep fp32 accuracy.  One K = 16 step = 16 pixels = 2 swizzle atoms = 2048 B -> +128 in
+      // descriptor units; the next 64 columns of A start kWgPx * 128 B further on.
+#pragma unroll
+      for (int j = 0; j < kBNk / 64; ++j) {
+        const uint64_t bj = (uint64_t)j * ((kWgPx * 128) >> 4);
+        const uint64_t ad[3] = {a_hi, stack_m ? a_hi : a_lo, a_hi}, bd[3] = {b_lo + bj, b_hi + bj, b_hi + bj};
+        float t[32];
+        wgmma_stage_issue<64, kBf16, kNProd, 1, 1>(t, ad, bd, 128u, 128u);
+        wgmma_wait<0>();
+        acc_fence(t);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[32 * j + i] += t[i];
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      mbar_arrive(&empty_bar[stage]);   // every consumer thread: see conv_igemm_kernel
       if (++stage == nstages) { stage = 0; phase ^= 1u; }
     }
     const int tw = threadIdx.x & 127;
-    if (stack_m) {
+    if constexpr (stack_m) {
       // dY_lo rows (warpgroup 1) join the dY_hi rows via smem
       float* xs = reinterpret_cast<float*>(smem);
       named_bar_sync(1, kMmaWarps * 32);   // MMAs done
       if (wg == 1) {
 #pragma unroll
-        for (int i = 0; i < 16 * kAccChunks; ++i) xs[i * 128 + tw] = acc[i];
+        for (int i = 0; i < kBNk / 2; ++i) xs[i * 128 + tw] = acc[i];
       }
       named_bar_sync(1, kMmaWarps * 32);
       if (wg == 0) {
 #pragma unroll
-        for (int i = 0; i < 16 * kAccChunks; ++i) acc[i] += xs[i * 128 + tw];
+        for (int i = 0; i < kBNk / 2; ++i) acc[i] += xs[i * 128 + tw];
       }
     }
     if (nch > 0 && !(stack_m && wg == 1)) {
@@ -572,12 +554,11 @@ __global__ void __launch_bounds__(kWgradThreads, 1) conv_wgrad_kernel(const cocl
       const int col0 = 2 * (tw & 3);
       const float os = P.out_scale != nullptr ? __ldg(P.out_scale) : 1.f;
 #pragma unroll
-      for (int c = 0; c < kAccChunks; ++c) {
-        if (c * 32 >= BNk) break;
+      for (int c = 0; c < kBNk / 32; ++c) {
 #pragma unroll
         for (int r = 0; r < 16; ++r) {
           const int n = c_tile * 128 + row0 + 8 * ((r >> 1) & 1);   // output channel
-          const int k = k_tile * BNk + c * 32 + col0 + 8 * (r >> 2) + (r & 1);
+          const int k = k_tile * kBNk + c * 32 + col0 + 8 * (r >> 2) + (r & 1);
           if (n < P.Cout && k < Kreal) {
             const int tap = k / P.src.C;
             const int ci = k - tap * P.src.C;
@@ -731,29 +712,6 @@ static bool src_ok(const coclr_src_t& s, int need_lo) {
   return true;
 }
 
-template <int kNPass, int kBN, bool kBf16>
-static int launch_conv_bn(const coclr_conv_t& P, const CUtensorMap& m_out, const ConvOut& O, int grid, uint32_t smem,
-                          cudaStream_t s) {
-  const cudaError_t e =
-      cudaFuncSetAttribute(conv_igemm_kernel<kNPass, kBN, kBf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  if (e != cudaSuccess) return COCLR_E_LAUNCH;
-  conv_igemm_kernel<kNPass, kBN, kBf16><<<grid, kThreads, smem, s>>>(m_out, P, O);
-  return COCLR_OK;
-}
-
-// One kernel instance per (pass count, tile width, 16-bit format): the wgmma shape and type are compile-time constants.
-template <int kNPass, bool kBf16>
-static int launch_conv_np(const coclr_conv_t& P, const CUtensorMap& m_out, const ConvOut& O, int grid, uint32_t smem,
-                          cudaStream_t s) {
-  switch (P.BN) {
-    case 32: return launch_conv_bn<kNPass, 32, kBf16>(P, m_out, O, grid, smem, s);
-    case 64: return launch_conv_bn<kNPass, 64, kBf16>(P, m_out, O, grid, smem, s);
-    case 96: return launch_conv_bn<kNPass, 96, kBf16>(P, m_out, O, grid, smem, s);
-    case 128: return launch_conv_bn<kNPass, 128, kBf16>(P, m_out, O, grid, smem, s);
-    default: return COCLR_E_ARG;
-  }
-}
-
 static int launch_conv(const coclr_conv_t& P, int num_sms, cudaStream_t s) {
   const int M = P.B * P.Td * P.Hd * P.Wd;
   const int m_tiles = (M + kTileM - 1) / kTileM;
@@ -783,12 +741,15 @@ static int launch_conv(const coclr_conv_t& P, int num_sms, cudaStream_t s) {
   CUtensorMap m_out;
   if (!encode_map(&m_out, ms, 0, 5, /*swizzle=*/true)) return COCLR_E_LAUNCH;
   const int grid = total < num_sms ? total : num_sms;
-  const bool bf16 = P.a_bf16 != 0;
-  int rc;
-  if (P.npass > 1) rc = bf16 ? launch_conv_np<3, true>(P, m_out, O, grid, L.total, s)
-                             : launch_conv_np<3, false>(P, m_out, O, grid, L.total, s);
-  else rc = bf16 ? launch_conv_np<1, true>(P, m_out, O, grid, L.total, s)
-                 : launch_conv_np<1, false>(P, m_out, O, grid, L.total, s);
+  // one kernel instance per (pass count, tile width, 16-bit format): the wgmma shape and type are compile-time constants
+  int rc = COCLR_E_ARG;
+  with_int<1, 3>(P.npass > 1 ? 3 : 1, [&](auto np) {
+    with_int<32, 64, 96, 128>(P.BN, [&](auto bn) {
+      with_int<0, 1>(P.a_bf16 != 0, [&](auto bf) {
+        rc = launch_with_smem(conv_igemm_kernel<np, bn, bf != 0>, grid, kThreads, L.total, s, m_out, P, O);
+      });
+    });
+  });
   if (rc != COCLR_OK) return rc;
   return cudaGetLastError() == cudaSuccess ? COCLR_OK : COCLR_E_LAUNCH;
 }
@@ -815,19 +776,25 @@ extern "C" int coclr_conv_igemm(const coclr_conv_t* p, int num_sms, coclr_stream
   return launch_conv(*p, num_sms, s);
 }
 
-template <int NP>
 static int launch_wgrad(const coclr_wgrad_t& P, cudaStream_t s) {
   const int taps = P.g.kt * P.g.kh * P.g.kw;
   const int Kreal = taps * P.src.C;
   const int BNk = wgrad_bnk(Kreal);
   const int k_tiles = (Kreal + BNk - 1) / BNk;
   const int c_tiles = (P.Cout + 127) / 128;
-  const WgradSmemLayout L = wgrad_smem_layout(BNk, NP);
+  const WgradSmemLayout L = wgrad_smem_layout(BNk, P.npass);
   if (L.stages < 2) return COCLR_E_ARG;
-  cudaError_t e = cudaFuncSetAttribute(conv_wgrad_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total);
-  if (e != cudaSuccess) return COCLR_E_LAUNCH;
   const int grid = k_tiles * c_tiles * P.splits;
-  conv_wgrad_kernel<NP><<<grid, kWgradThreads, L.total, s>>>(P);
+  // one kernel instance per (products per K step, K-column tile width, 16-bit format)
+  int rc = COCLR_E_ARG;
+  with_int<1, 2, 3>(P.npass > 1 ? (P.Cout <= 64 ? 2 : 3) : 1, [&](auto nprod) {
+    with_int<64, 128>(BNk, [&](auto bnk) {
+      with_int<0, 1>(P.dy_bf16 != 0, [&](auto bf) {
+        rc = launch_with_smem(conv_wgrad_kernel<nprod, bnk, bf != 0>, grid, kWgradThreads, L.total, s, P);
+      });
+    });
+  });
+  if (rc != COCLR_OK) return rc;
   return cudaGetLastError() == cudaSuccess ? COCLR_OK : COCLR_E_LAUNCH;
 }
 
@@ -843,5 +810,5 @@ extern "C" int coclr_conv_wgrad(const coclr_wgrad_t* p, coclr_stream_t stream) {
   // TMA-staged kernel first (wgrad_tma.cu: stride-1 "same" convolutions); everything else on the gather kernel
   const int rc = coclr::wgrad_tma_try(*p, s);
   if (rc <= 0) return rc;
-  return p->npass > 1 ? launch_wgrad<3>(*p, s) : launch_wgrad<1>(*p, s);
+  return launch_wgrad(*p, s);
 }

@@ -192,27 +192,28 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
       const int ty0 = tma_first_type(L, t);
       const int ty1 = L.sel_dim >= 0 ? ty0 + 1 : L.n_types;
       // ---- MMA ----
-      // Stages (64-deep K chunks) in order cc, slab type, shift.  Stage s + 1 is issued into the other fresh block
-      // before stage s is waited for, added into acc and its A-slab / weight slots released, so one stage is always in
-      // flight while a warpgroup folds, releases and waits on the next barrier.
+      // Stages (64-deep K chunks) in order cc, slab type, shift, one in flight while a warpgroup folds, releases and
+      // waits on the next barrier (run_stages).
 #pragma unroll
       for (int i = 0; i < kBN / 2; ++i) acc[i] = 0.f;
       int cc = 0, ty = ty0, j = 0;   // the next stage to issue
-      // Waits for the next stage's operands and issues it into t; rel_a / rel_b = the A and weight slots to release
-      // once it has completed (-1: none; an A slab is released after its last shift, resident weights never).
-      // Returns false after the tile's last stage.
-      auto issue = [&](float (&t)[kBN / 2], int& rel_a, int& rel_b) -> bool {
+      // The A and weight slots a stage releases once it has completed (-1: none; an A slab is released after its last
+      // shift, resident weights never).
+      struct Rel {
+        int a, b;
+      };
+      auto issue = [&](float (&t)[kBN / 2], Rel& rel) -> bool {
         if (cc == L.nc) return false;
         const TmaSlabType& S = L.type[ty];
         if (j == 0) mbar_wait_spin(&a_full[aslot], aphase);
         uint32_t sb;
         if (L.b_resident) {
           sb = b_base + (uint32_t)(S.tap[j] * L.nc + cc) * kBTileBytes;
-          rel_b = -1;
+          rel.b = -1;
         } else {
           mbar_wait_spin(&b_full[bslot], bphase);
           sb = b_base + bslot * kBTileBytes;
-          rel_b = (int)bslot;
+          rel.b = (int)bslot;
           if (++bslot == (uint32_t)L.b_slots) { bslot = 0; bphase ^= 1u; }
         }
         const uint32_t sa = a_base + aslot * (uint32_t)L.a_slot_bytes + (uint32_t)j * (uint32_t)L.shift_bytes + a_row_off;
@@ -227,45 +228,25 @@ __global__ void __launch_bounds__(kTmaThreads, 1)
           const uint64_t ad[3] = {a_hi, a_hi, a_hi}, bd[3] = {b_hi, b_hi, b_hi};
           wgmma_stage_issue<kBN, kBf16, 1>(t, ad, bd, 2u, 2u);
         }
-        rel_a = -1;
+        rel.a = -1;
         if (++j == S.nshift) {
           j = 0;
-          rel_a = (int)aslot;
+          rel.a = (int)aslot;
           if (++aslot == (uint32_t)L.a_slots) { aslot = 0; aphase ^= 1u; }
           if (++ty == ty1) { ty = ty0; ++cc; }
         }
         return true;
       };
-      // Adds a completed stage into acc and releases its slots.
-      auto retire = [&](float (&t)[kBN / 2], int rel_a, int rel_b) {
+      auto retire = [&](float (&t)[kBN / 2], const Rel& rel) {
         acc_fence(t);
 #pragma unroll
         for (int i = 0; i < kBN / 2; ++i) acc[i] += t[i];
         // every consumer thread arrives: an arrival under `lane == 0` would be a thread-dependent branch inside the
         // wgmma pipeline, which ptxas answers by serialising every wgmma of the kernel
-        if (rel_b >= 0) mbar_arrive(&b_empty[rel_b]);
-        if (rel_a >= 0) mbar_arrive(&a_empty[rel_a]);   // the slab may be overwritten once every thread has read it
+        if (rel.b >= 0) mbar_arrive(&b_empty[rel.b]);
+        if (rel.a >= 0) mbar_arrive(&a_empty[rel.a]);   // the slab may be overwritten once every thread has read it
       };
-      float t0[kBN / 2], t1[kBN / 2];
-      int rel_a0, rel_b0, rel_a1, rel_b1;
-      if (issue(t0, rel_a0, rel_b0)) {
-        while (true) {
-          if (!issue(t1, rel_a1, rel_b1)) {
-            wgmma_wait<0>();
-            retire(t0, rel_a0, rel_b0);
-            break;
-          }
-          wgmma_wait<1>();
-          retire(t0, rel_a0, rel_b0);
-          if (!issue(t0, rel_a0, rel_b0)) {
-            wgmma_wait<0>();
-            retire(t1, rel_a1, rel_b1);
-            break;
-          }
-          wgmma_wait<1>();
-          retire(t1, rel_a1, rel_b1);
-        }
-      }
+      run_stages<kBN, Rel>(issue, retire);
       epi.tile(P, L.out, &map_out, smem_base + L.off_stage, acc, t.idx, t.n_tile);
     }
     epi.finish(P, L.out, smem + L.off_stage);
@@ -650,29 +631,6 @@ extern "C" int coclr_conv_tma_plan(const coclr_conv_t* p, int* info) {
   return 1;
 }
 
-template <int kNPass, int kBN, bool kBf16>
-static int conv_tma_launch_bn(int grid, const CUtensorMap& m_hi, const CUtensorMap& m_lo, const CUtensorMap& m_out,
-                              const TmaArgs& args, cudaStream_t stream) {
-  const cudaError_t e = cudaFuncSetAttribute(conv_tma_kernel<kNPass, kBN, kBf16>,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)args.plan.total);
-  if (e != cudaSuccess) return COCLR_E_LAUNCH;
-  conv_tma_kernel<kNPass, kBN, kBf16><<<grid, kTmaThreads, args.plan.total, stream>>>(m_hi, m_lo, m_out, args);
-  return COCLR_OK;
-}
-
-// One kernel instance per (pass count, tile width, 16-bit format): the wgmma shape and type are compile-time constants.
-template <int kNPass, bool kBf16>
-static int conv_tma_launch(int BN, int grid, const CUtensorMap& m_hi, const CUtensorMap& m_lo, const CUtensorMap& m_out,
-                           const TmaArgs& args, cudaStream_t stream) {
-  switch (BN) {
-    case 32: return conv_tma_launch_bn<kNPass, 32, kBf16>(grid, m_hi, m_lo, m_out, args, stream);
-    case 64: return conv_tma_launch_bn<kNPass, 64, kBf16>(grid, m_hi, m_lo, m_out, args, stream);
-    case 96: return conv_tma_launch_bn<kNPass, 96, kBf16>(grid, m_hi, m_lo, m_out, args, stream);
-    case 128: return conv_tma_launch_bn<kNPass, 128, kBf16>(grid, m_hi, m_lo, m_out, args, stream);
-    default: return COCLR_E_ARG;
-  }
-}
-
 // Returns COCLR_OK when the launch was issued, 1 when this shape is not handled here (caller falls through to the
 // cp.async kernel), a negative COCLR_E_* on a launch error.
 int coclr::conv_tma_try(const coclr_conv_t& P, int num_sms, cudaStream_t stream) {
@@ -698,12 +656,16 @@ int coclr::conv_tma_try(const coclr_conv_t& P, int num_sms, cudaStream_t stream)
   args.a_bf16 = P.a_bf16;
   args.b_bf16 = P.b_bf16;
   const int grid = L.total_tiles < num_sms ? L.total_tiles : num_sms;
-  const bool bf16 = P.a_bf16 != 0;
-  int rc;
-  if (P.npass > 1) rc = bf16 ? conv_tma_launch<3, true>(L.out.BN, grid, m_hi, m_lo, m_out, args, stream)
-                             : conv_tma_launch<3, false>(L.out.BN, grid, m_hi, m_lo, m_out, args, stream);
-  else rc = bf16 ? conv_tma_launch<1, true>(L.out.BN, grid, m_hi, m_lo, m_out, args, stream)
-                 : conv_tma_launch<1, false>(L.out.BN, grid, m_hi, m_lo, m_out, args, stream);
+  // one kernel instance per (pass count, tile width, 16-bit format): the wgmma shape and type are compile-time constants
+  int rc = COCLR_E_ARG;
+  with_int<1, 3>(P.npass > 1 ? 3 : 1, [&](auto np) {
+    with_int<32, 64, 96, 128>(L.out.BN, [&](auto bn) {
+      with_int<0, 1>(P.a_bf16 != 0, [&](auto bf) {
+        rc = launch_with_smem(conv_tma_kernel<np, bn, bf != 0>, grid, kTmaThreads, L.total, stream, m_hi, m_lo, m_out,
+                              args);
+      });
+    });
+  });
   if (rc != COCLR_OK) return rc;
   return cudaGetLastError() == cudaSuccess ? COCLR_OK : COCLR_E_LAUNCH;
 }

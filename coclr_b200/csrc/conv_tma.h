@@ -1,9 +1,12 @@
-// Tile plan of the TMA-staged convolution kernel (conv_tma.cu), shared between the host planner and the kernel, and the
-// epilogue that both convolution kernels (conv_tma.cu, conv_igemm.cu) run on their register accumulators.
+// Tile plan of the TMA-staged convolution kernel (conv_tma.cu), shared between the host planner and the kernel; the
+// stage driver and the epilogue that both convolution kernels (conv_tma.cu, conv_igemm.cu) run on their register
+// accumulators; and the instance dispatch of every wgmma kernel's launcher.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 #include "coclr_b200.h"
 #include "common.cuh"
@@ -276,6 +279,51 @@ struct ConvEpilogue {
     if (leader) bulk_wait_group<0>();   // all global writes of this thread's bulk stores are complete
   }
 };
+
+// The K loop of a convolution tile on two fresh register blocks: stage s + 1 is issued into the other block before
+// stage s is waited for and retired, so one stage is always in flight.  issue(t, rel) waits for the next stage's
+// operands, issues it into t and records in rel the slots to release once it has completed; it returns false after the
+// tile's last stage.  retire(t, rel) adds the completed block t into the accumulator and releases rel's slots.
+template <int kBN, class Rel, class Issue, class Retire>
+COCLR_DEVINL void run_stages(Issue&& issue, Retire&& retire) {
+  float t0[kBN / 2], t1[kBN / 2];
+  Rel rel0, rel1;
+  if (!issue(t0, rel0)) return;
+  while (true) {
+    if (!issue(t1, rel1)) {
+      wgmma_wait<0>();
+      retire(t0, rel0);
+      return;
+    }
+    wgmma_wait<1>();
+    retire(t0, rel0);
+    if (!issue(t0, rel0)) {
+      wgmma_wait<0>();
+      retire(t1, rel1);
+      return;
+    }
+    wgmma_wait<1>();
+    retire(t1, rel1);
+  }
+}
+
+// Kernel instances are picked from run-time values, one compile-time parameter at a time:
+// with_int<V...>(v, f) calls f(std::integral_constant<int, V>()) for the V that equals v, and returns false when none
+// does.
+template <int... Vs, class F>
+inline bool with_int(int v, F&& f) {
+  return ((v == Vs && (f(std::integral_constant<int, Vs>()), true)) || ...);
+}
+
+// Launches kernel with `smem` bytes of dynamic shared memory; COCLR_E_LAUNCH when that much cannot be granted.
+template <class... Params, class... Args>
+inline int launch_with_smem(void (*kernel)(Params...), int grid, int threads, uint32_t smem, cudaStream_t stream,
+                            const Args&... args) {
+  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+    return COCLR_E_LAUNCH;
+  kernel<<<grid, threads, smem, stream>>>(args...);
+  return COCLR_OK;
+}
 
 // One TMA slab load: coordinate offsets (logical dims 1..4 of the tensor map) relative to the tile origin, and the
 // taps it serves -- shift j reads the slab at row offset j * shift_rows and multiplies with packed K chunk

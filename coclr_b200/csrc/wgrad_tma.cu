@@ -601,30 +601,6 @@ static bool wgrad_tma_plan(const coclr_wgrad_t& P, WgPlan& L, MapSpec& DY, MapSp
 
 static bool g_wgrad_tma = true;
 
-template <int kN, int kNProd, bool kBf16>
-static int wgrad_tma_launch_n(int grid, const CUtensorMap& dy_hi, const CUtensorMap& dy_lo, const CUtensorMap& x_hi,
-                              const CUtensorMap& x_lo, const WgArgs& args, cudaStream_t stream) {
-  const cudaError_t e = cudaFuncSetAttribute(wgrad_tma_kernel<kN, kNProd, kBf16>,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)args.plan.total);
-  if (e != cudaSuccess) return COCLR_E_LAUNCH;
-  wgrad_tma_kernel<kN, kNProd, kBf16><<<grid, kWgThreads, args.plan.total, stream>>>(dy_hi, dy_lo, x_hi, x_lo, args);
-  return COCLR_OK;
-}
-
-// One kernel instance per (columns, products per K step, 16-bit format): the wgmma shapes and type are compile-time
-// constants.
-template <int kNProd, bool kBf16>
-static int wgrad_tma_launch(int grid, const CUtensorMap& dy_hi, const CUtensorMap& dy_lo, const CUtensorMap& x_hi,
-                            const CUtensorMap& x_lo, const WgArgs& args, cudaStream_t stream) {
-  switch (args.plan.N) {
-    case 64: return wgrad_tma_launch_n<64, kNProd, kBf16>(grid, dy_hi, dy_lo, x_hi, x_lo, args, stream);
-    case 128: return wgrad_tma_launch_n<128, kNProd, kBf16>(grid, dy_hi, dy_lo, x_hi, x_lo, args, stream);
-    case 192: return wgrad_tma_launch_n<192, kNProd, kBf16>(grid, dy_hi, dy_lo, x_hi, x_lo, args, stream);
-    case 256: return wgrad_tma_launch_n<256, kNProd, kBf16>(grid, dy_hi, dy_lo, x_hi, x_lo, args, stream);
-    default: return COCLR_E_ARG;
-  }
-}
-
 int wgrad_tma_try(const coclr_wgrad_t& P, cudaStream_t stream) {
   if (!g_wgrad_tma || P.ws == nullptr || ((uintptr_t)P.ws & 15)) return 1;
   WgArgs args;
@@ -645,14 +621,17 @@ int wgrad_tma_try(const coclr_wgrad_t& P, cudaStream_t stream) {
   args.dy_bf16 = P.dy_bf16;
   args.src_bf16 = P.src_bf16;
   const int grid = L.n_types * L.n_cgroups * L.m_groups * L.splits;
-  const int nprod = L.planes == 1 ? 1 : (L.stacked ? 2 : 3);
-  int rc;
-  if (nprod == 1) rc = args.dy_bf16 ? wgrad_tma_launch<1, true>(grid, m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, args, stream)
-                                    : wgrad_tma_launch<1, false>(grid, m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, args, stream);
-  else if (nprod == 2) rc = args.dy_bf16 ? wgrad_tma_launch<2, true>(grid, m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, args, stream)
-                                         : wgrad_tma_launch<2, false>(grid, m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, args, stream);
-  else rc = args.dy_bf16 ? wgrad_tma_launch<3, true>(grid, m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, args, stream)
-                         : wgrad_tma_launch<3, false>(grid, m_dy_hi, m_dy_lo, m_x_hi, m_x_lo, args, stream);
+  // one kernel instance per (columns, products per K step, 16-bit format): the wgmma shapes and type are compile-time
+  // constants
+  int rc = COCLR_E_ARG;
+  with_int<64, 128, 192, 256>(L.N, [&](auto n) {
+    with_int<1, 2, 3>(L.planes == 1 ? 1 : (L.stacked ? 2 : 3), [&](auto nprod) {
+      with_int<0, 1>(args.dy_bf16 != 0, [&](auto bf) {
+        rc = launch_with_smem(wgrad_tma_kernel<n, nprod, bf != 0>, grid, kWgThreads, L.total, stream, m_dy_hi, m_dy_lo,
+                              m_x_hi, m_x_lo, args);
+      });
+    });
+  });
   if (rc != COCLR_OK) return rc;
   const int rows = L.stacked ? 64 : L.mb * 64;
   const dim3 rgrid((L.N * rows + 255) / 256, L.n_types * L.n_cgroups * L.m_groups);
