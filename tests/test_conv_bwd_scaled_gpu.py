@@ -5,9 +5,11 @@ scalar out_scale (&dy_scale[1]).  Every fp16 (pass count, tile width) instance o
 TMA-staged one and the cp.async gather one) runs a data gradient here, stored and accumulated into a channel slice of a
 wider buffer, with 1/s far from 1 in both directions and per-row weight scales spread over several octaves (so that
 the packer's unscale differs from column to column and from one N tile to the next).  Truth: float64 autograd of
-torch's conv3d; single-pass launches are also held to the float64 product of their exact operands.  Also: the weight
-gradient of the shapes the TMA-staged weight-gradient kernel declines, the BatchNorm-backward -> convolution chain as
-the engine wires it, and the batched weight packer against the per-layer one."""
+torch's conv3d; single-pass launches are also held to the float64 product of their exact operands.  Also: weight
+gradients in the same format on every kind (1x1x1, (1,3,3), (3,1,1), the temporally strided and the space-to-depth
+stems) and product count of the TMA-staged weight-gradient kernel and on the gather kernel's shapes, the
+BatchNorm-backward -> convolution chain as the engine wires it, and the batched weight packer against the per-layer
+one."""
 import ctypes as C
 import math
 
@@ -192,53 +194,117 @@ def test_dgrad_bf16_control(case, diag):
     assert err < 2e-4, (key, err)
 
 
-# Weight gradients the TMA-staged weight-gradient kernel declines (they run on the gather kernel):
-# (name, Cin, Cout, k, s, p, B, T, H, W)
+# Weight gradients dW[Cout, Cin, *k] += X x dY: (name, kernel, width, Cin, Cout, k, s, p, B, T, H, W).  kernel and width
+# are the instance the launch must reach: the TMA-staged kernel at item width N = coclr_wgrad_tma_plan info[3], or the
+# gather kernel at K-column tile width wgrad_bnk(Kreal).  One TMA case per kind and product count (3 passes: 2 products
+# when Cout <= 64, stacked, else 3; single pass: 1), the block kind at every N; test_conv_bwd_scaled_plan_cpu.py
+# checks the labels and that every weight-gradient launch class of the training plans is among these or the other
+# float64 weight-gradient tests.  A (., 4, 4) kernel is a space-to-depth stem: Cin = 12 real channels of 16-channel
+# pixels, rows zero-padded by engine.S2D_PAD = 2 pixels on each side, and (T, H, W) the destination frame.
 WGRAD_CASES = [
-    ("r50_conv2_s2", 128, 128, (1, 3, 3), (1, 2, 2), (0, 1, 1), 2, 2, 16, 16),
-    ("r50_conv2_s2_odd", 64, 96, (1, 3, 3), (1, 2, 2), (0, 1, 1), 1, 3, 9, 7),
-    ("r50_ds_s2_odd", 64, 256, (1, 1, 1), (1, 2, 2), (0, 0, 0), 1, 2, 7, 9),
-    ("r50_ds_s2_T3", 256, 128, (1, 1, 1), (1, 2, 2), (0, 0, 0), 2, 3, 8, 8),
-    ("sp_4x4", 96, 208, (1, 3, 3), (1, 1, 1), (0, 1, 1), 2, 4, 4, 4),
+    ("tma64_pw_64_256", "tma", 64, 64, 256, (1, 1, 1), (1, 1, 1), (0, 0, 0), 2, 2, 7, 9),
+    ("tma64_pw_48_32", "tma", 64, 48, 32, (1, 1, 1), (1, 1, 1), (0, 0, 0), 2, 3, 5, 7),
+    ("tma128_pw_128_192", "tma", 128, 128, 192, (1, 1, 1), (1, 1, 1), (0, 0, 0), 2, 2, 9, 7),
+    ("tma128_pw_96_48", "tma", 128, 96, 48, (1, 1, 1), (1, 1, 1), (0, 0, 0), 1, 3, 6, 7),
+    ("tma192_pw_192_96", "tma", 192, 192, 96, (1, 1, 1), (1, 1, 1), (0, 0, 0), 2, 3, 7, 9),
+    ("tma192_pw_192_32", "tma", 192, 192, 32, (1, 1, 1), (1, 1, 1), (0, 0, 0), 2, 3, 6, 5),
+    ("tma256_pw_256_128", "tma", 256, 256, 128, (1, 1, 1), (1, 1, 1), (0, 0, 0), 2, 2, 5, 9),
+    ("tma256_pw_480_64", "tma", 256, 480, 64, (1, 1, 1), (1, 1, 1), (0, 0, 0), 2, 2, 8, 5),
+    ("tma192_sp_64_192", "tma", 192, 64, 192, (1, 3, 3), (1, 1, 1), (0, 1, 1), 2, 2, 8, 12),
+    ("tma192_sp_32_48", "tma", 192, 32, 48, (1, 3, 3), (1, 1, 1), (0, 1, 1), 1, 3, 8, 8),
+    ("tma192_tm_64_96", "tma", 192, 64, 96, (3, 1, 1), (1, 1, 1), (1, 0, 0), 2, 4, 6, 6),
+    ("tma192_tm_48_48", "tma", 192, 48, 48, (3, 1, 1), (1, 1, 1), (1, 0, 0), 2, 5, 5, 5),
+    # the stem's temporally strided (7,1,1) conv: taps 0,2,4,6 / 1,3,5 per frame parity, both at N = 256
+    ("tma256_stem_tm", "tma", 256, 64, 64, (7, 1, 1), (2, 1, 1), (3, 0, 0), 2, 6, 10, 12),
+    # the S3D space-to-depth stem (1,4,4): one slab serves all 16 taps
+    ("tma256_stem_s2d", "tma", 256, 12, 64, (1, 4, 4), (1, 1, 1), (0, 2, 0), 2, 3, 12, 24),
+    # shapes the TMA-staged kernel declines: spatially strided ResNet-50 convs, (1,3,3) on 4x4 frames, and the ResNet-50
+    # space-to-depth stem (5,4,4) with temporal stride 2
+    ("g128_r50_conv2_s2", "gather", 128, 128, 128, (1, 3, 3), (1, 2, 2), (0, 1, 1), 2, 2, 16, 16),
+    ("g128_r50_conv2_s2_odd", "gather", 128, 64, 96, (1, 3, 3), (1, 2, 2), (0, 1, 1), 1, 3, 9, 7),
+    ("g64_r50_ds_s2_odd", "gather", 64, 64, 256, (1, 1, 1), (1, 2, 2), (0, 0, 0), 1, 2, 7, 9),
+    ("g128_r50_ds_s2_T3", "gather", 128, 256, 128, (1, 1, 1), (1, 2, 2), (0, 0, 0), 2, 3, 8, 8),
+    ("g128_sp_4x4", "gather", 128, 96, 208, (1, 3, 3), (1, 1, 1), (0, 1, 1), 2, 4, 4, 4),
+    ("g128_r50_stem_s2d", "gather", 128, 12, 64, (5, 4, 4), (2, 1, 1), (2, 2, 0), 2, 5, 8, 12),
 ]
+WGRAD_IDS = [c[0] for c in WGRAD_CASES]
+
+
+def wgrad_bnk(Kreal):
+    """K-column tile width of the gather weight-gradient kernel: wgrad_bnk() in coclr_b200/csrc/conv_igemm.cu
+    (multiples of 64, at most 128, balanced over the tiles)."""
+    kt = (Kreal + 127) // 128
+    w = (Kreal + kt - 1) // kt
+    return (w + 63) // 64 * 64
+
+
+def wgrad_window(case):
+    """True for the space-to-depth stems (see WGRAD_CASES)."""
+    return case[5][1:] == (4, 4)
+
+
+def wgrad_dims(ops, case):
+    """(source T, H, W) and (destination To, Ho, Wo) of a weight-gradient case."""
+    name, kernel, width, Cin, Cout, k, s, p, B, T, H, W = case
+    geom = ops.Geometry(k, s, p)
+    if wgrad_window(case):
+        return (T, H, W + 4), (geom.out_dims(T, H, W + 4)[0], H, W)
+    return (T, H, W), geom.out_dims(T, H, W)
 
 
 @pytest.mark.parametrize("mag", MAGS)
 @pytest.mark.parametrize("npass", [3, 1])
-@pytest.mark.parametrize("case", WGRAD_CASES, ids=[c[0] for c in WGRAD_CASES])
-def test_wgrad_fp16_scaled_gather(case, npass, mag, diag):
+@pytest.mark.parametrize("case", WGRAD_CASES, ids=WGRAD_IDS)
+def test_wgrad_fp16_scaled(case, npass, mag, diag):
     """dW += (fp16 activation planes) x (fp16 planes of dY * s), times out_scale = 1/s, added to a dW that holds a
-    nonzero value."""
+    nonzero value, on the kernel instance the case names (the TMA-staged kernel with a NaN-poisoned workspace)."""
     from coclr_b200 import ops, lib as L
-    name, Cin, Cout, k, s, p, B, T, H, W = case
+    lib = L.load()
+    name, kernel, width, Cin, Cout, k, s, p, B, T, H, W = case
     geom = ops.Geometry(k, s, p)
-    To, Ho, Wo = geom.out_dims(T, H, W)
+    (Ts, Hs, Ws), (To, Ho, Wo) = wgrad_dims(ops, case)
     g = torch.Generator(device="cuda").manual_seed(3000 + sum(map(ord, name)) + npass)
     x = torch.relu(torch.randn(B, Cin, T, H, W, device="cuda", generator=g))
     dy = torch.randn(B, Cout, To, Ho, Wo, device="cuda", generator=g) * mag
     sc = _pow2_scale(dy)
-    xp, Cp, xcoff = _planes_of(ops, x, 0, lo=(npass > 1))
+    if wgrad_window(case):
+        xpad = F.pad(F.pad(x, (0, 0, 0, 0, 0, 0, 0, 16 - Cin)), (2, 2))
+        xp, Cp, xcoff = _planes_of(ops, xpad, 0, ld_extra=0, coff=0, lo=(npass > 1))
+    else:
+        xp, Cp, xcoff = _planes_of(ops, x, 0, lo=(npass > 1))
     dp, Cop, dcoff = _planes_of(ops, dy * sc, 0, lo=(npass > 1))
     out_scale = torch.tensor([1.0 / sc], device="cuda")
     wd = torch.zeros(Cout, Cin, *k, device="cuda", dtype=torch.float64, requires_grad=True)
+
+    def truth(xv, dyv):
+        (r,) = torch.autograd.grad(F.conv3d(xv, wd, stride=s, padding=p)[..., :Ho, :Wo], wd, dyv)
+        return r
+
     xv = xp.value()[..., xcoff:xcoff + Cin].permute(0, 4, 1, 2, 3).double()          # exact operand values
-    (ref,) = torch.autograd.grad(F.conv3d(xv, wd, stride=s, padding=p), wd, dy.double())
+    ref = truth(xv, dy.double())
     top = float(ref.abs().max())
     base = torch.randn(Cout, Cin, *k, device="cuda", generator=g) * top
     dw = base.clone()
-    src, dsrc = xp.src(xcoff, Cp, T, H, W), dp.src(dcoff, Cop, To, Ho, Wo)
-    wg = L.Wgrad(src, geom.c(0), dsrc, B, To, Ho, Wo, Cout, Cin, None, npass, 0, 0, 1, None)
-    assert L.load().coclr_wgrad_tma_plan(C.byref(wg), None) == 0, "shape taken by the TMA-staged kernel"
-    diag["kernel/wgrad_fp16/%s" % name] = "gather"
-    ops.conv_wgrad(src, 0, geom.c(0), dsrc, 0, B, (To, Ho, Wo), Cout, Cin, dw, npass=npass, out_scale=out_scale)
+    wg = L.Wgrad(xp.src(xcoff, Cp, Ts, Hs, Ws), geom.c(0), dp.src(dcoff, Cop, To, Ho, Wo), B, To, Ho, Wo, Cout, Cin,
+                 L.dptr(dw), npass, 0, 0, 1, L.dptr(out_scale))
+    info = (C.c_int * 8)()
+    if lib.coclr_wgrad_tma_plan(C.byref(wg), info) == 1:
+        ran = ("tma", info[3])
+        need = int(lib.coclr_wgrad_ws_floats(C.byref(wg)))
+        ws = torch.full((need,), float("nan"), device="cuda")       # every element read must have been written
+        wg.ws, wg.ws_floats = L.dptr(ws).value, need
+    else:
+        ran = ("gather", wgrad_bnk(geom.taps * Cp))
+    diag["kernel/wgrad_fp16/%s/p%d" % (name, npass)] = list(ran)
+    assert ran == (kernel, width), (name, ran)
+    L.check(lib.coclr_conv_wgrad(C.byref(wg), L.stream_ptr()), "coclr_conv_wgrad")
     torch.cuda.synchronize()
     got = dw.double() - base.double()
     errs = [_rel(got, ref)]
     if npass == 1:
         xh = xp.hi[..., xcoff:xcoff + Cin].double().permute(0, 4, 1, 2, 3)
         dh = dp.hi[..., dcoff:dcoff + Cout].double().permute(0, 4, 1, 2, 3) / sc
-        (ref_hi,) = torch.autograd.grad(F.conv3d(xh, wd, stride=s, padding=p), wd, dh)
-        errs.append(_rel(got, ref_hi))
+        errs.append(_rel(got, truth(xh, dh)))
     key = "wgrad_fp16/%s/p%d/m%g" % (name, npass, mag)
     diag[key] = errs
     if npass == 3:

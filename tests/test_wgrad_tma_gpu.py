@@ -2,9 +2,13 @@
   (a) float64 autograd of torch's conv3d on the exact plane values (what cuDNN's wgrad computes in the reference behind
       loss.backward(), main_nce.py:330, for backbone/s3dg.py:11-13,39-42), and
   (b) the cp.async gather kernel on the same inputs (coclr_set_wgrad_tma(0)).
-Shapes: every kind the kernel covers (1x1x1 / (1,3,3) / (3,1,1), stride 1), ragged tiles in every dimension, channel
-counts that are not multiples of 64, channel slices of wider (poisoned) buffers, Cout <= 64 (hi / lo stacked into one
-M = 128 operand) up to 384 (several cout groups), and the benchmark shapes at a small batch."""
+Shapes: every wgrad_tma_kernel<N, NPROD, BF16> instance (item width N = 64, 128, 192, 256; 1, 2 (stacked) or 3
+products per K step; fp16 and bf16), over the kinds 1x1x1 / (1,3,3) / (3,1,1) at stride 1, the temporally strided
+(7,1,1) stem and the space-to-depth window stem; ragged tiles in every dimension, channel counts that are not multiples
+of 64, channel slices of wider (poisoned) buffers, Cout <= 64 (hi / lo stacked into one M = 128 operand) up to 512
+(several cout groups), and the benchmark shapes at a small batch.  test_conv_bwd_scaled_plan_cpu.py checks that these
+cases reach all 24 instances.  Also: several launches back to back on one shared, larger workspace, as the engine runs
+them."""
 import ctypes as C
 
 import pytest
@@ -20,6 +24,10 @@ CASES = [
     ("pw_832_384", 832, 384, (1, 1, 1), (0, 0, 0), 4, 2, 4, 4),        # 13 channel chunks, 2 cout groups
     ("pw_480_16", 480, 16, (1, 1, 1), (0, 0, 0), 2, 2, 8, 8),
     ("pw_24_40", 24, 40, (1, 1, 1), (0, 0, 0), 1, 2, 5, 5),
+    ("pw_64_256", 64, 256, (1, 1, 1), (0, 0, 0), 2, 4, 7, 9),          # N = 64 with 2 cout groups: <64, 3>
+    ("pw_128_512", 128, 512, (1, 1, 1), (0, 0, 0), 2, 4, 9, 7),        # N = 128 (two n64 sub-blocks), 4 cout groups
+    ("pw_128_48", 128, 48, (1, 1, 1), (0, 0, 0), 2, 2, 5, 7),          # N = 128 stacked, partial cout block
+    ("pw_192_32", 192, 32, (1, 1, 1), (0, 0, 0), 2, 3, 6, 5),          # N = 192 stacked (Mixed_3b 192 -> 32)
     ("sp_64_192", 64, 192, (1, 3, 3), (0, 1, 1), 2, 2, 16, 16),        # Conv_2c.conv1
     ("sp_96_208", 96, 208, (1, 3, 3), (0, 1, 1), 2, 2, 8, 8),          # Mixed_4b.branch1.1.conv1: partial chunk, 4 blocks
     ("sp_16_48", 16, 48, (1, 3, 3), (0, 1, 1), 2, 3, 8, 8),
@@ -51,14 +59,10 @@ def _planes(ops, x_ncdhw, bf16, lo, coff, extra):
     return pl, C8
 
 
-@pytest.mark.parametrize("fmt", ["fp16", "bf16"])
-@pytest.mark.parametrize("npass", [3, 1])
-@pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
-def test_wgrad_tma_vs_float64_and_gather(case, npass, fmt, diag):
-    from coclr_b200 import ops, lib as L
-    lib = L.load()
+def _operands(ops, case, npass, bf16):
+    """Seeded planes of one case and the float64 truth: (xp, Cp, dp, Cop, ref, ref_hi); ref_hi (single pass only) is
+    the product of the hi planes alone."""
     name, Cin, Cout, k, p, B, T, H, W = case
-    bf16 = int(fmt == "bf16")
     lo = npass > 1
     g = torch.Generator(device="cuda").manual_seed(sum(ord(ch) for ch in name))
     x = torch.relu(torch.randn(B, Cin, T, H, W, device="cuda", generator=g))
@@ -69,6 +73,23 @@ def test_wgrad_tma_vs_float64_and_gather(case, npass, fmt, diag):
     dv = dp.value()[..., 16:16 + Cout].permute(0, 4, 1, 2, 3).double()
     wd = torch.zeros(Cout, Cin, *k, device="cuda", dtype=torch.float64, requires_grad=True)
     (ref,) = torch.autograd.grad(F.conv3d(xv, wd, padding=p), wd, dv)
+    ref_hi = None
+    if npass == 1:
+        xh = xp.hi.float()[..., 8:8 + Cin].permute(0, 4, 1, 2, 3).double()
+        dh = dp.hi.float()[..., 16:16 + Cout].permute(0, 4, 1, 2, 3).double()
+        (ref_hi,) = torch.autograd.grad(F.conv3d(xh, wd, padding=p), wd, dh)
+    return xp, Cp, dp, Cop, ref, ref_hi
+
+
+@pytest.mark.parametrize("fmt", ["fp16", "bf16"])
+@pytest.mark.parametrize("npass", [3, 1])
+@pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
+def test_wgrad_tma_vs_float64_and_gather(case, npass, fmt, diag):
+    from coclr_b200 import ops, lib as L
+    lib = L.load()
+    name, Cin, Cout, k, p, B, T, H, W = case
+    bf16 = int(fmt == "bf16")
+    xp, Cp, dp, Cop, ref, ref_hi = _operands(ops, case, npass, bf16)
     geom = ops.Geometry(k, (1, 1, 1), p)
     out_scale = torch.tensor([0.25], device="cuda")
     res = {}
@@ -95,9 +116,6 @@ def test_wgrad_tma_vs_float64_and_gather(case, npass, fmt, diag):
     # operands are exact; what remains is fp32 accumulation over B*T*H*W pixels (3 passes) or the dropped lo planes
     tol = 2e-5 if npass == 3 else (2e-2 if bf16 else 4e-3)
     if npass == 1:   # single pass: the reference for the kernel is the product of the hi planes alone
-        xh = xp.hi.float()[..., 8:8 + Cin].permute(0, 4, 1, 2, 3).double()
-        dh = dp.hi.float()[..., 16:16 + Cout].permute(0, 4, 1, 2, 3).double()
-        (ref_hi,) = torch.autograd.grad(F.conv3d(xh, wd, padding=p), wd, dh)
         assert _rel(res[2], ref_hi) < 2e-5, (_rel(res[2], ref_hi), "tma vs hi-plane product")
     assert e_ws < tol and e_gather < tol, (e_ws, e_gather)
     # the workspace epilogue is deterministic: a second run gives the same bits
@@ -108,6 +126,59 @@ def test_wgrad_tma_vs_float64_and_gather(case, npass, fmt, diag):
     L.check(lib.coclr_conv_wgrad(C.byref(wg), L.stream_ptr()), "coclr_conv_wgrad")
     torch.cuda.synchronize()
     assert torch.equal((dw2 - 0.5) * 4.0, res[2])
+
+
+# Launches that share one workspace, in this order: the widest first, then a stacked (3 passes) or single-block (mb = 1,
+# single pass) item, a (3,1,1) conv with several cout groups, and another small item after it
+SHARED_WS = ["pw_832_384", "sp_16_48", "tm_ragged", "pw_24_40"]
+
+
+@pytest.mark.parametrize("npass", [3, 1])
+def test_wgrad_tma_shared_workspace(npass, diag):
+    """The engine gives every weight gradient of a plan ONE workspace of the largest coclr_wgrad_ws_floats and runs them
+    back to back on one stream, so each launch finds the partial sums of the launches before it (wider items, other
+    row counts) where it does not write.  Each dW must be bit-equal to its run on a fresh NaN-poisoned workspace of
+    exactly its own size, and within the float64 bound."""
+    from coclr_b200 import ops, lib as L
+    lib = L.load()
+    by_name = {c[0]: c for c in CASES}
+    out_scale = torch.tensor([0.25], device="cuda")
+    runs = []
+    for name in SHARED_WS:
+        case = by_name[name]
+        _, Cin, Cout, k, p, B, T, H, W = case
+        xp, Cp, dp, Cop, ref, ref_hi = _operands(ops, case, npass, 0)
+        geom = ops.Geometry(k, (1, 1, 1), p)
+        dw_own = torch.full((Cout, Cin) + k, 0.5, device="cuda")
+        wg = L.Wgrad(xp.src(8, Cp, T, H, W), geom.c(0), dp.src(16, Cop, T, H, W), B, T, H, W, Cout, Cin, L.dptr(dw_own),
+                     npass, 0, 0, 1, L.dptr(out_scale))
+        info = (C.c_int * 8)()
+        assert lib.coclr_wgrad_tma_plan(C.byref(wg), info) == 1, name
+        need = int(lib.coclr_wgrad_ws_floats(C.byref(wg)))
+        own = torch.full((need,), float("nan"), device="cuda")
+        wg.ws, wg.ws_floats = L.dptr(own).value, need
+        L.check(lib.coclr_conv_wgrad(C.byref(wg), L.stream_ptr()), "coclr_conv_wgrad")
+        runs.append((name, wg, need, list(info), dw_own, ref, ref_hi, (xp, dp, own)))
+    torch.cuda.synchronize()
+    mbs = [r[3][4] for r in runs]
+    needs = [r[2] for r in runs]
+    # a smaller item (stacked, or mb = 1) follows a wider one
+    assert needs[0] == max(needs) and needs[1] < needs[0] and (mbs[1] == 1) == (npass == 1), (needs, mbs)
+    shared = torch.full((max(needs) + 4096,), float("nan"), device="cuda")     # poisoned once, larger than any need
+    outs = []
+    for name, wg, need, info, dw_own, ref, ref_hi, _ in runs:
+        dw = torch.full_like(dw_own, 0.5)
+        wg.dw = L.dptr(dw).value
+        wg.ws, wg.ws_floats = L.dptr(shared).value, shared.numel()
+        L.check(lib.coclr_conv_wgrad(C.byref(wg), L.stream_ptr()), "coclr_conv_wgrad")
+        outs.append(dw)
+    torch.cuda.synchronize()
+    for (name, wg, need, info, dw_own, ref, ref_hi, _), dw in zip(runs, outs):
+        got = (dw - 0.5) * 4.0
+        err = _rel(got, ref_hi if npass == 1 else ref)
+        diag["wgrad_tma/shared_ws/%s/p%d" % (name, npass)] = [err, info[3], info[4]]
+        assert torch.equal(dw, dw_own), (name, "differs from its run on its own workspace")
+        assert err < 2e-5, (name, err)
 
 
 def test_benchmark_shapes_take_the_tma_kernel():
