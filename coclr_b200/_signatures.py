@@ -45,6 +45,11 @@ EXPORTS = {
     "coclr_gate_bwd_apply": (I, [P, I, P, P, I, I, I, P]),
     "coclr_cls_head_fwd": (I, [P, P]),
     "coclr_cls_head_bwd": (I, [P, P]),
+    "coclr_video_accumulate": (I, [P, P, P, P, P, P, I, I, I, P]),
+    "coclr_video_finalize": (I, [P, P]),
+    "coclr_center_normalize": (I, [P, P, P, I, I, P]),
+    "coclr_sim_fp32": (I, [P, P, P, I, I, I, P]),
+    "coclr_retrieval_rank": (I, [P, P, P, I, I, P, I, P, P, P]),
 }
 
 

@@ -112,6 +112,13 @@ class ClsHead(C.Structure):
                 ("dbeta", C.c_void_p), ("dx", C.c_void_p), ("dfeat", C.c_void_p)]
 
 
+class VideoFinalize(C.Structure):
+    _fields_ = [("prob_sum", C.c_void_p), ("feat_sum", C.c_void_p), ("count", C.c_void_p),
+                ("Nv", C.c_int), ("C", C.c_int), ("D", C.c_int), ("n_views", C.c_int),
+                ("feat_mean", C.c_void_p), ("prob_mean", C.c_void_p), ("views_sum", C.c_void_p), ("prob", C.c_void_p),
+                ("target", C.c_void_p), ("rank", C.c_void_p), ("hits", C.c_void_p)]
+
+
 def library_path():
     return _LIB_PATH
 
@@ -133,7 +140,8 @@ def load():
 
 
 LAUNCHES = 0  # kernels of this library launched so far in this process (bench.py reports the per-step count)
-KERNELS_PER_CALL = {"coclr_bn_bwd": 2, "coclr_l2norm_bwd": 2, "coclr_conv_packed_bytes": 0, "coclr_gate_fc_bwd": 2, "coclr_wgrad_ws_floats": 0, "coclr_wgrad_tma_plan": 0}
+KERNELS_PER_CALL = {"coclr_bn_bwd": 2, "coclr_l2norm_bwd": 2, "coclr_conv_packed_bytes": 0, "coclr_gate_fc_bwd": 2, "coclr_wgrad_ws_floats": 0, "coclr_wgrad_tma_plan": 0,
+                    "coclr_center_normalize": 2}
 
 
 def kernels_of(fn, args):

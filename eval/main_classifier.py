@@ -10,12 +10,22 @@ train / validate loop, on the engine's LinearClassifier (model/classifier.py), p
 --train_what last (linear probe: l2norm + final BN, no dropout, frozen eval-mode backbone), ft (backbone at lr / 10)
 and all (everything at lr) select the parameters and learning rates as the reference does (:102-147); the optimizer is
 Adam with coupled L2 (--wd) as one launch per group over flat buffers (coclr_b200.moco.SpanAdam).  Accuracy and loss are
-accumulated on the device and read back every --print_freq steps.  --test / --retrieval / the multi-crop tests need
-the per-video LMDB datasets, --optim sgd and more than one GPU (the reference's nn.DataParallel) are not available:
-they raise.
+accumulated on the device and read back every --print_freq steps.
+
+--test CKPT with --retrieval (nearest-neighbour retrieval, R@1/5/10/20/50) or --center_crop / --five_crop / --ten_crop
+(per-video test accuracy over the crops) runs the reference's test paths (:170-208, :425-718) on the engine
+(coclr_b200.evaluate) and writes the reference's output files.  The per-video LMDB datasets and the PIL crop / scale /
+jitter transforms are not part of this repository, so these paths run with --synthetic only:
+
+  --synthetic-videos N   videos per split: seeded, 1-4 clips each, a per-class pattern so that the accuracies are well
+                         above chance; every (crop, flip) view of a video has its own deterministic content
+
+--optim sgd and more than one GPU (the reference's nn.DataParallel) are not available: they raise.
 """
 import argparse
+import json
 import os
+import pickle
 import random
 import sys
 import time
@@ -30,6 +40,7 @@ import torch.nn as nn  # noqa: E402
 
 from model.classifier import LinearClassifier  # noqa: E402
 from coclr_b200 import moco  # noqa: E402
+from coclr_b200 import evaluate as EV  # noqa: E402
 
 NUM_CLASS = {'ucf101': 101, 'hmdb51': 51, 'k400': 400, 'ucf101-f': 101, 'hmdb51-f': 51, 'k400-f': 400}   # :98-100
 
@@ -73,15 +84,16 @@ def parse_args(argv=None):
     p.add_argument('--synthetic', action='store_true')
     p.add_argument('--precision', default='parity', choices=['parity', 'mixed', 'fast'])
     p.add_argument('--steps-per-epoch', default=20, type=int)
+    p.add_argument('--synthetic-videos', default=24, type=int, help='videos per split of the synthetic test sets')
     return p.parse_args(argv)
 
 
 def check_supported(args):
     """Raise for what this driver does not run (see the module docstring)."""
     for flag in ('test', 'retrieval', 'center_crop', 'five_crop', 'ten_crop'):
-        if getattr(args, flag):
+        if getattr(args, flag) and not args.synthetic:
             raise NotImplementedError("--%s needs the per-video LMDB test datasets of the reference (dataset/), which are "
-                                      "not part of this repository" % flag)
+                                      "not part of this repository; run it with --synthetic" % flag)
     if args.optim != 'adam':
         raise NotImplementedError("--optim %s: only Adam is available (--optim adam)" % args.optim)
     if args.model != 'lincls':
@@ -171,6 +183,164 @@ def get_data(args, device, mode):
     return SyntheticClips(args, device, seed=args.seed_base + (0 if mode == 'train' else 1))
 
 
+class SyntheticVideos:
+    """Stand-in for the per-video test datasets: (video [3, T_total, img_dim, img_dim] in [0, 1], label, vname) for
+    --synthetic-videos videos of one split.  Video i has 1-4 clips plus 0 to seq_len - 1 leftover frames; its label is
+    i modulo a class count that gives every class about three videos per split.  The content is a per-class pattern
+    (the same in every split) under seeded per-video noise; `view` = (aug_idx, flip_idx) shifts the crop window and
+    flips it, standing in for the reference's FiveCrop / horizontal flip of each test view."""
+
+    def __init__(self, args, split, device, view=(5, 0)):
+        self.args, self.split, self.device, self.view = args, split, device, view
+        self.n_cls = max(1, min(args.num_class, args.synthetic_videos // 3))
+
+    def __len__(self):
+        return self.args.synthetic_videos
+
+    def _pattern(self, label):
+        a = self.args
+        g = torch.Generator(device=self.device).manual_seed(7919 + label)
+        return torch.rand(3, 1, a.img_dim, a.img_dim, device=self.device, generator=g) * 2 - 1
+
+    def __iter__(self):
+        a = self.args
+        base = 1000003 * (1 if self.split == 'test' else 2)
+        aug, flip = self.view
+        for i in range(a.synthetic_videos):
+            label = i % self.n_cls
+            g = torch.Generator(device=self.device).manual_seed(base + 31 * i)
+            n_clips = 1 + (i * 5 + (3 if self.split == 'test' else 0)) % 4
+            T = n_clips * a.seq_len + (i * 3) % a.seq_len
+            noise = torch.rand(3, T, a.img_dim, a.img_dim, device=self.device, generator=g) * 2 - 1
+            video = 0.5 + 0.3 * self._pattern(label) + 0.15 * noise
+            if aug != 5:
+                video = video.roll(shifts=(aug, 2 * aug), dims=(2, 3))
+            if flip:
+                video = video.flip(3)
+            vname = 'synthetic/c%03d/v_c%03d_%s%04d' % (label, label, self.split, i)
+            yield video.clamp_(0, 1), label, vname
+
+
+def load_test_checkpoint(model, args):
+    """:170-185: with --retrieval, a pre-training checkpoint's encoder_q.0. -> backbone. (map_pretrained) loaded
+    non-strict; otherwise strict, falling back to the checkpoint entries whose name and shape match."""
+    if not os.path.isfile(args.test):
+        raise FileNotFoundError("no checkpoint found at '%s'" % args.test)
+    print("=> loading testing checkpoint '%s'" % args.test)
+    ckpt = torch.load(args.test, map_location='cpu', weights_only=False)
+    state_dict = ckpt['state_dict']
+    if args.retrieval:
+        missing = load_pretrained(model, state_dict)
+        print("=> keys not in the checkpoint: %s" % missing)
+        return ckpt.get('epoch', 0)
+    try:
+        model.load_state_dict(state_dict)
+    except RuntimeError:
+        own = model.state_dict()
+        sd = {k: v for k, v in state_dict.items() if k in own and own[k].shape == v.shape}
+        missing = model.load_state_dict(sd, strict=False).missing_keys
+        print("=> non-strict load; keys not in the checkpoint: %s" % missing)
+    return ckpt.get('epoch', 0)
+
+
+def retrieval_paths(args):
+    """Output files of test_retrieval (:607-700) under dirname(--test)/<--dirname or 'feature'>/."""
+    d = os.path.join(os.path.dirname(args.test), args.dirname if args.dirname is not None else 'feature')
+    out = {'dir': d, 'sim': os.path.join(d, '%s_sim.pth.tar' % args.dataset)}
+    for split in ('test', 'train'):
+        for what, ext in (('feature', 'pth.tar'), ('label', 'pth.tar'), ('vname', 'pkl')):
+            out[split, what] = os.path.join(d, '%s_%s_%s.%s' % (args.dataset, split, what, ext))
+    return out
+
+
+def vname_records(vnames):
+    """What the reference pickles: the vname of every batch of one video under default collation, i.e. a list of
+    one-element lists."""
+    return [[v] for v in vnames]
+
+
+def test_retrieval(model, args, device):
+    paths = retrieval_paths(args)
+    feats = {}
+    for split in ('test', 'train'):                      # test first, then train, as the reference
+        if os.path.exists(paths[split, 'feature']):
+            feats[split] = (torch.load(paths[split, 'feature']).to(device), torch.load(paths[split, 'label']).to(device))
+            continue
+        os.makedirs(paths['dir'], exist_ok=True)
+        print('Computing %s set feature ... ' % split)
+        res = EV.evaluate(model, SyntheticVideos(args, split, device), args.seq_len, args.batch_size, args.num_seq)
+        print(res.feature.size())
+        torch.save(res.feature.cpu(), paths[split, 'feature'])
+        torch.save(res.label.cpu(), paths[split, 'label'])
+        with open(paths[split, 'vname'], 'wb') as fp:
+            pickle.dump(vname_records(res.vname), fp)
+        feats[split] = (res.feature, res.label)
+    sim, _, accs = EV.retrieval(feats['test'][0], feats['test'][1], feats['train'][0], feats['train'][1])
+    torch.save(sim.cpu(), paths['sim'])
+    for k, acc in zip(EV.RETRIEVAL_KS, accs):
+        print('%dNN acc = %.4f' % (k, acc))
+    return accs
+
+
+def crop_schedule(args):
+    """test_10crop's views (:431-442, :453-512): [(flip_idx, aug_idx, [titles of the summaries written after it])] and
+    the mode's title.  The final summary is always written as 'ten' (:515), whatever the mode."""
+    if args.ten_crop:
+        augs, flips, title = [5, 1, 2, 3, 4], [0, 1], 'ten'
+    elif args.five_crop:
+        augs, flips, title = [5, 1, 2, 3, 4], [0], 'five'
+    else:
+        augs, flips, title = [5], [0], 'center'
+    views = []
+    for flip_idx in flips:
+        for aug_idx in augs:
+            after = []
+            if title == 'ten' and flip_idx == 0 and aug_idx == 5:
+                after.append('center')
+            if title == 'ten' and flip_idx == 0 and aug_idx == augs[-1]:
+                after.append('five')
+            views.append((flip_idx, aug_idx, after))
+    views[-1][2].append('ten')
+    return views, title
+
+
+def prob_json_path(test, title):
+    return os.path.join(os.path.dirname(test), '%s-prob-%s.json' % (os.path.basename(test), title))
+
+
+def summarize_probability(res, test, title):
+    """summarize_probability (:524-545) from the engine's per-video means: {vname: {'mean_prob': [[...C...]]}}."""
+    print('Mean: Acc@1: %.4f Acc@5: %.4f' % (res.top1, res.top5))
+    prob = res.prob.cpu().tolist()
+    stat = {v: {'mean_prob': [p]} for v, p in zip(res.vname, prob)}
+    with open(prob_json_path(test, title), 'w') as fp:
+        json.dump(stat, fp)
+    return res.top1, res.top5
+
+
+def test_10crop(model, args, device):
+    views, title = crop_schedule(args)
+    print('Test using %s crop' % {'center': 'center', 'five': '5', 'ten': '10'}[title])
+    res, summaries = None, []
+    for flip_idx, aug_idx, after in views:
+        print('Aug type: %d; flip: %d' % (aug_idx, flip_idx))
+        res = EV.evaluate(model, SyntheticVideos(args, 'test', device, view=(aug_idx, flip_idx)), args.seq_len,
+                          args.batch_size, args.num_seq, previous=res)
+        for t in after:
+            print('%s-crop result:' % (title if t == 'ten' else t))
+            summaries.append((t, summarize_probability(res, args.test, t)))
+    return summaries
+
+
+def run_test(model, args, device):
+    load_test_checkpoint(model, args)
+    if args.retrieval:
+        return test_retrieval(model, args, device)
+    if args.center_crop or args.five_crop or args.ten_crop:
+        return test_10crop(model, args, device)
+    raise NotImplementedError("--test needs --retrieval or one of --center_crop / --five_crop / --ten_crop")
+
+
 def set_path(args):
     if args.resume:
         exp_path = os.path.dirname(os.path.dirname(args.resume))
@@ -245,6 +415,8 @@ def main(args):
     args.seed_base = 0
     args.num_class = NUM_CLASS[args.dataset]
     model = build_model(args).to(device)
+    if args.test:
+        return run_test(model, args, device)
     optimizer = build_optimizer(model, args)
     criterion = nn.CrossEntropyLoss()
     args.iteration = 1

@@ -390,6 +390,38 @@ typedef struct {
 int coclr_cls_head_fwd(const coclr_cls_head_t* h, coclr_stream_t stream);
 int coclr_cls_head_bwd(const coclr_cls_head_t* h, coclr_stream_t stream);
 
+/* ---- Video-level evaluation (eval/main_classifier.py --test of the reference: test_10crop :425-545 and
+ * test_retrieval :548-718).  fp32 throughout, every sum in a fixed order; the only atomics are integer hit counters,
+ * so results are bit-identical from run to run.
+ *   coclr_video_accumulate: one pass of B clips.  slot[b] (int32) is the video slot of clip b, -1 for a padding clip;
+ *     the clips of one video are consecutive.  In clip order: prob_sum[v] += softmax(logits[b]) (max subtracted),
+ *     feat_sum[v] += feat[b], count[v] += 1.  Sums carry over from pass to pass.
+ *   coclr_video_finalize: per video v, feat_mean = feat_sum / count (skipped when feat_mean is NULL),
+ *     prob_mean = prob_sum / count (this view's softmax(logit).mean(0)), views_sum += prob_mean, and
+ *     prob = views_sum / n_views (the mean over the views so far).  With target: rank[v] = the number of classes
+ *     ranked above the target in prob (higher probability, ties to the lower index); hits[0] += rank < 1,
+ *     hits[1] += rank < 5.  A target outside [0, C) gets rank C and no hit (the reference scores it as a miss).
+ *   coclr_center_normalize: y = F.normalize(x - x.mean(0), dim=1, eps=1e-12); mean [D] receives the column mean.
+ *   coclr_sim_fp32: sim [Nq, Nk] = q [Nq, D] . k [Nk, D]^T on fp32 FFMA (D % 4 == 0, 16-byte aligned pointers).
+ *   coclr_retrieval_rank: rank[i] = position of query i's best same-label item in the order (sim descending, index
+ *     ascending), Nk when there is none; hits[m] += rank < ks[m] for the nks (<= COCLR_MAX_KS) values of ks, never for
+ *     a query with no same-label item (so a k above Nk counts the queries that have one). */
+#define COCLR_MAX_KS 8
+typedef struct {
+  const float* prob_sum; const float* feat_sum; const int* count;   /* [Nv, C], [Nv, D], [Nv] */
+  int Nv, C, D, n_views;
+  float* feat_mean; float* prob_mean;                               /* [Nv, D], [Nv, C] */
+  float* views_sum; float* prob;                                    /* [Nv, C] */
+  const long* target; int* rank; int* hits;                         /* [Nv] int64, [Nv], [2] (+=) */
+} coclr_video_finalize_t;
+int coclr_video_accumulate(const float* logits, const float* feat, const int* slot, float* prob_sum, float* feat_sum,
+                           int* count, int B, int C, int D, coclr_stream_t stream);
+int coclr_video_finalize(const coclr_video_finalize_t* a, coclr_stream_t stream);
+int coclr_center_normalize(const float* x, float* y, float* mean, int N, int D, coclr_stream_t stream);
+int coclr_sim_fp32(const float* q, const float* k, float* sim, int Nq, int Nk, int D, coclr_stream_t stream);
+int coclr_retrieval_rank(const float* sim, const long* qlabel, const long* klabel, int Nq, int Nk, const int* ks,
+                         int nks, int* rank, int* hits, coclr_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -164,10 +164,11 @@ class LinearClassifier(nn.Module):
                     p.grad = g
 
     # -- forward / backward -----------------------------------------------------------------------------
-    def _run(self, block, backbone_grad):
+    def _run(self, block, backbone_grad, batch_index=None, batch=None, norm=None):
         eng = self._engine_for(block.device)
-        B, fs = block.shape[0], self.param['feature_size']
-        plan = eng.forward(block, training=self.backbone.training, with_backward=backbone_grad)
+        B, fs = block.shape[0] if batch is None else batch, self.param['feature_size']
+        plan = eng.forward(block, training=self.backbone.training, with_backward=backbone_grad,
+                           batch_index=batch_index, batch=batch, norm=norm)
         f32 = dict(dtype=torch.float32, device=block.device)
         hd = {"feat": plan.feat.clone()}
         bn_train = self.use_final_bn and self.final_bn.training
@@ -228,4 +229,16 @@ class LinearClassifier(nn.Module):
             return _ClassifierFn.apply(self._anchor, self, block, backbone_grad)
         with torch.no_grad():
             logits, feat3d, _, _ = self._run(block, False)
+        return logits, feat3d
+
+    @torch.no_grad()
+    def infer(self, x, batch_index=None, batch=None, norm=None):
+        """Inference only (no autograd node, no backward plan): (logit, feat3d) of the clips
+        x[batch_index[b]] (b < batch; x[b] without an index), as forward() would return for them.  x is
+        [*, C, T, H, W] with free batch and channel strides (a strided view into a larger buffer is fine);
+        norm = (mean, std) device fp32 [C] applies the per-channel (x - mean) / std while the engine packs the input.
+        Each submodule's `training` flag is honoured as in forward()."""
+        if not x.is_cuda:
+            raise L.CoclrError("coclr_b200 classifiers run on CUDA (sm_90a) only; there is no CPU path")
+        logits, feat3d, _, _ = self._run(x, False, batch_index=batch_index, batch=batch, norm=norm)
         return logits, feat3d
