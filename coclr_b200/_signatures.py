@@ -50,6 +50,8 @@ EXPORTS = {
     "coclr_center_normalize": (I, [P, P, P, I, I, P]),
     "coclr_sim_fp32": (I, [P, P, P, I, I, I, P]),
     "coclr_retrieval_rank": (I, [P, P, P, I, I, P, I, P, P, P]),
+    "coclr_probe_work_floats": (LG, [P]),
+    "coclr_probe_run": (I, [P, P]),
 }
 
 

@@ -119,6 +119,19 @@ class VideoFinalize(C.Structure):
                 ("target", C.c_void_p), ("rank", C.c_void_p), ("hits", C.c_void_p)]
 
 
+class Probe(C.Structure):
+    _fields_ = [("N", C.c_int), ("Nq", C.c_int), ("D", C.c_int), ("C", C.c_int), ("S", C.c_int),
+                ("epochs", C.c_int), ("batch", C.c_int), ("eval_freq", C.c_int), ("final_bn", C.c_int),
+                ("momentum", C.c_float), ("eps", C.c_float),
+                ("train", C.c_void_p), ("train_label", C.c_void_p), ("test", C.c_void_p), ("test_label", C.c_void_p),
+                ("order", C.c_void_p), ("lr", C.c_void_p), ("wd", C.c_void_p),
+                ("W", C.c_void_p), ("bias", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p),
+                ("W_buf", C.c_void_p), ("bias_buf", C.c_void_p), ("gamma_buf", C.c_void_p), ("beta_buf", C.c_void_p),
+                ("running_mean", C.c_void_p), ("running_var", C.c_void_p), ("work", C.c_void_p),
+                ("train_loss", C.c_void_p), ("train_hits", C.c_void_p), ("val_loss", C.c_void_p),
+                ("val_hits", C.c_void_p), ("prob", C.c_void_p)]
+
+
 def library_path():
     return _LIB_PATH
 

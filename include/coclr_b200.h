@@ -422,6 +422,43 @@ int coclr_sim_fp32(const float* q, const float* k, float* sim, int Nq, int Nk, i
 int coclr_retrieval_rank(const float* sim, const long* qlabel, const long* klabel, int Nq, int Nk, const int* ks,
                          int nks, int* rank, int* hits, coclr_stream_t stream);
 
+/* ---- Linear probe on extracted features (eval/feature_linear_probe.py of the reference): optional BatchNorm1d
+ * (final_bn) + Linear, cross-entropy, SGD (momentum 0.9, coupled weight decay on every parameter), trained for S
+ * (lr, wd) configs at once over the same batches.  One call enqueues the whole run -- every epoch, every evaluation --
+ * with no host synchronisation and no allocation.  fp32, every sum in a fixed order, no float atomics: config s gives
+ * the same bits from run to run and as a run of that config alone (S = 1).
+ *   Training step t of epoch e: the B = min(batch, N - t * batch) train rows order[e, t * batch ..]; with final_bn the
+ *   batch mean / biased variance normalise the rows and update running_mean / running_var (momentum, unbiased
+ *   variance, shared by all configs); logits = x_hat . (W * gamma)^T + W . beta + bias; loss and top-1 hit per row
+ *   (ties to the lower class); the gradients of the batch-mean loss; then per config p -= lr[e, s] * buf with
+ *   buf = 0.9 buf + grad + wd[s] p.
+ *   After epoch e with e % eval_freq == 0, and once after the last epoch: eval mode (running statistics) over the test
+ *   set.  The final pass also writes softmax probabilities to prob.
+ * Per-chunk outputs (layout [slot, S]): train_loss / train_hits get the sum of the per-row losses and the hit count of
+ * each training step (slot e * steps + t, steps = ceil(N / batch)); val_loss / val_hits those of each chunk of `batch`
+ * test rows (slot v * ceil(Nq / batch) + chunk for the v-th evaluation, the final pass last).
+ * Requirements (COCLR_E_ARG otherwise): D % 4 == 0, 16-byte aligned train / test / W / work; with final_bn no
+ * training batch of one row (N % batch != 1).  Indices and labels are not range-checked on the device: order holds
+ * rows in [0, N), train labels and test labels lie in [0, C).  work: coclr_probe_work_floats(p) floats. */
+typedef struct {
+  int N, Nq, D, C, S;                         /* train rows, test rows, feature width, classes, configs */
+  int epochs, batch, eval_freq, final_bn;
+  float momentum, eps;                        /* BatchNorm1d: 0.1, 1e-5 */
+  const float* train; const long* train_label;   /* [N, D], [N] int64 */
+  const float* test; const long* test_label;     /* [Nq, D], [Nq] int64 */
+  const int* order;                           /* [epochs, N] int32: each epoch's train rows in batch order */
+  const float* lr; const float* wd;           /* [epochs, S], [S] */
+  float* W; float* bias; float* gamma; float* beta;               /* [S, C, D], [S, C], [S, D], [S, D] (updated) */
+  float* W_buf; float* bias_buf; float* gamma_buf; float* beta_buf;   /* momentum buffers, zero on entry */
+  float* running_mean; float* running_var;    /* [D] */
+  float* work;
+  double* train_loss; int* train_hits;        /* [epochs * steps, S] */
+  double* val_loss; int* val_hits;            /* [(evaluations + 1) * ceil(Nq / batch), S] */
+  float* prob;                                /* [S, Nq, C] */
+} coclr_probe_t;
+long coclr_probe_work_floats(const coclr_probe_t* p);
+int coclr_probe_run(const coclr_probe_t* p, coclr_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
