@@ -52,6 +52,8 @@ EXPORTS = {
     "coclr_retrieval_rank": (I, [P, P, P, I, I, P, I, P, P, P]),
     "coclr_probe_work_floats": (LG, [P]),
     "coclr_probe_run": (I, [P, P]),
+    "coclr_augment_smem_bytes": (C.c_size_t, [P]),
+    "coclr_augment": (I, [P, P]),
 }
 
 

@@ -132,6 +132,14 @@ class Probe(C.Structure):
                 ("val_hits", C.c_void_p), ("prob", C.c_void_p)]
 
 
+class Augment(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("B", C.c_int), ("F", C.c_int), ("Hmax", C.c_int), ("Wmax", C.c_int),
+                ("S", C.c_int), ("D", C.c_int), ("K", C.c_int), ("band_rows", C.c_int),
+                ("clips", C.c_void_p), ("coef", C.c_void_p), ("bounds", C.c_void_p), ("gray", C.c_void_p),
+                ("out", C.c_void_p), ("out_batch_stride", C.c_long), ("out_clip_stride", C.c_long),
+                ("out_chan_stride", C.c_long)]
+
+
 def library_path():
     return _LIB_PATH
 
@@ -154,7 +162,8 @@ def load():
 
 LAUNCHES = 0  # kernels of this library launched so far in this process (bench.py reports the per-step count)
 KERNELS_PER_CALL = {"coclr_bn_bwd": 2, "coclr_l2norm_bwd": 2, "coclr_conv_packed_bytes": 0, "coclr_gate_fc_bwd": 2, "coclr_wgrad_ws_floats": 0, "coclr_wgrad_tma_plan": 0,
-                    "coclr_center_normalize": 2}
+                    "coclr_center_normalize": 2,
+                    "coclr_augment_smem_bytes": 0}
 
 
 def kernels_of(fn, args):

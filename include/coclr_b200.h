@@ -459,6 +459,48 @@ typedef struct {
 long coclr_probe_work_floats(const coclr_probe_t* p);
 int coclr_probe_run(const coclr_probe_t* p, coclr_stream_t stream);
 
+/* Pre-training augmentation (reference utils/augmentation.py, get_transform('train') of main_nce.py / main_coclr.py):
+ * for every sample b and clip c in {0, 1} (the q and k clips), S frames starting at source frame clips[b, c].src_frame
+ * are cropped and bicubic-resized to D x D, colour-jittered, gray-split, blurred and flipped as PIL does, then written
+ * as float32 x / 255.  Output bits equal the reference's ToTensor output for the same decisions.
+ * One CTA per output frame; dynamic shared memory coclr_augment_smem_bytes(p) (at most 227 KB).
+ *
+ * src     uint8 [B, F, Hmax, Wmax, 3] (channels last); every coordinate the tables name lies inside the sample's frames
+ * clips   [B, 2] records (below); coclr_b200/augment.py builds them and the tables from a host plan
+ * coef    int32 [B, 2, 2, K, D]: per clip, axis (0 = x, 1 = y), tap k and output pixel o, Pillow's 22-bit bicubic
+ *         coefficient of source pixel start + k (zero past count)
+ * bounds  int32 [B, 2, 2, 2, D]: per clip and axis, start[D] (absolute source coordinate, crop offset included) then
+ *         count[D]; both nondecreasing in o, as Pillow's are
+ * gray    int8 [B, 2, S]: channel replicated into all three for that frame, -1 for none
+ * out     frame f of clip c of sample b, channel ch at out + b * out_batch_stride + c * out_clip_stride +
+ *         ch * out_chan_stride + f * D * D, rows of D floats: [B, 3, 2S, D, D] or [B, 2, 3, S, D, D]
+ * Requirements (COCLR_E_ARG otherwise): band_rows >= max(D, K) (the horizontal resize pass is done in bands of at most
+ * band_rows source rows), F >= 2S, shared memory within 227 KB.  Table contents are not range-checked on the device. */
+typedef struct {
+  int src_frame;                  /* first source frame of the clip */
+  int n_ops;                      /* ColorJitter ops applied (0: no jitter) */
+  int op[4];                      /* in application order: 0 brightness, 1 contrast, 2 saturation, 3 hue */
+  float factor[3];                /* float32 blend factor of brightness, contrast, saturation */
+  int hue_shift;                  /* byte added to PIL's H plane, mod 256 */
+  int blur_radius;                /* integer box radius of GaussianBlur, -1: no blur */
+  unsigned blur_ww, blur_fw;      /* BoxBlur.c 24-bit window and edge weights */
+  int flip;
+  int pad[2];
+} coclr_augment_clip_t;
+typedef struct {
+  const uint8_t* src;
+  int B, F, Hmax, Wmax;
+  int S, D, K, band_rows;         /* frames per clip, output side, taps per output pixel, rows per resize band */
+  const coclr_augment_clip_t* clips;
+  const int* coef;
+  const int* bounds;
+  const int8_t* gray;
+  float* out;
+  long out_batch_stride, out_clip_stride, out_chan_stride;
+} coclr_augment_t;
+size_t coclr_augment_smem_bytes(const coclr_augment_t* p);
+int coclr_augment(const coclr_augment_t* p, coclr_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

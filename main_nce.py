@@ -3,10 +3,13 @@
 hot path this repository accelerates, plus:
 
   --synthetic            random clips of the dataset's shape instead of the LMDB loaders (the reference's dataset/
-                         and utils/augmentation.py pipeline is outside the accelerated path; without --synthetic a
-                         dataset name raises, because lmdb/msgpack are not part of this repository)
+                         readers are outside the accelerated path; without --synthetic a dataset name raises, because
+                         lmdb/msgpack are not part of this repository)
   --precision MODE       parity | mixed | fast (see DESIGN.md)
   --steps-per-epoch N    length of a synthetic epoch
+  --gpu-augment          with --synthetic: the loader yields seeded uint8 source frames (--source-size H W, 240 320 by
+                         default) and the reference's get_transform('train') runs on the GPU (coclr_b200.augment); the
+                         clips go to the model in loader layout with the input normalisation fused
 
 Launch like the reference: `python -m torch.distributed.run --nproc_per_node=N main_nce.py ...` (one process per
 GPU; --local_rank, --local-rank and the LOCAL_RANK env variable are all accepted).
@@ -75,6 +78,10 @@ def parse_args(argv=None):
     p.add_argument('--raw-input', action='store_true',
                    help='feed the loader layout [B,3,num_seq*seq_len,H,W] in [0,1]; T.Normalize + view + transpose of the '
                         'reference\'s GPU-side `tr` (main_nce.py:207-209,299-302) run fused in the clip-packing kernel')
+    p.add_argument('--gpu-augment', action='store_true',
+                   help='with --synthetic: augment seeded uint8 source frames on the GPU (get_transform("train"))')
+    p.add_argument('--source-size', default=[240, 320], nargs=2, type=int, metavar=('H', 'W'),
+                   help='height and width of the synthetic source frames of --gpu-augment')
     p.add_argument('--precision', default='parity', choices=['parity', 'mixed', 'fast'])
     p.add_argument('--steps-per-epoch', default=20, type=int)
     p.add_argument('--num-classes', default=101, type=int, help='label range of the synthetic UberNCE labels')
@@ -121,13 +128,41 @@ class SyntheticClips:
         return self.args.steps_per_epoch
 
 
+class SyntheticSourceFrames:
+    """--gpu-augment: seeded uint8 source frames [B, F, H, W, 3] (what stacked decoded JPEGs give) augmented on the
+    GPU by the reference's get_transform('train').  The augmentation draws from its own random / np.random / torch
+    generators, as the reference's do in its DataLoader workers, so the training loop's draws are unchanged."""
+
+    def __init__(self, args, device, two_stream=False):
+        from coclr_b200.augment import PretrainAugment
+        self.args, self.device = args, device
+        self.aug = PretrainAugment(args.seq_len, args.img_dim, two_stream=two_stream)
+        seed = args.seed * 1000 + args.rank
+        self.gen = torch.Generator(device=device).manual_seed(seed)
+        self.py, self.np = random.Random(seed), np.random.RandomState(seed)
+        self.tg = torch.Generator().manual_seed(seed)
+
+    def __iter__(self):
+        a = self.args
+        h, w = a.source_size
+        for _ in range(a.steps_per_epoch):
+            frames = torch.randint(0, 256, (a.batch_size, self.aug.frames, h, w, 3), dtype=torch.uint8,
+                                   device=self.device, generator=self.gen)
+            plan = self.aug.plan([(h, w)] * a.batch_size, self.py, self.np, self.tg)
+            y = torch.randint(0, a.num_classes, (a.batch_size,), device=self.device, generator=self.gen)
+            yield self.aug(frames, plan), y
+
+    def __len__(self):
+        return self.args.steps_per_epoch
+
+
 def get_data(args, device):
     if not args.synthetic:
         raise NotImplementedError(
-            "dataset %r: the LMDB/JPEG loaders and PIL augmentations of the reference (dataset/, utils/augmentation.py) "
-            "are outside the accelerated hot path; run with --synthetic, or feed [B,2,3,T,H,W] float tensors from "
+            "dataset %r: the LMDB/JPEG loaders of the reference (dataset/) are outside the accelerated hot path; run "
+            "with --synthetic, or feed [B,2,3,T,H,W] float tensors (or uint8 frames through coclr_b200.augment) from "
             "your own loader" % args.dataset)
-    return SyntheticClips(args, device)
+    return SyntheticSourceFrames(args, device) if args.gpu_augment else SyntheticClips(args, device)
 
 
 def adjust_learning_rate(optimizer, epoch, args):
@@ -253,7 +288,7 @@ def main_worker(args):
     random.seed(args.seed)
     cls = {'infonce': InfoNCE, 'ubernce': UberNCE}[args.model]
     model = cls(args.net, args.moco_dim, args.moco_k, args.moco_m, args.moco_t, precision=args.precision).to(device)
-    if args.raw_input:
+    if args.raw_input or args.gpu_augment:
         model.set_input_transform(mean=[0.485, 0.456, 0.406], std=[0.229, 0.224, 0.225])   # reference main_nce.py:207-209
     optimizer = moco.FlatAdam(model.encoder_q, lr=args.lr, weight_decay=args.wd)
     args.iteration = 1
