@@ -54,6 +54,8 @@ EXPORTS = {
     "coclr_probe_run": (I, [P, P]),
     "coclr_augment_smem_bytes": (C.c_size_t, [P]),
     "coclr_augment": (I, [P, P]),
+    "coclr_augment_clf_smem_bytes": (C.c_size_t, [P]),
+    "coclr_augment_clf": (I, [P, P]),
 }
 
 

@@ -140,6 +140,14 @@ class Augment(C.Structure):
                 ("out_chan_stride", C.c_long)]
 
 
+class AugmentClf(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("NF", C.c_int), ("Hmax", C.c_int), ("Wmax", C.c_int), ("n_frames", C.c_int),
+                ("frames", C.c_void_p), ("samples", C.c_void_p),
+                ("M", C.c_int), ("D", C.c_int), ("K1", C.c_int), ("K2", C.c_int), ("band_rows", C.c_int),
+                ("rows", C.c_int), ("coef1", C.c_void_p), ("bounds1", C.c_void_p), ("coef2", C.c_void_p),
+                ("bounds2", C.c_void_p), ("out", C.c_void_p)]
+
+
 def library_path():
     return _LIB_PATH
 
@@ -163,7 +171,7 @@ def load():
 LAUNCHES = 0  # kernels of this library launched so far in this process (bench.py reports the per-step count)
 KERNELS_PER_CALL = {"coclr_bn_bwd": 2, "coclr_l2norm_bwd": 2, "coclr_conv_packed_bytes": 0, "coclr_gate_fc_bwd": 2, "coclr_wgrad_ws_floats": 0, "coclr_wgrad_tma_plan": 0,
                     "coclr_center_normalize": 2,
-                    "coclr_augment_smem_bytes": 0}
+                    "coclr_augment_smem_bytes": 0, "coclr_augment_clf_smem_bytes": 0}
 
 
 def kernels_of(fn, args):

@@ -14,11 +14,19 @@ accumulated on the device and read back every --print_freq steps.
 
 --test CKPT with --retrieval (nearest-neighbour retrieval, R@1/5/10/20/50) or --center_crop / --five_crop / --ten_crop
 (per-video test accuracy over the crops) runs the reference's test paths (:170-208, :425-718) on the engine
-(coclr_b200.evaluate) and writes the reference's output files.  The per-video LMDB datasets and the PIL crop / scale /
-jitter transforms are not part of this repository, so these paths run with --synthetic only:
+(coclr_b200.evaluate) and writes the reference's output files.  The per-video LMDB datasets are not part of this
+repository, so these paths run with --synthetic only (the PIL crop / scale / jitter transforms run on the GPU with
+--gpu-augment):
 
   --synthetic-videos N   videos per split: seeded, 1-4 clips each, a per-class pattern so that the accuracies are well
                          above chance; every (crop, flip) view of a video has its own deterministic content
+
+  --gpu-augment          with --synthetic: seeded uint8 source frames (--source-size H W, 240 320 by default) go through
+                         the reference's PIL transforms on the GPU (coclr_b200.clf_augment): get_transform('train' /
+                         'val') with the train batch's flip for training and validation, and the flip / FiveCrop /
+                         CenterCrop / Scale / ColorJitter views of --test; the test videos carry the per-class pattern
+                         at source resolution.  Training feeds [0, 1] clips with the input normalisation fused
+                         (LinearClassifier.set_input_transform)
 
 --optim sgd and more than one GPU (the reference's nn.DataParallel) are not available: they raise.
 """
@@ -85,6 +93,10 @@ def parse_args(argv=None):
     p.add_argument('--precision', default='parity', choices=['parity', 'mixed', 'fast'])
     p.add_argument('--steps-per-epoch', default=20, type=int)
     p.add_argument('--synthetic-videos', default=24, type=int, help='videos per split of the synthetic test sets')
+    p.add_argument('--gpu-augment', action='store_true',
+                   help='with --synthetic: augment seeded uint8 source frames on the GPU (the reference\'s transforms)')
+    p.add_argument('--source-size', default=[240, 320], nargs=2, type=int, metavar=('H', 'W'),
+                   help='height and width of the synthetic source frames of --gpu-augment')
     return p.parse_args(argv)
 
 
@@ -180,7 +192,41 @@ def get_data(args, device, mode):
             "dataset %r: the LMDB loaders and PIL augmentations of the reference (dataset/, utils/augmentation.py) are "
             "outside the accelerated hot path; run with --synthetic, or feed [B,3,T,H,W] float tensors from your own "
             "loader" % args.dataset)
-    return SyntheticClips(args, device, seed=args.seed_base + (0 if mode == 'train' else 1))
+    seed = args.seed_base + (0 if mode == 'train' else 1)
+    if args.gpu_augment:
+        return SyntheticSourceClips(args, device, seed, mode)
+    return SyntheticClips(args, device, seed=seed)
+
+
+class SyntheticSourceClips:
+    """--gpu-augment: seeded uint8 source frames [B, num_seq * seq_len, H, W, 3] (what stacked decoded JPEGs give) and
+    labels, augmented on the GPU by get_transform(mode) (coclr_b200.clf_augment).  The augmentation draws from its own
+    random.Random, as the reference's DataLoader workers do; the train batch's flip (T.RandomHorizontalFlip of
+    transform_train_cuda) is drawn from `random` itself, where the reference's main process draws it."""
+
+    def __init__(self, args, device, seed, mode):
+        from coclr_b200.clf_augment import ClassifierAugment
+        self.args, self.device, self.mode = args, device, mode
+        self.aug = ClassifierAugment(mode, args.seq_len, args.img_dim, num_seq=args.num_seq)
+        self.gen = torch.Generator(device=device).manual_seed(seed)
+        self.py = random.Random(seed)
+
+    def __iter__(self):
+        a = self.args
+        h, w = a.source_size
+        for _ in range(a.steps_per_epoch):
+            frames = torch.randint(0, 256, (a.batch_size, self.aug.frames, h, w, 3), dtype=torch.uint8,
+                                   device=self.device, generator=self.gen)
+            y = torch.randint(0, a.num_class, (a.batch_size,), device=self.device, generator=self.gen)
+            plan = self.aug.plan([(h, w)] * a.batch_size, self.py)
+            if self.mode == 'train':
+                flip = random.random() < 0.5                       # transform_train_cuda's T.RandomHorizontalFlip
+                for sp in plan.samples:
+                    sp.flip = flip
+            yield self.aug(frames, plan), y
+
+    def __len__(self):
+        return self.args.steps_per_epoch
 
 
 class SyntheticVideos:
@@ -219,6 +265,53 @@ class SyntheticVideos:
                 video = video.flip(3)
             vname = 'synthetic/c%03d/v_c%03d_%s%04d' % (label, label, self.split, i)
             yield video.clamp_(0, 1), label, vname
+
+
+class SyntheticSourceVideos(SyntheticVideos):
+    """--gpu-augment: the same split of seeded videos as uint8 source frames at --source-size, each a per-class pattern
+    under per-video noise, augmented on the GPU by one test view (mode 'test', view = (aug_idx, flip_idx)) or the
+    retrieval transform, `chunk` videos per launch.  The view's draws come from its own random.Random."""
+
+    def __init__(self, args, split, device, view=(5, 0), mode='test', chunk=8):
+        from coclr_b200.clf_augment import ClassifierAugment
+        super().__init__(args, split, device, view)
+        self.aug = ClassifierAugment(mode, args.seq_len, args.img_dim, num_seq=args.num_seq, view=view)
+        self.py = random.Random((1 if split == 'test' else 2) * 1000 + (500 if mode == 'retrieval' else 0)
+                                + 10 * view[0] + view[1])
+        self.chunk = chunk
+
+    def _pattern(self, label):
+        h, w = self.args.source_size
+        g = torch.Generator(device=self.device).manual_seed(7919 + label)
+        return torch.rand(1, h, w, 3, device=self.device, generator=g) * 2 - 1
+
+    def _source(self, i):
+        a = self.args
+        h, w = a.source_size
+        base = 1000003 * (1 if self.split == 'test' else 2)
+        label = i % self.n_cls
+        g = torch.Generator(device=self.device).manual_seed(base + 31 * i)
+        n_clips = 1 + (i * 5 + (3 if self.split == 'test' else 0)) % 4
+        T = n_clips * a.seq_len + (i * 3) % a.seq_len
+        noise = torch.rand(T, h, w, 3, device=self.device, generator=g) * 2 - 1
+        video = (0.5 + 0.3 * self._pattern(label) + 0.15 * noise).clamp_(0, 1).mul_(255).round_().to(torch.uint8)
+        return video, label, 'synthetic/c%03d/v_c%03d_%s%04d' % (label, label, self.split, i)
+
+    def __iter__(self):
+        a = self.args
+        h, w = a.source_size
+        for i0 in range(0, a.synthetic_videos, self.chunk):
+            src = [self._source(i) for i in range(i0, min(i0 + self.chunk, a.synthetic_videos))]
+            plan = self.aug.plan([(h, w)] * len(src), self.py, lengths=[v.shape[0] for v, _, _ in src])
+            videos = self.aug(torch.cat([v for v, _, _ in src]), plan)
+            for video, (_, label, vname) in zip(videos, src):
+                yield video, label, vname
+
+
+def test_videos(args, split, device, view=(5, 0), mode='test'):
+    if args.gpu_augment:
+        return SyntheticSourceVideos(args, split, device, view, mode)
+    return SyntheticVideos(args, split, device, view)
 
 
 def load_test_checkpoint(model, args):
@@ -268,7 +361,8 @@ def test_retrieval(model, args, device):
             continue
         os.makedirs(paths['dir'], exist_ok=True)
         print('Computing %s set feature ... ' % split)
-        res = EV.evaluate(model, SyntheticVideos(args, split, device), args.seq_len, args.batch_size, args.num_seq)
+        res = EV.evaluate(model, test_videos(args, split, device, mode='retrieval'), args.seq_len, args.batch_size,
+                          args.num_seq)
         print(res.feature.size())
         torch.save(res.feature.cpu(), paths[split, 'feature'])
         torch.save(res.label.cpu(), paths[split, 'label'])
@@ -324,7 +418,7 @@ def test_10crop(model, args, device):
     res, summaries = None, []
     for flip_idx, aug_idx, after in views:
         print('Aug type: %d; flip: %d' % (aug_idx, flip_idx))
-        res = EV.evaluate(model, SyntheticVideos(args, 'test', device, view=(aug_idx, flip_idx)), args.seq_len,
+        res = EV.evaluate(model, test_videos(args, 'test', device, view=(aug_idx, flip_idx)), args.seq_len,
                           args.batch_size, args.num_seq, previous=res)
         for t in after:
             print('%s-crop result:' % (title if t == 'ten' else t))
@@ -415,6 +509,10 @@ def main(args):
     args.seed_base = 0
     args.num_class = NUM_CLASS[args.dataset]
     model = build_model(args).to(device)
+    if args.gpu_augment:
+        if not args.synthetic:
+            raise NotImplementedError("--gpu-augment reads the synthetic source frames of --synthetic")
+        model.set_input_transform(mean=[0.485, 0.456, 0.406], std=[0.229, 0.224, 0.225])   # :216-220
     if args.test:
         return run_test(model, args, device)
     optimizer = build_optimizer(model, args)

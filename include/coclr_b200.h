@@ -501,6 +501,57 @@ typedef struct {
 size_t coclr_augment_smem_bytes(const coclr_augment_t* p);
 int coclr_augment(const coclr_augment_t* p, coclr_stream_t stream);
 
+/* Fine-tuning and test augmentation (reference eval/main_classifier.py with utils/augmentation.py): the train / val
+ * recipe RandomSizedCrop(224, consistent) -> Scale(D) [-> ColorJitter] -> ToTensor (+ the train batch's flip), and the
+ * test views flip -> FiveCrop(224) / CenterCrop(224) -> Scale((D, D)) -> ColorJitter -> ToTensor.  Every output frame
+ * is a stage-1 bicubic resize of a window of its source frame to M x M (the sample's tables), then, when M != D, a
+ * second bicubic resize M -> D with a uint8 image in between (Pillow's two resizes), the sample's jitter chain and
+ * flip, written as float32 x / 255.  Output bits equal the reference's ToTensor output for the same decisions.
+ * One CTA per output frame; dynamic shared memory coclr_augment_clf_smem_bytes(p) (at most 227 KB).
+ *
+ * src      uint8 [NF, Hmax, Wmax, 3] (channels last); a sample's source occupies the top-left h x w of its frames
+ * frames   [n_frames] records (below): sample index, source frame, output offset and channel stride; output frame
+ *          channel c, row y, column x is out[out + c * chan_stride + y * D + x]
+ * samples  per-sample records (below); coclr_b200/clf_augment.py builds them and the tables from a host plan
+ * coef1    int32 [NS, 2, K1, M]: per sample and axis (0 = x, 1 = y), Pillow's 22-bit bicubic coefficient of tap k of
+ *          stage-1 output pixel o (zero past count); bounds1 int32 [NS, 2, 2, M]: start[M] (absolute coordinate in
+ *          the sample's frame, or in its mirror image when src_flip is set) then count[M], nondecreasing in o
+ * coef2    int32 [K2, D], bounds2 int32 [2, D]: the M -> D resize, the same on both axes (unused when M == D)
+ * Requirements (COCLR_E_ARG otherwise): band_rows >= K1 (stage 1's horizontal pass runs in bands of at most band_rows
+ * source rows), rows >= 1 and K2 <= M when M != D (stage 1's output is staged `rows` rows at a time), shared memory
+ * within 227 KB.  Table contents are not range-checked on the device. */
+typedef struct {
+  int n_ops;                      /* ColorJitter ops applied (0: no jitter) */
+  int op[4];                      /* in application order: 0 brightness, 1 contrast, 2 saturation, 3 hue */
+  float factor[3];                /* float32 blend factor of brightness, contrast, saturation */
+  int hue_shift;                  /* byte added to PIL's H plane, mod 256 */
+  int flip;                       /* mirror the output frame (the train recipe's batch flip) */
+  int src_flip;                   /* read the mirror image of the source (the test views' flip before the crop) */
+  int src_w;                      /* source width, for src_flip */
+  int pad[4];
+} coclr_augment_clf_sample_t;
+typedef struct {
+  int64_t sample;                 /* index into samples */
+  int64_t src_frame;              /* frame of src */
+  int64_t out;                    /* float offset of the frame's channel 0 in out */
+  int64_t chan_stride;            /* floats between its channels */
+} coclr_augment_clf_frame_t;
+typedef struct {
+  const uint8_t* src;
+  int NF, Hmax, Wmax;
+  int n_frames;
+  const coclr_augment_clf_frame_t* frames;
+  const coclr_augment_clf_sample_t* samples;
+  int M, D, K1, K2, band_rows, rows; /* stage-1 side, output side, taps per pixel, band and staged-row heights */
+  const int* coef1;
+  const int* bounds1;
+  const int* coef2;
+  const int* bounds2;
+  float* out;
+} coclr_augment_clf_t;
+size_t coclr_augment_clf_smem_bytes(const coclr_augment_clf_t* p);
+int coclr_augment_clf(const coclr_augment_clf_t* p, coclr_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

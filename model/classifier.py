@@ -34,7 +34,7 @@ class _ClassifierFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, anchor, model, x, backbone_grad):
-        logits, feat3d, plan, head = model._run(x, backbone_grad)
+        logits, feat3d, plan, head = model._run(x, backbone_grad, norm=model._input_norm(x.device))
         if backbone_grad:
             # the plan's activations are shared by every pass of this shape: a backward whose activations were
             # overwritten by a later forward must fail loudly
@@ -95,6 +95,23 @@ class LinearClassifier(nn.Module):
         self._head = None
         self._anchor = None
         self.dropout_mask = None
+        self._input_tf = None
+        self._input_tf_dev = None
+
+    def set_input_transform(self, mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225)):
+        """Fold the reference's GPU-side T.Normalize(mean, std, channel=1) (eval/main_classifier.py:216-220) into the
+        engine's input packing: after this call forward() takes clips [B, 3, T, H, W] in [0, 1] (what ToTensor and
+        coclr_b200.clf_augment give) and normalises them on the fly, with no extra pass.  mean=None switches it off
+        (the default).  infer() is unaffected: it takes its `norm` argument."""
+        self._input_tf = None if mean is None else (tuple(float(v) for v in mean), tuple(float(v) for v in std))
+        self._input_tf_dev = None
+
+    def _input_norm(self, device):
+        if self._input_tf is None:
+            return None
+        if self._input_tf_dev is None or self._input_tf_dev[0].device != device:
+            self._input_tf_dev = tuple(torch.tensor(v, dtype=torch.float32, device=device) for v in self._input_tf)
+        return self._input_tf_dev
 
     def _initialize_weights(self, module):
         for name, param in module.named_parameters():
@@ -228,7 +245,7 @@ class LinearClassifier(nn.Module):
         if backbone_grad or head_grad:
             return _ClassifierFn.apply(self._anchor, self, block, backbone_grad)
         with torch.no_grad():
-            logits, feat3d, _, _ = self._run(block, False)
+            logits, feat3d, _, _ = self._run(block, False, norm=self._input_norm(block.device))
         return logits, feat3d
 
     @torch.no_grad()
