@@ -56,6 +56,9 @@ EXPORTS = {
     "coclr_augment": (I, [P, P]),
     "coclr_augment_clf_smem_bytes": (C.c_size_t, [P]),
     "coclr_augment_clf": (I, [P, P]),
+    "coclr_jpeg_parse": (I, [P, P, I, P, P, I, C.POINTER(I), P, I, C.POINTER(I)]),
+    "coclr_jpeg_work_bytes": (C.c_size_t, [P]),
+    "coclr_jpeg_decode": (I, [P, P]),
 }
 
 

@@ -148,6 +148,13 @@ class AugmentClf(C.Structure):
                 ("bounds2", C.c_void_p), ("out", C.c_void_p)]
 
 
+class Jpeg(C.Structure):
+    _fields_ = [("n", C.c_int), ("data", C.c_void_p), ("frames", C.c_void_p), ("frames_host", C.c_void_p),
+                ("quant", C.c_void_p), ("huff", C.c_void_p), ("out", C.c_void_p),
+                ("frame_stride", C.c_int64), ("row_stride", C.c_int64), ("status", C.c_void_p),
+                ("work", C.c_void_p), ("work_bytes", C.c_size_t)]
+
+
 def library_path():
     return _LIB_PATH
 
@@ -171,7 +178,8 @@ def load():
 LAUNCHES = 0  # kernels of this library launched so far in this process (bench.py reports the per-step count)
 KERNELS_PER_CALL = {"coclr_bn_bwd": 2, "coclr_l2norm_bwd": 2, "coclr_conv_packed_bytes": 0, "coclr_gate_fc_bwd": 2, "coclr_wgrad_ws_floats": 0, "coclr_wgrad_tma_plan": 0,
                     "coclr_center_normalize": 2,
-                    "coclr_augment_smem_bytes": 0, "coclr_augment_clf_smem_bytes": 0}
+                    "coclr_augment_smem_bytes": 0, "coclr_augment_clf_smem_bytes": 0,
+                    "coclr_jpeg_parse": 0, "coclr_jpeg_work_bytes": 0, "coclr_jpeg_decode": 3}
 
 
 def kernels_of(fn, args):

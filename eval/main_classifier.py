@@ -27,6 +27,9 @@ repository, so these paths run with --synthetic only (the PIL crop / scale / jit
                          CenterCrop / Scale / ColorJitter views of --test; the test videos carry the per-class pattern
                          at source resolution.  Training feeds [0, 1] clips with the input normalisation fused
                          (LinearClassifier.set_input_transform)
+  --jpeg                 with --synthetic --gpu-augment: the training and validation loaders hold a seeded pool of
+                         videos as lists of JPEG bytes (the reference LMDB's value format, encoded once by Pillow at
+                         --source-size), decoded on the GPU (coclr_b200.jpeg) in front of the augmentation
 
 --optim sgd and more than one GPU (the reference's nn.DataParallel) are not available: they raise.
 """
@@ -97,6 +100,9 @@ def parse_args(argv=None):
                    help='with --synthetic: augment seeded uint8 source frames on the GPU (the reference\'s transforms)')
     p.add_argument('--source-size', default=[240, 320], nargs=2, type=int, metavar=('H', 'W'),
                    help='height and width of the synthetic source frames of --gpu-augment')
+    p.add_argument('--jpeg', action='store_true',
+                   help='with --synthetic --gpu-augment: decode a pool of JPEG-encoded videos on the GPU in front of '
+                        'the train / val augmentation')
     return p.parse_args(argv)
 
 
@@ -106,6 +112,8 @@ def check_supported(args):
         if getattr(args, flag) and not args.synthetic:
             raise NotImplementedError("--%s needs the per-video LMDB test datasets of the reference (dataset/), which are "
                                       "not part of this repository; run it with --synthetic" % flag)
+    if args.jpeg and not (args.synthetic and args.gpu_augment):
+        raise NotImplementedError("--jpeg decodes the synthetic JPEG pool of --synthetic --gpu-augment")
     if args.optim != 'adam':
         raise NotImplementedError("--optim %s: only Adam is available (--optim adam)" % args.optim)
     if args.model != 'lincls':
@@ -210,15 +218,29 @@ class SyntheticSourceClips:
         self.aug = ClassifierAugment(mode, args.seq_len, args.img_dim, num_seq=args.num_seq)
         self.gen = torch.Generator(device=device).manual_seed(seed)
         self.py = random.Random(seed)
+        self.pool = None
+        if getattr(args, 'jpeg', False):
+            from coclr_b200.jpeg import JpegDecoder, JpegVideoPool
+            h, w = args.source_size
+            self.pool = JpegVideoPool(8, self.aug.frames, h, w, seed=seed)
+            self.dec, self.pick = JpegDecoder(), random.Random(seed + 1)
 
     def __iter__(self):
         a = self.args
         h, w = a.source_size
         for _ in range(a.steps_per_epoch):
-            frames = torch.randint(0, 256, (a.batch_size, self.aug.frames, h, w, 3), dtype=torch.uint8,
-                                   device=self.device, generator=self.gen)
+            if self.pool is not None:        # the dataset's pil_from_raw_rgb, on the GPU
+                batch = self.dec.parse(self.pool.frames([self.pick.randrange(len(self.pool))
+                                                         for _ in range(a.batch_size)]))
+                frames = self.dec(batch)
+                frames = frames.view(a.batch_size, self.aug.frames, *frames.shape[1:])
+                sizes = batch.sample_sizes(a.batch_size)
+            else:
+                frames = torch.randint(0, 256, (a.batch_size, self.aug.frames, h, w, 3), dtype=torch.uint8,
+                                       device=self.device, generator=self.gen)
+                sizes = [(h, w)] * a.batch_size
             y = torch.randint(0, a.num_class, (a.batch_size,), device=self.device, generator=self.gen)
-            plan = self.aug.plan([(h, w)] * a.batch_size, self.py)
+            plan = self.aug.plan(sizes, self.py)
             if self.mode == 'train':
                 flip = random.random() < 0.5                       # transform_train_cuda's T.RandomHorizontalFlip
                 for sp in plan.samples:

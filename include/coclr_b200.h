@@ -552,6 +552,96 @@ typedef struct {
 size_t coclr_augment_clf_smem_bytes(const coclr_augment_clf_t* p);
 int coclr_augment_clf(const coclr_augment_clf_t* p, coclr_stream_t stream);
 
+/* JPEG decoding (the reference datasets' `Image.open(BytesIO(raw)).convert('RGB')`), bit-identical to Pillow's
+ * libjpeg-turbo for baseline / extended sequential Huffman JPEGs with 8-bit samples: grayscale (replicated into R, G
+ * and B) or YCbCr with luma sampling 1x1, 2x1 or 2x2 and chroma 1x1, decoded with the ISLOW IDCT, fancy upsampling
+ * and libjpeg's fixed-point colour conversion.
+ *
+ * coclr_jpeg_parse (host only, no CUDA call) reads the headers of n frames, frame i being data[offsets[i],
+ * offsets[i + 1]).  It fills frames[i] and stores every distinct quant and Huffman table once: up to max_quant /
+ * max_huff of them, *n_quant / *n_huff being the number the batch needs.  It returns 0, or 1 when a table array was
+ * too small (call again with the reported sizes), or COCLR_E_ARG.  A frame it cannot decode gets a non-zero reason
+ * (COCLR_JPEG_*) and no blocks.  Where the scan names a Huffman table no DHT defined, tables 0 and 1 are the
+ * standard ones of ITU T.81 Annex K.3, as libjpeg does. */
+#define COCLR_JPEG_OK 0
+#define COCLR_JPEG_NO_SOI 1
+#define COCLR_JPEG_TRUNCATED 2      /* a segment runs past the end of the frame */
+#define COCLR_JPEG_PROGRESSIVE 3
+#define COCLR_JPEG_ARITHMETIC 4
+#define COCLR_JPEG_SOF_KIND 5       /* lossless or hierarchical */
+#define COCLR_JPEG_PRECISION 6      /* not 8-bit samples */
+#define COCLR_JPEG_COMPONENTS 7     /* not 1 or 3 components (CMYK, YCCK, ...) */
+#define COCLR_JPEG_RGB 8            /* 3 components coded as RGB (Adobe transform 0, or component ids R, G, B) */
+#define COCLR_JPEG_SAMPLING 9
+#define COCLR_JPEG_NO_SOF 10
+#define COCLR_JPEG_NO_SOS 11
+#define COCLR_JPEG_NO_EOI 12
+#define COCLR_JPEG_MULTI_SCAN 13    /* more than one scan, or a scan without every component */
+#define COCLR_JPEG_BAD_TABLE 14     /* a missing quant / Huffman table, or an invalid Huffman table */
+#define COCLR_JPEG_BAD_SEGMENT 15   /* a malformed segment */
+typedef struct {
+  int reason;                     /* COCLR_JPEG_*; the other fields are valid only when it is 0 */
+  int h, w;
+  int ncomp;                      /* 1 (grayscale) or 3 (YCbCr) */
+  int hs, vs;                     /* luma sampling (1 1, 2 1 or 2 2; chroma is 1 1); 1 1 for grayscale */
+  int restart;                    /* restart interval in MCUs, 0: none */
+  int mcus_x, mcus_y;             /* MCU grid; a grayscale MCU is one block */
+  int qt[3];                      /* per component: index into the quant tables */
+  int dc[3], ac[3];               /* per component: index into the Huffman tables */
+  int pad[2];
+  int64_t ecs_begin, ecs_end;     /* the entropy-coded segment: bytes [begin, end) of data, markers RSTn included */
+  int64_t blocks;                 /* 8 x 8 blocks of all components */
+  int64_t block0;                 /* blocks of the batch's frames before this one */
+} coclr_jpeg_frame_t;
+typedef struct {
+  uint16_t q[64];                 /* quantiser of each coefficient, natural (row-major) order */
+} coclr_jpeg_quant_t;
+typedef struct {
+  uint16_t look[512];             /* next 9 bits -> (code length << 8) | symbol; 0: the code is longer */
+  int maxcode[18];                /* largest code of length l = 1..16, -1: none */
+  int valoff[18];                 /* symbol of code c of length l: val[c + valoff[l]] */
+  uint8_t val[256];
+  uint8_t bits[16];               /* codes of each length 1..16 (the DHT counts) */
+  int nval;
+  int pad[3];
+} coclr_jpeg_huff_t;
+int coclr_jpeg_parse(const uint8_t* data, const int64_t* offsets, int n, coclr_jpeg_frame_t* frames,
+                     coclr_jpeg_quant_t* quant, int max_quant, int* n_quant,
+                     coclr_jpeg_huff_t* huff, int max_huff, int* n_huff);
+
+/* coclr_jpeg_decode decodes n parsed frames (every reason 0) into out: frame i, row y, column x, channel c is
+ * out[i * frame_stride + y * row_stride + 3 * x + c], and only the frame's h x w x 3 bytes are written.  It runs in
+ * passes of consecutive frames whose blocks fit the workspace (at most 65535 frames each), three kernels per pass:
+ *   entropy  one warp per frame: lane 0 decodes (9-bit lookahead tables in shared memory), the warp stores each
+ *            block; raw int16 coefficients, natural order, 128 bytes per block
+ *   idct     dequantise and ISLOW IDCT (13-bit constants, 2 pass-1 bits), +128 and clamp; block b's 8 x 8 uint8
+ *            samples overwrite the first 64 bytes of its own 128
+ *   colour   fancy upsampling of the chroma and YCbCr -> RGB (or gray replicated), fused into the store
+ * Workspace: frame i's blocks start at byte 128 * (block0 of i - block0 of the pass's first frame); its component c
+ * holds blocks_h(c) x blocks_w(c) blocks, row-major, after the blocks of components < c.  work_bytes must hold at
+ * least the largest frame; coclr_jpeg_work_bytes gives what the whole batch needs (one pass).  status [n] int32 gets
+ * 0, or COCLR_JPEG_ST_* for a frame whose entropy-coded data is invalid (its pixels are then undefined, the other
+ * frames are unaffected).  Every device read of a frame stays inside its [ecs_begin, ecs_end).  No allocation, no
+ * synchronisation; frames_host is read on the host to plan the passes. */
+#define COCLR_JPEG_ST_BAD_CODE 1      /* a bit pattern that is no code of the Huffman table */
+#define COCLR_JPEG_ST_EARLY_END 2     /* the segment (or a restart interval) ends before its last block */
+#define COCLR_JPEG_ST_BAD_RESTART 3   /* a restart interval not followed by the expected RSTn marker */
+typedef struct {
+  int n;
+  const uint8_t* data;                    /* device: the batch's bytes (offsets as given to coclr_jpeg_parse) */
+  const coclr_jpeg_frame_t* frames;       /* device [n] */
+  const coclr_jpeg_frame_t* frames_host;  /* host [n], the same records */
+  const coclr_jpeg_quant_t* quant;        /* device */
+  const coclr_jpeg_huff_t* huff;          /* device */
+  uint8_t* out;
+  int64_t frame_stride, row_stride;       /* bytes */
+  int* status;                            /* device [n] */
+  void* work;                             /* device, 16-byte aligned */
+  size_t work_bytes;
+} coclr_jpeg_t;
+size_t coclr_jpeg_work_bytes(const coclr_jpeg_t* p);
+int coclr_jpeg_decode(const coclr_jpeg_t* p, coclr_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

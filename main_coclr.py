@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """CoCLR co-training driver -- command line of the reference's main_coclr.py (:38-95) for the accelerated hot
-path, with --synthetic / --gpu-augment / --precision / --steps-per-epoch as in main_nce.py.
+path, with --synthetic / --gpu-augment / --jpeg / --precision / --steps-per-epoch as in main_nce.py.
 
 Loop semantics kept from the reference (main_coclr.py:348-435): the sampler stays in eval mode (:363); the
 self-positive column is masked out with probability 0.9 for rows that have other positives (:382-388, Python
@@ -185,6 +185,7 @@ def main_worker(args):
         return model
     if not args.synthetic:
         raise NotImplementedError("the 2-stream LMDB datasets are outside the accelerated hot path; use --synthetic")
+    base.check_jpeg_flag(args)
     if args.gpu_augment:
         model.set_input_transform(mean=[0.485, 0.456, 0.406], std=[0.229, 0.224, 0.225])
         loader = base.SyntheticSourceFrames(args, device, two_stream=True)

@@ -10,6 +10,9 @@ hot path this repository accelerates, plus:
   --gpu-augment          with --synthetic: the loader yields seeded uint8 source frames (--source-size H W, 240 320 by
                          default) and the reference's get_transform('train') runs on the GPU (coclr_b200.augment); the
                          clips go to the model in loader layout with the input normalisation fused
+  --jpeg                 with --synthetic --gpu-augment: the loader holds a seeded pool of videos as lists of JPEG
+                         bytes (the reference LMDB's value format, encoded once by Pillow at --source-size); each
+                         batch's frames are decoded on the GPU (coclr_b200.jpeg) in front of the augmentation
 
 Launch like the reference: `python -m torch.distributed.run --nproc_per_node=N main_nce.py ...` (one process per
 GPU; --local_rank, --local-rank and the LOCAL_RANK env variable are all accepted).
@@ -82,6 +85,9 @@ def parse_args(argv=None):
                    help='with --synthetic: augment seeded uint8 source frames on the GPU (get_transform("train"))')
     p.add_argument('--source-size', default=[240, 320], nargs=2, type=int, metavar=('H', 'W'),
                    help='height and width of the synthetic source frames of --gpu-augment')
+    p.add_argument('--jpeg', action='store_true',
+                   help='with --synthetic --gpu-augment: decode a pool of JPEG-encoded videos on the GPU in front of '
+                        'the augmentation')
     p.add_argument('--precision', default='parity', choices=['parity', 'mixed', 'fast'])
     p.add_argument('--steps-per-epoch', default=20, type=int)
     p.add_argument('--num-classes', default=101, type=int, help='label range of the synthetic UberNCE labels')
@@ -141,11 +147,26 @@ class SyntheticSourceFrames:
         self.gen = torch.Generator(device=device).manual_seed(seed)
         self.py, self.np = random.Random(seed), np.random.RandomState(seed)
         self.tg = torch.Generator().manual_seed(seed)
+        self.pool = None
+        if getattr(args, 'jpeg', False):
+            from coclr_b200.jpeg import JpegDecoder, JpegVideoPool
+            h, w = args.source_size
+            self.pool = JpegVideoPool(8, self.aug.frames, h, w, seed=seed)
+            self.dec, self.pick = JpegDecoder(), random.Random(seed + 1)
 
     def __iter__(self):
         a = self.args
         h, w = a.source_size
         for _ in range(a.steps_per_epoch):
+            if self.pool is not None:        # the dataset's pil_from_raw_rgb, on the GPU
+                batch = self.dec.parse(self.pool.frames([self.pick.randrange(len(self.pool))
+                                                         for _ in range(a.batch_size)]))
+                frames = self.dec(batch)
+                frames = frames.view(a.batch_size, self.aug.frames, *frames.shape[1:])
+                plan = self.aug.plan(batch.sample_sizes(a.batch_size), self.py, self.np, self.tg)
+                y = torch.randint(0, a.num_classes, (a.batch_size,), device=self.device, generator=self.gen)
+                yield self.aug(frames, plan), y
+                continue
             frames = torch.randint(0, 256, (a.batch_size, self.aug.frames, h, w, 3), dtype=torch.uint8,
                                    device=self.device, generator=self.gen)
             plan = self.aug.plan([(h, w)] * a.batch_size, self.py, self.np, self.tg)
@@ -156,12 +177,18 @@ class SyntheticSourceFrames:
         return self.args.steps_per_epoch
 
 
+def check_jpeg_flag(args):
+    if getattr(args, 'jpeg', False) and not (args.synthetic and args.gpu_augment):
+        raise NotImplementedError("--jpeg decodes the synthetic JPEG pool of --synthetic --gpu-augment")
+
+
 def get_data(args, device):
     if not args.synthetic:
         raise NotImplementedError(
             "dataset %r: the LMDB/JPEG loaders of the reference (dataset/) are outside the accelerated hot path; run "
             "with --synthetic, or feed [B,2,3,T,H,W] float tensors (or uint8 frames through coclr_b200.augment) from "
             "your own loader" % args.dataset)
+    check_jpeg_flag(args)
     return SyntheticSourceFrames(args, device) if args.gpu_augment else SyntheticClips(args, device)
 
 
