@@ -34,6 +34,7 @@ EXPORTS = {
     "coclr_ema_update": (I, [P, P, F, F, LG, I, P]),
     "coclr_queue_enqueue": (I, [P, P, I, I, I, I, P]),
     "coclr_adam_step": (I, [P, I, P]),
+    "coclr_sgd_step": (I, [P, I, P]),
     "coclr_nce_logits_ce": (I, [P, P, P, F, I, I, I, P, P, P, P, P]),
     "coclr_nce_logits_bwd": (I, [P, P, P, F, I, I, I, P, P]),
     "coclr_mask_topk": (I, [P, P, P, P, I, I, I, I, P, P]),

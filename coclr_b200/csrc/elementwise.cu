@@ -1186,6 +1186,22 @@ __global__ void adam_kernel(const coclr_adam_t P) {
   }
 }
 
+// torch.optim.SGD with momentum (dampening 0, no Nesterov) over one flat buffer, bit-identical to torch's default
+// foreach path.  ATen's `a + alpha * b` foreach functor is contracted by nvcc into one fused multiply-add, so
+// _foreach_add(grads, params, alpha=wd) and _foreach_add_(params, bufs, alpha=-lr) are fmaf here; _foreach_mul_ is
+// a rounded product and the alpha = 1 add of the momentum update a plain add, so those two stay separate.
+__global__ void __launch_bounds__(256) sgd_kernel(const coclr_sgd_t P) {
+  const float wd = P.weight_decay, neg_lr = -P.lr, m = P.momentum;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < P.n; i += (long)gridDim.x * blockDim.x) {
+    const float p = P.param[i];
+    float d = P.grad[i];
+    if (wd != 0.f) d = fmaf(wd, p, d);
+    const float buf = P.first ? d : __fadd_rn(__fmul_rn(P.momentum_buf[i], m), d);
+    P.momentum_buf[i] = buf;
+    P.param[i] = fmaf(neg_lr, buf, p);
+  }
+}
+
 static inline int grid_for(long total, int threads, int cap) {
   long g = (total + threads - 1) / threads;
   if (g > cap) g = cap;
@@ -1451,5 +1467,12 @@ extern "C" int coclr_queue_enqueue(float* queue, const float* keys, int dim, int
 extern "C" int coclr_adam_step(const coclr_adam_t* p, int num_sms, coclr_stream_t stream) {
   if (!p || !p->param || !p->grad || !p->exp_avg || !p->exp_avg_sq) return COCLR_E_ARG;
   adam_kernel<<<grid_for(p->n, 256, num_sms * 8), 256, 0, (cudaStream_t)stream>>>(*p);
+  return LAUNCH_OK();
+}
+
+extern "C" int coclr_sgd_step(const coclr_sgd_t* p, int num_sms, coclr_stream_t stream) {
+  if (!p || !p->param || !p->grad || !p->momentum_buf || p->n < 0) return COCLR_E_ARG;
+  if (p->n == 0) return COCLR_OK;
+  sgd_kernel<<<grid_for(p->n, 256, num_sms * 8), 256, 0, (cudaStream_t)stream>>>(*p);
   return LAUNCH_OK();
 }

@@ -874,13 +874,27 @@ class EncoderEngine:
         L.check(L.load().coclr_pack_weights_batch(L.dptr(raw), L.dptr(rs), n, rows, L.stream_ptr()),
                 "coclr_pack_weights_batch")
 
-    def plan(self, B, T, H, W, training, with_backward):
+    def plan(self, B, T, H, W, training, with_backward, replica=0):
+        """The plan of one input shape.  `replica` r > 0 gives a separate plan (own activations) of the same shape, so
+        that the chunks of a data-parallel batch each keep theirs until backward; replica 0 is the plain shape key."""
         key = (B, T, H, W, bool(training), bool(with_backward))
+        if replica:
+            key += (int(replica),)
         p = self.plans.get(key)
         if p is None:
             p = Plan(self, B, T, H, W, training, with_backward)
             self.plans[key] = p
         return p
+
+    def gate_grad_views(self):
+        """Gradient views of the S3D-G gating fc parameters (empty for other backbones).  coclr_gate_fc_bwd writes
+        these (=) where every other parameter-gradient launch of a backward accumulates (+=)."""
+        out = []
+        for kind, it in self.graph.items:
+            if kind == "bn" and it.gates:
+                for nm, _, _ in it.gates:
+                    out += [self.store.view(nm + ".fc.weight", grad=True), self.store.view(nm + ".fc.bias", grad=True)]
+        return out
 
     def _run_lanes(self, oplist, lanes):
         """Forward launch list with fork/join: ops tagged lane 1..3 run on side streams that wait for the fork
@@ -946,12 +960,13 @@ class EncoderEngine:
         L.LAUNCHES += sum(L.kernels_of(fn, args) for fn, args in oplist)
 
     def forward(self, x, training=True, with_backward=False, repack=True, batch_index=None, batch=None, peers=None,
-                norm=None):
+                norm=None, replica=0):
         """x: [*, C, T, H, W] fp32 CUDA (any batch stride). Clip b of the pass is x[batch_index[b]] when a
         device int64 index is given (shuffle-BN gather), else x[b].  peers = (device pointer of an array with one
         peer-mapped clip buffer per rank, clips per rank): batch_index then is a GLOBAL clip index and the clips are
         read straight from the owning ranks' buffers (same layout as x) over NVLink.  norm = (mean, std) device fp32
-        [C]: per-channel (x - mean) / std applied while packing (the reference's GPU-side T.Normalize).  Only the three
+        [C]: per-channel (x - mean) / std applied while packing (the reference's GPU-side T.Normalize).  replica: plan
+        slot (see plan()).  Only the three
         innermost dims of x must be dense: batch and channel strides are free, so a clip may be a view into the loader's
         [B, C, num_seq*seq_len, H, W] tensor.  Returns the plan; plan.q holds
         the normalised features [B, dim] (plan.backbone_out the backbone output when there is no head)."""
@@ -964,7 +979,7 @@ class EncoderEngine:
         nm, ns = (L.dptr(norm[0]), L.dptr(norm[1])) if norm is not None else (None, None)
         if batch_index is not None:
             assert batch_index.dtype == torch.long and batch_index.is_cuda and batch_index.numel() == B
-        p = self.plan(B, T, H, W, training, with_backward)
+        p = self.plan(B, T, H, W, training, with_backward, replica)
         lib = L.load()
         peer_ptr, cpp = (C.c_void_p(int(peers[0])), int(peers[1])) if peers is not None else (None, 0)
         assert peers is None or batch_index is not None

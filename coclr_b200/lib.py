@@ -98,6 +98,11 @@ class Adam(C.Structure):
                 ("step_size", C.c_float), ("bc2_sqrt", C.c_float)]
 
 
+class Sgd(C.Structure):
+    _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("momentum_buf", C.c_void_p), ("n", C.c_long),
+                ("lr", C.c_float), ("weight_decay", C.c_float), ("momentum", C.c_float), ("first", C.c_int)]
+
+
 class ClsHead(C.Structure):
     _fields_ = [("B", C.c_int), ("fs", C.c_int), ("ncls", C.c_int),
                 ("l2norm", C.c_int), ("bn", C.c_int), ("bn_training", C.c_int), ("dropout", C.c_int),

@@ -6,7 +6,8 @@
 * nce_cross_entropy -- nn.CrossEntropyLoss-compatible criterion that reuses those by-products;
 * momentum_update / enqueue / concat_all_gather helpers;
 * FlatAdam      -- torch.optim.Adam semantics (main_nce.py:190-200) as one fused launch over the flat buffer;
-* SpanAdam      -- the same with one param group (own lr) per flat span (eval/main_classifier.py:134-141).
+* SpanAdam      -- the same with one param group (own lr) per flat span (eval/main_classifier.py:134-141);
+* SpanSGD       -- torch.optim.SGD with momentum, one param group per flat span (eval/main_classifier.py:156-161).
 """
 import ctypes as C
 import math
@@ -345,4 +346,59 @@ class SpanAdam:
             for dst, src in zip(self.exp_avg + self.exp_avg_sq, list(sd["exp_avg"]) + list(sd["exp_avg_sq"])):
                 dst.copy_(src)
         self.step_count = sd["step"]
+        self.param_groups = [dict(g) for g in sd["param_groups"]]
+
+
+def _sgd_step(param, grad, buf, group, first):
+    """One coclr_sgd_step launch over a flat span: torch.optim.SGD with momentum, hyper-parameters of `group`."""
+    p = L.Sgd(L.dptr(param), L.dptr(grad), L.dptr(buf), param.numel(), group["lr"], group["weight_decay"],
+              group["momentum"], int(first))
+    L.check(L.load().coclr_sgd_step(C.byref(p), L.num_sms(param.device), L.stream_ptr()), "coclr_sgd_step")
+
+
+class SpanSGD:
+    """torch.optim.SGD(lr, momentum, weight_decay) (dampening 0, no Nesterov) with one param group per flat span
+    (params, grad), bit-identical to torch's default CUDA path over the same values (coclr_sgd_step).  The
+    reference's linear probe builds one group per tensor with the learning rates of SpanAdam's groups, which is
+    equivalent.  A group without a momentum buffer (a new optimizer, or a state saved before its first step) creates it
+    from its first step's gradient, as torch does.  One launch per group; single process (no all-reduce).
+    groups: [{'name': str, 'params': flat fp32 tensor, 'grad': tensor of the same size, 'lr': float}]."""
+
+    def __init__(self, groups, momentum=0.9, weight_decay=0.0):
+        self.param_groups = [{"name": g["name"], "lr": g["lr"], "momentum": momentum, "weight_decay": weight_decay}
+                             for g in groups]
+        self.spans = [(g["params"], g["grad"]) for g in groups]
+        self.momentum_buffer = [None] * len(groups)
+
+    def zero_grad(self, set_to_none=False):
+        for _, g in self.spans:
+            g.zero_()
+
+    @torch.no_grad()
+    def step(self):
+        for i, ((p, g), grp) in enumerate(zip(self.spans, self.param_groups)):
+            first = self.momentum_buffer[i] is None
+            if first:
+                self.momentum_buffer[i] = torch.empty_like(p)
+            _sgd_step(p, g, self.momentum_buffer[i], grp, first)
+
+    def state_dict(self):
+        return {"momentum_buffer": list(self.momentum_buffer), "param_groups": self.param_groups}
+
+    def load_state_dict(self, sd):
+        if "momentum_buffer" not in sd:
+            kind = "SpanAdam" if "exp_avg" in sd else "unknown"
+            raise ValueError("optimizer state is a %s state (keys %s); SpanSGD needs a SpanSGD state"
+                             % (kind, sorted(sd)))
+        if [g["name"] for g in sd["param_groups"]] != [g["name"] for g in self.param_groups]:
+            raise ValueError("optimizer state has groups %s, expected %s"
+                             % ([g["name"] for g in sd["param_groups"]], [g["name"] for g in self.param_groups]))
+        with torch.no_grad():
+            for i, (src, (p, _)) in enumerate(zip(sd["momentum_buffer"], self.spans)):
+                if src is None:
+                    self.momentum_buffer[i] = None
+                else:
+                    if self.momentum_buffer[i] is None:
+                        self.momentum_buffer[i] = torch.empty_like(p)
+                    self.momentum_buffer[i].copy_(src)
         self.param_groups = [dict(g) for g in sd["param_groups"]]

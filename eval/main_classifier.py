@@ -9,8 +9,16 @@ train / validate loop, on the engine's LinearClassifier (model/classifier.py), p
 
 --train_what last (linear probe: l2norm + final BN, no dropout, frozen eval-mode backbone), ft (backbone at lr / 10)
 and all (everything at lr) select the parameters and learning rates as the reference does (:102-147); the optimizer is
-Adam with coupled L2 (--wd) as one launch per group over flat buffers (coclr_b200.moco.SpanAdam).  Accuracy and loss are
-accumulated on the device and read back every --print_freq steps.
+Adam with coupled L2 (--wd, coclr_b200.moco.SpanAdam) or, with --optim sgd, SGD with momentum 0.9 and coupled L2
+(coclr_b200.moco.SpanSGD), as one launch per group over flat buffers.  Accuracy and loss are accumulated on the device
+and read back every --print_freq steps.
+
+--gpu with a comma-separated list of R devices (training with --synthetic) runs the reference's nn.DataParallel
+arithmetic on the first listed device: the batch becomes R x --batch_size (printed as the effective batch size, and
+what the loaders produce), and LinearClassifier(replicas=R) takes BatchNorm statistics per chunk of --batch_size clips
+and keeps the running statistics of chunk 0 only.  The replicas run one after the other on that device.  A single
+--gpu, or none, trains as one replica; CUDA_VISIBLE_DEVICES is not read (the reference derives its replica count from
+it), so setting it changes nothing here.
 
 --test CKPT with --retrieval (nearest-neighbour retrieval, R@1/5/10/20/50) or --center_crop / --five_crop / --ten_crop
 (per-video test accuracy over the crops) runs the reference's test paths (:170-208, :425-718) on the engine
@@ -31,7 +39,8 @@ repository, so these paths run with --synthetic only (the PIL crop / scale / jit
                          videos as lists of JPEG bytes (the reference LMDB's value format, encoded once by Pillow at
                          --source-size), decoded on the GPU (coclr_b200.jpeg) in front of the augmentation
 
---optim sgd and more than one GPU (the reference's nn.DataParallel) are not available: they raise.
+--optim sgd and a --gpu list are available for training with --synthetic only; the --test paths run one replica with
+Adam's options and raise for either.
 """
 import argparse
 import json
@@ -114,26 +123,48 @@ def check_supported(args):
                                       "not part of this repository; run it with --synthetic" % flag)
     if args.jpeg and not (args.synthetic and args.gpu_augment):
         raise NotImplementedError("--jpeg decodes the synthetic JPEG pool of --synthetic --gpu-augment")
-    if args.optim != 'adam':
-        raise NotImplementedError("--optim %s: only Adam is available (--optim adam)" % args.optim)
+    synthetic_training = args.synthetic and not args.test
+    if args.optim not in ('adam', 'sgd'):
+        raise NotImplementedError("--optim %s: Adam (--optim adam) and SGD (--optim sgd) are available" % args.optim)
+    if args.optim == 'sgd' and not synthetic_training:
+        raise NotImplementedError("--optim sgd trains with --synthetic only (not with --test)")
     if args.model != 'lincls':
         raise NotImplementedError("--model %s" % args.model)
     if args.train_what not in ('last', 'ft', 'all'):
         raise ValueError("--train_what must be last, ft or all")
-    if args.gpu is not None and len(str(args.gpu).split(',')) > 1:
-        raise NotImplementedError("--gpu %s: multi-GPU fine-tuning (the reference's nn.DataParallel) is not available; "
-                                  "use one GPU" % args.gpu)
+    if len(gpu_list(args)) > 1 and not synthetic_training:
+        raise NotImplementedError("--gpu %s: the reference's nn.DataParallel replicas are available for training with "
+                                  "--synthetic only (not with --test)" % args.gpu)
     if args.dataset not in NUM_CLASS:
         raise NotImplementedError("dataset %r" % args.dataset)
 
 
+def gpu_list(args):
+    """The devices of --gpu: [] without it, else the comma-separated integers."""
+    if args.gpu is None:
+        return []
+    return [int(g) for g in str(args.gpu).split(',') if g.strip() != '']
+
+
+def apply_gpu_list(args):
+    """A list of R > 1 GPUs (:92-94): args.replicas = R and args.batch_size = R x --batch_size (printed); one GPU or
+    none leaves args.batch_size alone and sets args.replicas = 1."""
+    gpus = gpu_list(args)
+    args.replicas = max(1, len(gpus))
+    if args.replicas > 1:
+        args.batch_size = args.replicas * args.batch_size
+        print('=> Effective BatchSize = %d' % args.batch_size)
+    return gpus
+
+
 def build_model(args):
-    """LinearClassifier in the configuration of --train_what (:102-118) and the parameters it trains (:125-147)."""
+    """LinearClassifier in the configuration of --train_what (:102-118) and the parameters it trains (:125-147), with
+    args.replicas DataParallel replicas (1 when unset)."""
     last = args.train_what == 'last'
     args.final_bn, args.final_norm, args.use_dropout = last, last, not last
     model = LinearClassifier(network=args.net, num_class=args.num_class, dropout=args.dropout,
                              use_dropout=args.use_dropout, use_final_bn=args.final_bn, use_l2_norm=args.final_norm,
-                             precision=args.precision)
+                             precision=args.precision, replicas=getattr(args, 'replicas', 1))
     if last:
         for p in model.backbone.parameters():
             p.requires_grad = False
@@ -141,12 +172,15 @@ def build_model(args):
 
 
 def build_optimizer(model, args):
-    """Adam groups (:125-161): the head at lr, plus the backbone at lr / 10 (ft) or lr (all); none for it with last."""
+    """Adam or (--optim sgd) SGD with momentum 0.9 over the groups of :125-161: the head at lr, plus the backbone at
+    lr / 10 (ft) or lr (all); none for it with last."""
     spans = model.flat_spans()
     groups = [dict(name='head', params=spans['head'][0], grad=spans['head'][1], lr=args.lr)]
     if args.train_what != 'last':
         groups.insert(0, dict(name='backbone', params=spans['backbone'][0], grad=spans['backbone'][1],
                               lr=args.lr / 10 if args.train_what == 'ft' else args.lr))
+    if getattr(args, 'optim', 'adam') == 'sgd':
+        return moco.SpanSGD(groups, momentum=0.9, weight_decay=args.wd)
     return moco.SpanAdam(groups, weight_decay=args.wd)
 
 
@@ -461,9 +495,11 @@ def set_path(args):
     if args.resume:
         exp_path = os.path.dirname(os.path.dirname(args.resume))
     else:
-        exp_path = 'log-eval-{a.prefix}/{a.dataset}-{a.img_dim}_sp{a.which_split}_{a.model}_{a.net}_Adam_bs{a.batch_size}_' \
-                   'lr{a.lr}_dp{a.dropout}_wd{a.wd}_seq{a.num_seq}_len{a.seq_len}_ds{a.ds}_train-{a.train_what}{pt}'.format(
-                       a=args, pt='_pt=%s' % args.pretrain.replace('/', '-') if args.pretrain else '')
+        exp_path = 'log-eval-{a.prefix}/{a.dataset}-{a.img_dim}_sp{a.which_split}_{a.model}_{a.net}{opt}_' \
+                   'bs{a.batch_size}_lr{a.lr}_dp{a.dropout}_wd{a.wd}_seq{a.num_seq}_len{a.seq_len}_ds{a.ds}_' \
+                   'train-{a.train_what}{pt}'.format(
+                       a=args, pt='_pt=%s' % args.pretrain.replace('/', '-') if args.pretrain else '',
+                       opt='_SGD' if args.optim == 'sgd' else '_Adam')
     model_path = os.path.join(exp_path, 'model')
     os.makedirs(model_path, exist_ok=True)
     return model_path
@@ -522,8 +558,9 @@ def validate(loader, model, criterion, epoch, args):
 
 def main(args):
     check_supported(args)
-    if args.gpu is not None:
-        torch.cuda.set_device(int(args.gpu))
+    gpus = apply_gpu_list(args)
+    if gpus:
+        torch.cuda.set_device(gpus[0])
     device = torch.device('cuda')
     torch.manual_seed(0)
     np.random.seed(0)

@@ -320,6 +320,21 @@ typedef struct {
 } coclr_adam_t;
 int coclr_adam_step(const coclr_adam_t* p, int num_sms, coclr_stream_t stream);
 
+/* ---- torch.optim.SGD(lr, momentum, weight_decay), dampening 0, no Nesterov (eval/main_classifier.py:156-161),
+ * flat buffers, bit-identical to torch's default CUDA path (_multi_tensor_sgd) in fp32:
+ *   d = fma(wd, p, g) (skipped when wd == 0); buf = d on the first step, else buf = buf * m (rounded), then
+ *   buf = buf + d; p = fma(-lr, buf, p)  (ATen's foreach `a + alpha * b` is one fused multiply-add).
+ * first != 0: momentum_buf is write-only (the buffer is created from d). */
+typedef struct {
+  float* param;
+  const float* grad;
+  float* momentum_buf;
+  long n;
+  float lr, weight_decay, momentum;
+  int first;
+} coclr_sgd_t;
+int coclr_sgd_step(const coclr_sgd_t* p, int num_sms, coclr_stream_t stream);
+
 /* ---- InfoNCE logits + temperature + cross-entropy (model/pretrain.py:175-182; main_nce.py:201,314) ----
  * logits[b, 0] = q_b.k_b / T, logits[b, 1+j] = q_b.queue[:, j] / T; loss_rows[b] = logsumexp - logits[b,0];
  * dlogits = d(mean_b loss_rows)/d(logits).  loss_rows / dlogits may be NULL.

@@ -18,6 +18,16 @@ coclr_b200.moco.SpanAdam.  `feat3d` is returned without a gradient path.
 The dropout mask comes from a counter-based Philox generator on the device, seeded from torch's default generator (so
 `torch.manual_seed` makes runs reproducible); it is not bit-equal to torch's own dropout mask.  The mask of the last
 forward is kept in `dropout_mask` ([B, feature_size] uint8, 1 = kept).
+
+`replicas=R` (R > 1) makes forward() compute what nn.DataParallel(model, device_ids=<R GPUs>) computes (the reference's
+multi-GPU fine-tuning and linear probe), on the model's one device.  The batch is split as torch.chunk(block, R) does
+(`replica_chunks`), and wherever it is read as a batch -- a train-mode backbone, a train-mode final_bn -- each chunk
+runs as its own pass: its own BatchNorm statistics and dropout seed.  As DataParallel's replica 0 shares the module's
+buffers and the other replicas' updates are lost, the running statistics and num_batches_tracked end as chunk 0 left
+them.  The outputs are the chunks' outputs concatenated; gradients accumulate over the chunks (DataParallel's
+reduce-add).  A pass whose BatchNorms are all in eval mode reads no batch statistics and runs over all B clips at once,
+and a frozen eval-mode backbone (the linear probe) runs once over B with only the head chunked.  infer() is always
+one pass.  Every replica runs on the model's device (`_replica_device`).
 """
 import ctypes as C
 
@@ -57,10 +67,58 @@ class _ClassifierFn(torch.autograd.Function):
         return None, None, None, None
 
 
+def replica_chunks(B, replicas):
+    """Row ranges [(r0, r1)] of torch.chunk(x, replicas, dim=0) for a batch of B: ceil(B / replicas) rows each, the
+    last one shorter; fewer than `replicas` chunks when B does not fill them (DataParallel then runs only that many)."""
+    step = -(-B // replicas)
+    return [(r0, min(r0 + step, B)) for r0 in range(0, B, step)]
+
+
+class _ReplicaClassifierFn(torch.autograd.Function):
+    """The data-parallel forward (LinearClassifier._run_replicas) as one autograd node.  Backward splits dlogits by
+    chunk and runs each chunk's head backward and backbone backward in replica order; both accumulate into the flat
+    gradients, which therefore end with the sum over the replicas.  The one exception, the S3D-G gating fc gradients
+    (written, not accumulated, by coclr_gate_fc_bwd), are carried over from pass to pass here."""
+
+    @staticmethod
+    def forward(ctx, anchor, model, x, backbone_grad):
+        logits, feat3d, passes = model._run_replicas(x, backbone_grad, norm=model._input_norm(x.device))
+        if backbone_grad:
+            ctx.generations = []
+            for plan, _ in passes:
+                plan.generation = getattr(plan, "generation", 0) + 1
+                ctx.generations.append(plan.generation)
+        ctx.model, ctx.passes, ctx.backbone_grad = model, passes, backbone_grad
+        ctx.mark_non_differentiable(feat3d)
+        return logits, feat3d
+
+    @staticmethod
+    def backward(ctx, dlogits, _dfeat3d):
+        model = ctx.model
+        if ctx.backbone_grad and any(plan.generation != g for (plan, _), g in zip(ctx.passes, ctx.generations)):
+            raise L.CoclrError("backward of a classifier pass whose saved activations were overwritten by a later "
+                               "forward of the same shape (one outstanding training forward per input shape)")
+        model._prepare_grads(ctx.backbone_grad)
+        gates = model._engine.gate_grad_views() if ctx.backbone_grad else []
+        for i, (plan, heads) in enumerate(ctx.passes):
+            for hd, (r0, r1) in heads:
+                model._head_backward(hd, dlogits[r0:r1].contiguous(), ctx.backbone_grad)
+            if ctx.backbone_grad:
+                dfeat = heads[0][0]["dfeat"] if len(heads) == 1 else torch.cat([hd["dfeat"] for hd, _ in heads])
+                before = [g.clone() for g in gates] if i > 0 else []
+                model._engine.backward_feat(plan, dfeat)
+                for g, b in zip(gates, before):
+                    g.add_(b)
+        return None, None, None, None
+
+
 class LinearClassifier(nn.Module):
     def __init__(self, num_class=101, network='resnet50', dropout=0.5, use_dropout=True, use_l2_norm=False,
-                 use_final_bn=False, precision="parity"):
+                 use_final_bn=False, precision="parity", replicas=1):
         super().__init__()
+        if int(replicas) < 1:
+            raise ValueError("replicas must be >= 1, got %r" % (replicas,))
+        self.replicas = int(replicas)
         self.network = network
         self.num_class = num_class
         self.dropout = dropout
@@ -183,15 +241,83 @@ class LinearClassifier(nn.Module):
     # -- forward / backward -----------------------------------------------------------------------------
     def _run(self, block, backbone_grad, batch_index=None, batch=None, norm=None):
         eng = self._engine_for(block.device)
-        B, fs = block.shape[0] if batch is None else batch, self.param['feature_size']
+        B = block.shape[0] if batch is None else batch
         plan = eng.forward(block, training=self.backbone.training, with_backward=backbone_grad,
                            batch_index=batch_index, batch=batch, norm=norm)
-        f32 = dict(dtype=torch.float32, device=block.device)
-        hd = {"feat": plan.feat.clone()}
-        bn_train = self.use_final_bn and self.final_bn.training
-        if bn_train and B == 1:
+        feat = plan.feat.clone()
+        if self.use_final_bn and self.final_bn.training and B == 1:
             raise ValueError("Expected more than 1 value per channel when training, got input size %s"
-                             % (list(hd["feat"].shape),))
+                             % (list(feat.shape),))
+        logits, hd = self._head_forward(feat)
+        self.dropout_mask = hd.get("mask")
+        return logits, hd.get("xn", hd["feat"]), plan, hd
+
+    def _replica_device(self, r):
+        """Device of replica r: the model's own for every replica (one place to change for one GPU per replica)."""
+        return self.final_fc[-1].weight.device
+
+    def _running_state(self):
+        """Every buffer a forward may update: the backbone's flat running statistics and num_batches_tracked, and
+        final_bn's."""
+        st = self._engine.store
+        out = [st.running_mean, st.running_var, st.nbt]
+        if self.use_final_bn:
+            bn = self.final_bn
+            out += [bn.running_mean, bn.running_var, bn.num_batches_tracked]
+        return out
+
+    def _run_replicas(self, block, backbone_grad, norm=None):
+        """nn.DataParallel's forward over replica_chunks(B, replicas) (see the module docstring).  Returns the gathered
+        (logits, feat3d) and the passes for backward: [(plan, [(head buffers, (r0, r1))])], one pass per chunk when
+        the backbone is in train mode, else one pass over B with one head per chunk."""
+        eng = self._engine_for(block.device)
+        B, fs = block.shape[0], self.param['feature_size']
+        chunks = replica_chunks(B, self.replicas)
+        if self.use_final_bn and self.final_bn.training and any(r1 - r0 == 1 for r0, r1 in chunks):
+            raise ValueError("Expected more than 1 value per channel when training, got input size %s" % ([1, fs],))
+        for r in range(len(chunks)):
+            if self._replica_device(r) != block.device:
+                raise L.CoclrError("replica %d runs on %s, the input is on %s"
+                                   % (r, self._replica_device(r), block.device))
+        state, kept = self._running_state(), None
+        passes, logits, feats, masks = [], [], [], []
+        if self.backbone.training:
+            for r, (r0, r1) in enumerate(chunks):
+                plan = eng.forward(block[r0:r1], training=True, with_backward=backbone_grad, norm=norm, repack=r == 0,
+                                   replica=r)
+                lg, hd = self._head_forward(plan.feat.clone())
+                passes.append((plan, [(hd, (r0, r1))]))
+                logits.append(lg)
+                feats.append(hd.get("xn", hd["feat"]))
+                masks.append(hd.get("mask"))
+                if r == 0 and len(chunks) > 1:
+                    kept = [t.clone() for t in state]
+        else:
+            plan = eng.forward(block, training=False, with_backward=backbone_grad, norm=norm)
+            heads = []
+            for r, (r0, r1) in enumerate(chunks):
+                lg, hd = self._head_forward(plan.feat[r0:r1].clone())
+                heads.append((hd, (r0, r1)))
+                logits.append(lg)
+                feats.append(hd.get("xn", hd["feat"]))
+                masks.append(hd.get("mask"))
+                if r == 0 and len(chunks) > 1:
+                    kept = [t.clone() for t in state]
+            passes.append((plan, heads))
+        if kept is not None:
+            with torch.no_grad():
+                for t, v in zip(state, kept):
+                    t.copy_(v)
+        self.dropout_mask = None if masks[0] is None else torch.cat(masks)
+        return torch.cat(logits), torch.cat(feats), passes
+
+    def _head_forward(self, feat):
+        """Classifier-head forward (coclr_cls_head_fwd) of the pooled features feat [B, feature_size] (kept in the
+        returned buffers); updates final_bn's running statistics in train mode.  Returns (logits, head buffers)."""
+        B, fs = feat.shape
+        f32 = dict(dtype=torch.float32, device=feat.device)
+        hd = {"feat": feat}
+        bn_train = self.use_final_bn and self.final_bn.training
         p = float(self.final_fc[0].p) if self.use_dropout else 0.0
         drop = self.use_dropout and self.final_fc[0].training and p > 0
         fc = self.final_fc[-1]
@@ -209,18 +335,17 @@ class LinearClassifier(nn.Module):
             h.running_mean, h.running_var = L.dptr(bn.running_mean), L.dptr(bn.running_var)
             h.momentum, h.eps = bn.momentum, bn.eps
         if drop:
-            hd["mask"] = torch.empty(B, fs, dtype=torch.uint8, device=block.device)
+            hd["mask"] = torch.empty(B, fs, dtype=torch.uint8, device=feat.device)
             hd["xd"] = torch.empty(B, fs, **f32)
             h.mask, h.xd = L.dptr(hd["mask"]), L.dptr(hd["xd"])
             h.seed = int(torch.randint(0, 2 ** 62, (1,)))     # torch's default generator: torch.manual_seed applies
-        self.dropout_mask = hd.get("mask")
         logits = torch.empty(B, fc.out_features, **f32)
         h.logits = L.dptr(logits)
         L.check(L.load().coclr_cls_head_fwd(C.byref(h), L.stream_ptr()), "coclr_cls_head_fwd")
         if bn_train:
             self.final_bn.num_batches_tracked.add_(1)
         hd["struct"] = h
-        return logits, hd.get("xn", hd["feat"]), plan, hd
+        return logits, hd
 
     def _head_backward(self, hd, dlogits, backbone_grad):
         h = hd["struct"]
@@ -242,6 +367,12 @@ class LinearClassifier(nn.Module):
         grad_on = torch.is_grad_enabled()
         backbone_grad = grad_on and any(p.requires_grad for p in self.backbone.parameters())
         head_grad = grad_on and any(p.requires_grad for p in self._head_params())
+        if self.replicas > 1 and (self.backbone.training or (self.use_final_bn and self.final_bn.training)):
+            if backbone_grad or head_grad:
+                return _ReplicaClassifierFn.apply(self._anchor, self, block, backbone_grad)
+            with torch.no_grad():
+                logits, feat3d, _ = self._run_replicas(block, False, norm=self._input_norm(block.device))
+            return logits, feat3d
         if backbone_grad or head_grad:
             return _ClassifierFn.apply(self._anchor, self, block, backbone_grad)
         with torch.no_grad():
