@@ -3,7 +3,7 @@ reference's names; the arithmetic of a bare-backbone forward runs on the engine.
 import torch
 import torch.nn as nn
 
-from .engine import Graph, ParamStore, EncoderEngine
+from .engine import Graph, bind_engine
 
 
 def holder_forward(self, *a, **k):
@@ -21,15 +21,8 @@ class EngineBackbone(nn.Module):
         self._engine = None
 
     def _get_engine(self):
-        w = dict(self.named_parameters())[self._probe]
-        if not w.is_cuda:
-            raise RuntimeError("coclr_b200 backbones run on CUDA (sm_90a) only; move the module to the GPU")
-        if self._engine is None or self._engine.store.device != w.device or \
-                w.data_ptr() != self._engine.store.view(self._probe).data_ptr():
-            graph = Graph(self._stages, self.input_channel, head_dim=None)
-            store = ParamStore(graph, w.device)
-            store.bind_module(dict(self.named_parameters()), dict(self.named_buffers()))
-            self._engine = EncoderEngine(store, graph, self.precision)
+        self._engine = bind_engine(self._engine, self.get_parameter(self._probe), self,
+                                   lambda: Graph(self._stages, self.input_channel), self.precision)
         return self._engine
 
     def forward(self, x):

@@ -6,7 +6,7 @@
 //             gate_fc     mean -> gate[B, C]                          (one block per member Linear)
 //             gate_apply  planes <- split(gate * (hi + lo))           (reads 4 B, writes 4 B / element, in place)
 //   backward  gate_bwd_reduce  dgate[b, c] = sum_thw dout * a         (a recomputed from the raw conv output: 8 B)
-//             gate_fc_bwd      dW, dbias, dmean                       (tiny)
+//             gate_fc_bwd      dW += , dbias += , dmean =             (tiny)
 //             gate_bwd_apply   dout <- gate * dout + dmean / THW      (in place; BatchNorm backward follows unchanged)
 #include "common.cuh"
 #include "coclr_b200.h"
@@ -140,7 +140,7 @@ __device__ __forceinline__ float gate_dz(const float* dgate, const float* gate, 
   return dgate[at] * g * (1.f - g);      // d sigmoid
 }
 
-// grid (n): row i of dW (threads over j), and dbias[i]
+// grid (n): row i of dW (threads over j), and dbias[i]; both accumulate (+=) like every other parameter gradient
 __global__ void __launch_bounds__(128)
 gate_fc_bwd_w_kernel(const float* dgate, const float* gate, const float* mean, float* dW, float* dbias, int B, int C,
                      int coff, int n) {
@@ -151,12 +151,12 @@ gate_fc_bwd_w_kernel(const float* dgate, const float* gate, const float* mean, f
   for (int j = threadIdx.x; j < n; j += blockDim.x) {
     float acc = 0.f;
     for (int b = 0; b < B; ++b) acc = fmaf(dz[b], mean[(size_t)b * C + coff + j], acc);
-    dW[(size_t)i * n + j] = acc;
+    dW[(size_t)i * n + j] += acc;
   }
   if (threadIdx.x == 0) {
     float acc = 0.f;
     for (int b = 0; b < B; ++b) acc += dz[b];
-    dbias[i] = acc;
+    dbias[i] += acc;
   }
 }
 

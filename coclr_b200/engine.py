@@ -338,13 +338,18 @@ class Graph:
 # flat parameter storage
 # ---------------------------------------------------------------------------------------------
 class ParamStore:
-    """One flat fp32 buffer for all parameters of an encoder (+ flat grad, flat BN running stats)."""
+    """One flat fp32 buffer for a module's parameters (+ flat grad, flat BN running stats)."""
 
-    def __init__(self, graph, device):
-        self.graph, self.device = graph, device
+    def __init__(self, layout, device, buffer_layout=()):
+        """layout: [(name, shape)] of the parameters in flat-buffer order, each starting 16-byte aligned;
+        buffer_layout: [(name, C)] of the BatchNorms whose running statistics and num_batches_tracked live in flat
+        buffers too.  A Graph as `layout` stands for its param_layout() and buffer_layout()."""
+        if isinstance(layout, Graph):
+            layout, buffer_layout = layout.param_layout(), layout.buffer_layout()
+        self.device = device
         self.offsets = {}
         off = 0
-        for name, shape in graph.param_layout():
+        for name, shape in layout:
             n = 1
             for s in shape:
                 n *= s
@@ -355,13 +360,18 @@ class ParamStore:
         self.grad = torch.zeros(off, dtype=torch.float32, device=device)
         self.buf_offsets = {}
         boff = 0
-        for name, c in graph.buffer_layout():
+        for name, c in buffer_layout:
             self.buf_offsets[name] = (boff, c)
             boff += c
         self.running_mean = torch.zeros(boff, dtype=torch.float32, device=device)
         self.running_var = torch.ones(boff, dtype=torch.float32, device=device)
         self.nbt = torch.zeros(len(self.buf_offsets), dtype=torch.long, device=device)
-        self.nbt_index = {name: i for i, name in enumerate(self.buf_offsets)}
+        self.params = []   # the bound nn.Parameters in layout order (bind_module)
+
+    def owns(self, t):
+        """Whether tensor t lies in the flat parameter buffer (its module's parameters are still views of it)."""
+        off = t.data_ptr() - self.flat.data_ptr()
+        return t.device == self.flat.device and 0 <= off < 4 * self.numel
 
     def view(self, name, grad=False):
         off, n, shape = self.offsets[name]
@@ -378,33 +388,57 @@ class ParamStore:
             end, rows = off + n, rows + shape[0]
         return (self.grad if grad else self.flat)[off0:end].view((rows,) + tuple(shape0[1:]))
 
-    def bind_module(self, named_params, named_buffers, prefix_map=lambda n: n):
+    def bind_module(self, named_params, named_buffers):
         """Copy the module's current values in and rebind every Parameter / BN buffer to a view."""
         with torch.no_grad():
+            self.params = []
             for name in self.offsets:
-                p = named_params[prefix_map(name)]
+                p = named_params[name]
                 v = self.view(name)
                 v.copy_(p.detach().to(self.device))
                 p.data = v
                 p.grad = None
+                self.params.append((name, p))
             nbt_host = []
             for name, (boff, c) in self.buf_offsets.items():
                 for suffix, flat in ((".running_mean", self.running_mean), (".running_var", self.running_var)):
-                    b = named_buffers[prefix_map(name + suffix)]
+                    b = named_buffers[name + suffix]
                     assert b.device == flat.device, "move the module to the CUDA device before the first forward"
                     v = flat[boff:boff + c]
                     v.copy_(b)
                     b.set_(v.untyped_storage(), v.storage_offset(), v.shape, v.stride())
-                nbt_host.append(named_buffers[prefix_map(name + ".num_batches_tracked")])
-            self.nbt.copy_(torch.stack([t.detach().reshape(()) for t in nbt_host]).to(self.nbt.device))
+                nbt_host.append(named_buffers[name + ".num_batches_tracked"])
+            if nbt_host:
+                self.nbt.copy_(torch.stack([t.detach().reshape(()) for t in nbt_host]).to(self.nbt.device))
             for i, nb in enumerate(nbt_host):
                 nb.set_(self.nbt.untyped_storage(), i, (), ())
 
-    def attach_grads(self, named_params, prefix_map=lambda n: n):
-        for name in self.offsets:
-            p = named_params[prefix_map(name)]
-            if p.requires_grad:
+    def attach_grads(self):
+        """Make the .grad of every bound parameter that requires one its view of the flat gradient.  When the first
+        such parameter's .grad is not that view (None after zero_grad(set_to_none=True), or replaced), the gradients
+        count as cleared: the flat gradient is zeroed first.  Every way of clearing gradients clears all of them."""
+        trained = [(name, p) for name, p in self.params if p.requires_grad]
+        if not trained:
+            return
+        name, p = trained[0]
+        if p.grad is None or p.grad.data_ptr() != self.view(name, grad=True).data_ptr():
+            self.grad.zero_()
+            for name, p in trained:
                 p.grad = self.view(name, grad=True)
+
+
+def bind_engine(engine, probe, module, make_graph, precision):
+    """The engine that runs `module`'s parameters: `engine` itself while its store still owns `probe` (one of the
+    module's parameter tensors), else a new engine over a new store of make_graph()'s layout, with the module's
+    parameters and BatchNorm buffers re-bound to views of the store's flat buffers (first call, .cuda(), .to())."""
+    if not probe.is_cuda:
+        raise L.CoclrError("coclr_b200 runs on CUDA (sm_90a) only; move the module to the GPU")
+    if engine is not None and engine.store.owns(probe):
+        return engine
+    graph = make_graph()
+    store = ParamStore(graph, probe.device)
+    store.bind_module(dict(module.named_parameters()), dict(module.named_buffers()))
+    return EncoderEngine(store, graph, precision)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -777,6 +811,8 @@ class EncoderEngine:
         self.store, self.graph, self.precision = store, graph, precision
         self.plans = {}
         dev = store.device
+        # input of the modules' autograd nodes, so that their outputs require a gradient whatever the caller passes in
+        self.anchor = torch.zeros(1, device=dev, requires_grad=True)
         fnp, fbf, bnp = PRECISIONS[precision]
         self.packed_fwd, self.packed_bwd, self._packs = {}, {}, []
         for kind, it in graph.items:
@@ -883,18 +919,9 @@ class EncoderEngine:
         p = self.plans.get(key)
         if p is None:
             p = Plan(self, B, T, H, W, training, with_backward)
+            p.generation = 0   # training forwards that have filled the plan (see backward)
             self.plans[key] = p
         return p
-
-    def gate_grad_views(self):
-        """Gradient views of the S3D-G gating fc parameters (empty for other backbones).  coclr_gate_fc_bwd writes
-        these (=) where every other parameter-gradient launch of a backward accumulates (+=)."""
-        out = []
-        for kind, it in self.graph.items:
-            if kind == "bn" and it.gates:
-                for nm, _, _ in it.gates:
-                    out += [self.store.view(nm + ".fc.weight", grad=True), self.store.view(nm + ".fc.bias", grad=True)]
-        return out
 
     def _run_lanes(self, oplist, lanes):
         """Forward launch list with fork/join: ops tagged lane 1..3 run on side streams that wait for the fork
@@ -969,7 +996,8 @@ class EncoderEngine:
         slot (see plan()).  Only the three
         innermost dims of x must be dense: batch and channel strides are free, so a clip may be a view into the loader's
         [B, C, num_seq*seq_len, H, W] tensor.  Returns the plan; plan.q holds
-        the normalised features [B, dim] (plan.backbone_out the backbone output when there is no head)."""
+        the normalised features [B, dim] (plan.backbone_out the backbone output when there is no head).  With
+        with_backward, plan.generation right after the call is the token that backward() takes."""
         if not x.is_cuda:
             raise L.CoclrError("coclr_b200 encoders run on CUDA only (no CPU fallback)")
         _, Cin, T, H, W = x.shape
@@ -1006,6 +1034,8 @@ class EncoderEngine:
             else:
                 self._run(p.fwd)
         self._graphed(p, "fwd" + ("_repack" if repack else ""), body)
+        if with_backward:
+            p.generation += 1
         return p
 
     use_graphs = True   # capture every launch list into a CUDA graph after its first eager run
@@ -1032,16 +1062,15 @@ class EncoderEngine:
             state[0].replay()
             L.LAUNCHES += state[1]
 
-    def backward(self, p, dq):
-        """dq: gradient w.r.t. the normalised features [B, dim]; accumulates into store.grad."""
-        p.dq.copy_(dq)
-        wg = L.load().coclr_conv_wgrad
-        self._graphed(p, "bwd", lambda: self._run(p.bwd, side_fn=wg))
-
-    def backward_feat(self, p, dfeat):
-        """dfeat: gradient w.r.t. the pooled feature [B, feature_size] of a `pooled` graph; accumulates into
-        store.grad."""
-        p.dfeat.copy_(dfeat)
+    def backward(self, p, grad, generation):
+        """grad: gradient w.r.t. the pass's output -- the normalised features [B, dim] with a head, the pooled feature
+        [B, feature_size] of a `pooled` graph; accumulates into store.grad.  generation: plan.generation as forward()
+        left it.  The plan's activations are shared by every pass of its shape, so a backward whose pass was
+        overwritten by a later training forward raises."""
+        if p.generation != generation:
+            raise L.CoclrError("backward of an engine pass whose saved activations were overwritten by a later forward "
+                               "of the same shape (one outstanding training forward per module and input shape)")
+        (p.dq if self.graph.head_dim is not None else p.dfeat).copy_(grad)
         wg = L.load().coclr_conv_wgrad
         self._graphed(p, "bwd", lambda: self._run(p.bwd, side_fn=wg))
 

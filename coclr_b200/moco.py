@@ -17,7 +17,7 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from . import lib as L
-from .engine import Graph, ParamStore, EncoderEngine
+from .engine import Graph, bind_engine
 from .s3d_spec import S3D_FEATURE_SIZE
 
 
@@ -78,22 +78,16 @@ class _EncodeFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, anchor, enc, x, training):
-        plan = enc._engine_for(x.device).forward(x, training=training, with_backward=True, norm=enc.input_norm)
-        # the plan (activation buffers + captured graphs) is shared by every pass of this shape: remember which pass
-        # filled it, so that a backward whose activations were overwritten by a later forward fails loudly
-        plan.generation = getattr(plan, "generation", 0) + 1
+        plan = enc._engine.forward(x, training=training, with_backward=True, norm=enc.input_norm)
         ctx.enc, ctx.plan, ctx.generation = enc, plan, plan.generation
         return plan.q.clone()
 
     @staticmethod
     def backward(ctx, dq):
-        enc = ctx.enc
-        if ctx.plan.generation != ctx.generation:
-            raise L.CoclrError("backward of an encoder pass whose saved activations were overwritten by a later forward "
-                               "of the same shape (one outstanding training forward per encoder and input shape)")
-        enc._prepare_grads()
+        eng = ctx.enc._engine
+        eng.store.attach_grads()
         mark("bwd:start")
-        enc._engine.backward(ctx.plan, dq.contiguous())
+        eng.backward(ctx.plan, dq.contiguous(), ctx.generation)
         mark("bwd:end")
         return None, None, None, None
 
@@ -110,36 +104,20 @@ class MoCoEncoder(nn.Sequential):
                          nn.Conv3d(feature_size, dim, kernel_size=1, bias=True))
         self.feature_size, self.dim, self.precision = feature_size, dim, precision
         self._engine = None
-        self._anchor = None
         self.input_norm = None   # (mean, std) device tensors: per-channel normalisation fused into the clip packing
 
     # -- engine -------------------------------------------------------------------------------
+    def _graph(self):
+        bb = self[0]
+        return Graph(bb._stages, bb.input_channel, head_dim=self.dim, feature_size=self.feature_size, bb_prefix="0.")
+
     def _engine_for(self, device):
-        w = self[2].weight
-        if not w.is_cuda:
-            raise L.CoclrError("coclr_b200 encoders run on CUDA (sm_90a) only; there is no CPU path")
-        e = self._engine
-        if e is None or e.store.device != w.device or w.data_ptr() != e.store.view("2.weight").data_ptr():
-            bb = self[0]
-            graph = Graph(bb._stages, bb.input_channel, head_dim=self.dim, feature_size=self.feature_size,
-                          bb_prefix="0.")
-            store = ParamStore(graph, w.device)
-            store.bind_module(dict(self.named_parameters()), dict(self.named_buffers()))
-            self._engine = EncoderEngine(store, graph, self.precision)
-            self._anchor = torch.zeros(1, device=w.device, requires_grad=True)
+        self._engine = bind_engine(self._engine, self[2].weight, self, self._graph, self.precision)
         return self._engine
 
     @property
     def store(self):
         return self._engine_for(self[2].weight.device).store
-
-    def _prepare_grads(self):
-        """(Re-)attach the .grad views; a parameter whose grad was set to None means 'zeroed'."""
-        st = self._engine.store
-        first = self[2].weight
-        if first.grad is None or first.grad.data_ptr() != st.view("2.weight", grad=True).data_ptr():
-            st.grad.zero_()
-            st.attach_grads(dict(self.named_parameters()))
 
     def encode(self, x, batch_index=None, batch=None, peers=None):
         """L2-normalised features [B, dim] of clips x[B,C,T,H,W] (what the reference obtains with
@@ -148,7 +126,7 @@ class MoCoEncoder(nn.Sequential):
         want_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
         if want_grad:
             assert batch_index is None
-            return _EncodeFn.apply(self._anchor, self, x, self.training)
+            return _EncodeFn.apply(eng.anchor, self, x, self.training)
         plan = eng.forward(x, training=self.training, with_backward=False, batch_index=batch_index, batch=batch,
                            peers=peers, norm=self.input_norm)
         return plan.q.clone()

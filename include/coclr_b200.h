@@ -360,8 +360,9 @@ int coclr_mask_topk(const float* kf, const float* queue_second, const long* k_vs
  * are the diagonal blocks (coff, n) of the fc step: call coclr_gate_fc / coclr_gate_fc_bwd once per member.
  *   forward : coclr_gate_mean -> coclr_gate_fc (x members) -> coclr_gate_apply (planes scaled in place)
  *   backward: coclr_gate_bwd_reduce (dgate[b, c] = sum_thw dout * a, a = act(y * scale + shift) recomputed from the raw
- *             conv output y and the BatchNorm affine) -> coclr_gate_fc_bwd (x members; dW [n, n] row-major like
- *             nn.Linear.weight, dbias [n], dmean) -> coclr_gate_bwd_apply (dout <- gate * dout + dmean / P, in place:
+ *             conv output y and the BatchNorm affine) -> coclr_gate_fc_bwd (x members; ACCUMULATES into dW [n, n]
+ *             row-major like nn.Linear.weight and dbias [n], as every parameter-gradient kernel does; writes dmean)
+ *             -> coclr_gate_bwd_apply (dout <- gate * dout + dmean / P, in place:
  *             the gradient w.r.t. the un-gated activation, which coclr_bn_bwd then consumes unchanged).
  * mean / gate / dgate / dmean: fp32 [B, C]. */
 int coclr_gate_mean(const void* x_hi, const void* x_lo, int bf16 /* plane format */, int ld, int B, int P, int C, float* mean,

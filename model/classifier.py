@@ -36,35 +36,7 @@ import torch.nn as nn
 
 from backbone.select_backbone import select_backbone
 from coclr_b200 import lib as L
-from coclr_b200.engine import Graph, ParamStore, EncoderEngine
-
-
-class _ClassifierFn(torch.autograd.Function):
-    """Backbone pass + head as one autograd node; gradients go straight into the flat gradient buffers."""
-
-    @staticmethod
-    def forward(ctx, anchor, model, x, backbone_grad):
-        logits, feat3d, plan, head = model._run(x, backbone_grad, norm=model._input_norm(x.device))
-        if backbone_grad:
-            # the plan's activations are shared by every pass of this shape: a backward whose activations were
-            # overwritten by a later forward must fail loudly
-            plan.generation = getattr(plan, "generation", 0) + 1
-            ctx.generation = plan.generation
-        ctx.model, ctx.plan, ctx.head, ctx.backbone_grad = model, plan, head, backbone_grad
-        ctx.mark_non_differentiable(feat3d)
-        return logits, feat3d
-
-    @staticmethod
-    def backward(ctx, dlogits, _dfeat3d):
-        model, plan, head = ctx.model, ctx.plan, ctx.head
-        if ctx.backbone_grad and plan.generation != ctx.generation:
-            raise L.CoclrError("backward of a classifier pass whose saved activations were overwritten by a later "
-                               "forward of the same shape (one outstanding training forward per input shape)")
-        model._prepare_grads(ctx.backbone_grad)
-        model._head_backward(head, dlogits.contiguous(), ctx.backbone_grad)
-        if ctx.backbone_grad:
-            model._engine.backward_feat(plan, head["dfeat"])
-        return None, None, None, None
+from coclr_b200.engine import Graph, ParamStore, bind_engine
 
 
 def replica_chunks(B, replicas):
@@ -74,20 +46,14 @@ def replica_chunks(B, replicas):
     return [(r0, min(r0 + step, B)) for r0 in range(0, B, step)]
 
 
-class _ReplicaClassifierFn(torch.autograd.Function):
-    """The data-parallel forward (LinearClassifier._run_replicas) as one autograd node.  Backward splits dlogits by
-    chunk and runs each chunk's head backward and backbone backward in replica order; both accumulate into the flat
-    gradients, which therefore end with the sum over the replicas.  The one exception, the S3D-G gating fc gradients
-    (written, not accumulated, by coclr_gate_fc_bwd), are carried over from pass to pass here."""
+class _ClassifierFn(torch.autograd.Function):
+    """LinearClassifier._run as one autograd node.  Backward splits dlogits by chunk and runs each chunk's head backward
+    and backbone backward in replica order; both accumulate into the flat gradients, which therefore end with the sum
+    over the replicas."""
 
     @staticmethod
-    def forward(ctx, anchor, model, x, backbone_grad):
-        logits, feat3d, passes = model._run_replicas(x, backbone_grad, norm=model._input_norm(x.device))
-        if backbone_grad:
-            ctx.generations = []
-            for plan, _ in passes:
-                plan.generation = getattr(plan, "generation", 0) + 1
-                ctx.generations.append(plan.generation)
+    def forward(ctx, anchor, model, x, chunks, backbone_grad):
+        logits, feat3d, passes = model._run(x, chunks, backbone_grad, norm=model._input_norm(x.device))
         ctx.model, ctx.passes, ctx.backbone_grad = model, passes, backbone_grad
         ctx.mark_non_differentiable(feat3d)
         return logits, feat3d
@@ -95,21 +61,14 @@ class _ReplicaClassifierFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dlogits, _dfeat3d):
         model = ctx.model
-        if ctx.backbone_grad and any(plan.generation != g for (plan, _), g in zip(ctx.passes, ctx.generations)):
-            raise L.CoclrError("backward of a classifier pass whose saved activations were overwritten by a later "
-                               "forward of the same shape (one outstanding training forward per input shape)")
         model._prepare_grads(ctx.backbone_grad)
-        gates = model._engine.gate_grad_views() if ctx.backbone_grad else []
-        for i, (plan, heads) in enumerate(ctx.passes):
+        for plan, generation, heads in ctx.passes:
             for hd, (r0, r1) in heads:
                 model._head_backward(hd, dlogits[r0:r1].contiguous(), ctx.backbone_grad)
             if ctx.backbone_grad:
                 dfeat = heads[0][0]["dfeat"] if len(heads) == 1 else torch.cat([hd["dfeat"] for hd, _ in heads])
-                before = [g.clone() for g in gates] if i > 0 else []
-                model._engine.backward_feat(plan, dfeat)
-                for g, b in zip(gates, before):
-                    g.add_(b)
-        return None, None, None, None
+                model._engine.backward(plan, dfeat, generation)
+        return None, None, None, None, None
 
 
 class LinearClassifier(nn.Module):
@@ -151,7 +110,6 @@ class LinearClassifier(nn.Module):
         self._initialize_weights(self.final_fc)
         self._engine = None
         self._head = None
-        self._anchor = None
         self.dropout_mask = None
         self._input_tf = None
         self._input_tf_dev = None
@@ -179,79 +137,32 @@ class LinearClassifier(nn.Module):
                 nn.init.normal_(param, mean=0.0, std=0.01)
 
     # -- flat storage ---------------------------------------------------------------------------------
-    def _head_params(self):
-        fc = self.final_fc[-1]
-        return [fc.weight, fc.bias] + ([self.final_bn.weight, self.final_bn.bias] if self.use_final_bn else [])
-
     def _engine_for(self, device):
         bb = self.backbone
-        w = dict(bb.named_parameters())[bb._probe]
-        if not w.is_cuda:
-            raise L.CoclrError("coclr_b200 classifiers run on CUDA (sm_90a) only; there is no CPU path")
-        e = self._engine
-        if e is None or e.store.device != w.device or w.data_ptr() != e.store.view(bb._probe).data_ptr():
-            graph = Graph(bb._stages, bb.input_channel, feature_size=self.param['feature_size'], pooled=True)
-            store = ParamStore(graph, w.device)
-            store.bind_module(dict(bb.named_parameters()), dict(bb.named_buffers()))
-            self._engine = EncoderEngine(store, graph, self.precision)
-            self._anchor = torch.zeros(1, device=w.device, requires_grad=True)
-        ps = self._head_params()
-        h = self._head
-        if h is None or h["flat"].device != ps[0].device or ps[0].data_ptr() != h["views"][0].data_ptr():
-            # one flat fp32 buffer (+ gradient) for the head parameters, like the backbone's ParamStore
-            offs, off = [], 0
-            for p in ps:
-                offs.append(off)
-                off += (p.numel() + 3) // 4 * 4
-            flat = torch.zeros(off, dtype=torch.float32, device=ps[0].device)
-            grad = torch.zeros_like(flat)
-            views = [flat[o:o + p.numel()].view(p.shape) for o, p in zip(offs, ps)]
-            gviews = [grad[o:o + p.numel()].view(p.shape) for o, p in zip(offs, ps)]
-            with torch.no_grad():
-                for p, v in zip(ps, views):
-                    v.copy_(p.detach())
-                    p.data = v
-                    p.grad = None
-            self._head = {"flat": flat, "grad": grad, "views": views, "gviews": gviews}
+        self._engine = bind_engine(self._engine, bb.get_parameter(bb._probe), bb,
+                                   lambda: Graph(bb._stages, bb.input_channel, feature_size=self.param['feature_size'],
+                                                 pooled=True), self.precision)
+        fc = "final_fc.%d." % (len(self.final_fc) - 1)
+        if self._head is None or not self._head.owns(self.get_parameter(fc + "weight")):
+            # one flat fp32 buffer (+ gradient) for the head parameters, names as in state_dict
+            names = [fc + "weight", fc + "bias"] + (["final_bn.weight", "final_bn.bias"] if self.use_final_bn else [])
+            named = {n: self.get_parameter(n) for n in names}
+            self._head = ParamStore([(n, tuple(p.shape)) for n, p in named.items()], named[fc + "weight"].device)
+            self._head.bind_module(named, {})
         return self._engine
 
     def flat_spans(self):
         """{'backbone': (params, grad), 'head': (params, grad)}: the flat fp32 buffers the parameters are views of."""
         eng = self._engine_for(self.final_fc[-1].weight.device)
-        return {"backbone": (eng.store.flat, eng.store.grad), "head": (self._head["flat"], self._head["grad"])}
+        return {"backbone": (eng.store.flat, eng.store.grad), "head": (self._head.flat, self._head.grad)}
 
     def _prepare_grads(self, backbone):
-        """(Re-)attach the .grad views; a parameter whose grad was set to None means 'zeroed'."""
+        """(Re-)attach the .grad views of the head and, with `backbone`, of the backbone (ParamStore.attach_grads)."""
         if backbone:
-            st = self._engine.store
-            named = dict(self.backbone.named_parameters())
-            first = next(n for n in st.offsets if named[n].requires_grad)
-            g = named[first].grad
-            if g is None or g.data_ptr() != st.view(first, grad=True).data_ptr():
-                st.grad.zero_()
-                st.attach_grads(named)
-        h = self._head
-        ps = self._head_params()
-        if ps[0].grad is None or ps[0].grad.data_ptr() != h["gviews"][0].data_ptr():
-            h["grad"].zero_()
-            for p, g in zip(ps, h["gviews"]):
-                if p.requires_grad:
-                    p.grad = g
+            self._engine.store.attach_grads()
+        self._head.attach_grads()
 
     # -- forward / backward -----------------------------------------------------------------------------
-    def _run(self, block, backbone_grad, batch_index=None, batch=None, norm=None):
-        eng = self._engine_for(block.device)
-        B = block.shape[0] if batch is None else batch
-        plan = eng.forward(block, training=self.backbone.training, with_backward=backbone_grad,
-                           batch_index=batch_index, batch=batch, norm=norm)
-        feat = plan.feat.clone()
-        if self.use_final_bn and self.final_bn.training and B == 1:
-            raise ValueError("Expected more than 1 value per channel when training, got input size %s"
-                             % (list(feat.shape),))
-        logits, hd = self._head_forward(feat)
-        self.dropout_mask = hd.get("mask")
-        return logits, hd.get("xn", hd["feat"]), plan, hd
-
     def _replica_device(self, r):
         """Device of replica r: the model's own for every replica (one place to change for one GPU per replica)."""
         return self.final_fc[-1].weight.device
@@ -266,48 +177,46 @@ class LinearClassifier(nn.Module):
             out += [bn.running_mean, bn.running_var, bn.num_batches_tracked]
         return out
 
-    def _run_replicas(self, block, backbone_grad, norm=None):
-        """nn.DataParallel's forward over replica_chunks(B, replicas) (see the module docstring).  Returns the gathered
-        (logits, feat3d) and the passes for backward: [(plan, [(head buffers, (r0, r1))])], one pass per chunk when
-        the backbone is in train mode, else one pass over B with one head per chunk."""
+    def _run(self, block, chunks, backbone_grad, batch_index=None, batch=None, norm=None):
+        """nn.DataParallel's forward over `chunks`, row ranges of the batch (see the module docstring; [(0, B)] is one
+        plain pass).  Returns the gathered (logits, feat3d) and the passes for backward: [(plan, generation, [(head
+        buffers, (r0, r1))])], one pass per chunk when the backbone is in train mode, else one pass over B with one
+        head per chunk."""
         eng = self._engine_for(block.device)
-        B, fs = block.shape[0], self.param['feature_size']
-        chunks = replica_chunks(B, self.replicas)
+        fs = self.param['feature_size']
         if self.use_final_bn and self.final_bn.training and any(r1 - r0 == 1 for r0, r1 in chunks):
             raise ValueError("Expected more than 1 value per channel when training, got input size %s" % ([1, fs],))
         for r in range(len(chunks)):
             if self._replica_device(r) != block.device:
                 raise L.CoclrError("replica %d runs on %s, the input is on %s"
                                    % (r, self._replica_device(r), block.device))
-        state, kept = self._running_state(), None
+        state = self._running_state() if len(chunks) > 1 else None
+        kept = None
         passes, logits, feats, masks = [], [], [], []
-        if self.backbone.training:
-            for r, (r0, r1) in enumerate(chunks):
-                plan = eng.forward(block[r0:r1], training=True, with_backward=backbone_grad, norm=norm, repack=r == 0,
-                                   replica=r)
-                lg, hd = self._head_forward(plan.feat.clone())
-                passes.append((plan, [(hd, (r0, r1))]))
+        # a train-mode backbone reads its batch: one pass (own plan slot) per chunk; else one pass over all the clips
+        groups = [[c] for c in chunks] if self.backbone.training else [chunks]
+        for r, heads in enumerate(groups):
+            x0 = heads[0][0]
+            x = block if len(groups) == 1 else block[x0:heads[-1][1]]
+            plan = eng.forward(x, training=self.backbone.training, with_backward=backbone_grad, repack=r == 0,
+                               batch_index=batch_index, batch=batch, norm=norm, replica=r)
+            hds = []
+            for r0, r1 in heads:
+                lg, hd = self._head_forward(plan.feat[r0 - x0:r1 - x0].clone())
+                hds.append((hd, (r0, r1)))
                 logits.append(lg)
                 feats.append(hd.get("xn", hd["feat"]))
                 masks.append(hd.get("mask"))
-                if r == 0 and len(chunks) > 1:
+                if state is not None and kept is None:     # the running statistics end as chunk 0 left them
                     kept = [t.clone() for t in state]
-        else:
-            plan = eng.forward(block, training=False, with_backward=backbone_grad, norm=norm)
-            heads = []
-            for r, (r0, r1) in enumerate(chunks):
-                lg, hd = self._head_forward(plan.feat[r0:r1].clone())
-                heads.append((hd, (r0, r1)))
-                logits.append(lg)
-                feats.append(hd.get("xn", hd["feat"]))
-                masks.append(hd.get("mask"))
-                if r == 0 and len(chunks) > 1:
-                    kept = [t.clone() for t in state]
-            passes.append((plan, heads))
+            passes.append((plan, plan.generation, hds))
         if kept is not None:
             with torch.no_grad():
                 for t, v in zip(state, kept):
                     t.copy_(v)
+        if len(chunks) == 1:
+            self.dropout_mask = masks[0]
+            return logits[0], feats[0], passes
         self.dropout_mask = None if masks[0] is None else torch.cat(masks)
         return torch.cat(logits), torch.cat(feats), passes
 
@@ -350,7 +259,7 @@ class LinearClassifier(nn.Module):
     def _head_backward(self, hd, dlogits, backbone_grad):
         h = hd["struct"]
         B, fs = h.B, h.fs
-        gv = self._head["gviews"]
+        gv = [self._head.view(n, grad=True) for n in self._head.offsets]
         hd["dx"] = torch.empty(B, fs, dtype=torch.float32, device=dlogits.device)
         hd["dfeat"] = torch.empty(B, fs, dtype=torch.float32, device=dlogits.device) if backbone_grad else None
         h.dlogits, h.dx, h.dfeat = L.dptr(dlogits), L.dptr(hd["dx"]), L.dptr(hd["dfeat"])
@@ -363,20 +272,17 @@ class LinearClassifier(nn.Module):
         """block [B, C, T, H, W] -> (logit [B, num_class], feat3d [B, feature_size]) (classifier.py:47-61)."""
         if not block.is_cuda:
             raise L.CoclrError("coclr_b200 classifiers run on CUDA (sm_90a) only; there is no CPU path")
-        self._engine_for(block.device)
+        eng = self._engine_for(block.device)
         grad_on = torch.is_grad_enabled()
         backbone_grad = grad_on and any(p.requires_grad for p in self.backbone.parameters())
-        head_grad = grad_on and any(p.requires_grad for p in self._head_params())
-        if self.replicas > 1 and (self.backbone.training or (self.use_final_bn and self.final_bn.training)):
-            if backbone_grad or head_grad:
-                return _ReplicaClassifierFn.apply(self._anchor, self, block, backbone_grad)
-            with torch.no_grad():
-                logits, feat3d, _ = self._run_replicas(block, False, norm=self._input_norm(block.device))
-            return logits, feat3d
+        head_grad = grad_on and any(p.requires_grad for _, p in self._head.params)
+        B = block.shape[0]
+        batch_read = self.backbone.training or (self.use_final_bn and self.final_bn.training)
+        chunks = replica_chunks(B, self.replicas) if self.replicas > 1 and batch_read else [(0, B)]
         if backbone_grad or head_grad:
-            return _ClassifierFn.apply(self._anchor, self, block, backbone_grad)
+            return _ClassifierFn.apply(eng.anchor, self, block, chunks, backbone_grad)
         with torch.no_grad():
-            logits, feat3d, _, _ = self._run(block, False, norm=self._input_norm(block.device))
+            logits, feat3d, _ = self._run(block, chunks, False, norm=self._input_norm(block.device))
         return logits, feat3d
 
     @torch.no_grad()
@@ -388,5 +294,6 @@ class LinearClassifier(nn.Module):
         Each submodule's `training` flag is honoured as in forward()."""
         if not x.is_cuda:
             raise L.CoclrError("coclr_b200 classifiers run on CUDA (sm_90a) only; there is no CPU path")
-        logits, feat3d, _, _ = self._run(x, False, batch_index=batch_index, batch=batch, norm=norm)
+        B = x.shape[0] if batch is None else batch
+        logits, feat3d, _ = self._run(x, [(0, B)], False, batch_index=batch_index, batch=batch, norm=norm)
         return logits, feat3d

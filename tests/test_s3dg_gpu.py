@@ -38,9 +38,10 @@ def _rel_l2(a, b):
 @pytest.mark.parametrize("B,P,members,lo", [(3, 37, [24, 40, 8, 16], True), (2, 512, [64, 128, 32, 32], True),
                                             (4, 64, [384, 384, 128, 128], True), (2, 50, [16, 8, 8, 8], False)],
                          ids=["ragged", "mixed3b", "mixed5c", "single_plane"])
-def test_gating_kernels_vs_float64(B, P, members, lo, diag):
-    """forward: planes -> mean -> gate -> planes scaled in place; backward: dgate, fc gradients, gradient w.r.t. the
-    un-gated activation -- against autograd through the reference's formula in float64."""
+def test_gating_kernels_accumulate_vs_float64(B, P, members, lo, diag):
+    """forward: planes -> mean -> gate -> planes scaled in place; backward: dgate, fc gradients (added into zeroed
+    buffers, as into the engine's flat gradient), gradient w.r.t. the un-gated activation -- against autograd through
+    the reference's formula in float64."""
     from coclr_b200 import lib as L, ops
     lib = L.load()
     dev = "cuda"
@@ -89,8 +90,8 @@ def test_gating_kernels_vs_float64(B, P, members, lo, diag):
     out64.backward(dout.double())
     dgate = torch.empty(B, Cc, device=dev)
     dmean = torch.empty(B, Cc, device=dev)
-    dWs = [torch.empty_like(w) for w in Ws]
-    dbs = [torch.empty_like(b) for b in bs]
+    dWs = [torch.zeros_like(w) for w in Ws]      # coclr_gate_fc_bwd accumulates
+    dbs = [torch.zeros_like(b) for b in bs]
     d_inplace = dout.clone()
     L.check(lib.coclr_gate_bwd_reduce(L.dptr(y), Cc, L.dptr(scale), L.dptr(shift), 1, L.dptr(dout), Cc, B, P, Cc,
                                       L.dptr(dgate), s), "coclr_gate_bwd_reduce")

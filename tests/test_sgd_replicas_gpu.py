@@ -243,7 +243,7 @@ def test_replicas_against_dataparallel_oracle(net, train_what, R, B, diag):
         med_ref = float(np.median([v[1] for v in bb.values()]))
         diag[tag + "grad_median_new_ref"] = [med_new, med_ref]
         assert med_new < BUDGET[net] * med_ref + 1e-3, (med_new, med_ref)
-        # the S3D-G gating fc gradients (coclr_gate_fc_bwd writes them; the replica backward carries them over)
+        # the S3D-G gating fc gradients, summed over the replicas like every other gradient
         for k, (e_new, e_ref) in bb.items():
             if ".fc." in k:
                 assert e_new < BUDGET[net] * e_ref + 5e-2, (k, e_new, e_ref)
