@@ -51,6 +51,8 @@ EXPORTS = {
     "coclr_center_normalize": (I, [P, P, P, I, I, P]),
     "coclr_sim_fp32": (I, [P, P, P, I, I, I, P]),
     "coclr_retrieval_rank": (I, [P, P, P, I, I, P, I, P, P, P]),
+    "coclr_sim2_fp32": (I, [P, P, I, P, P, I, P, I, I, P]),
+    "coclr_prob_merge": (I, [P, P, P, I, I, P, P, P]),
     "coclr_probe_work_floats": (LG, [P]),
     "coclr_probe_run": (I, [P, P]),
     "coclr_augment_smem_bytes": (C.c_size_t, [P]),

@@ -7,8 +7,10 @@
 //   video_finalize     one CTA per video                       feat_mean, prob_mean, views_sum (+=), prob, rank, hits
 //   column_mean        one CTA per 32 feature columns          mean (double sums)
 //   center_normalize   one CTA per row                         y = (x - mean) / max(||x - mean||, 1e-12)
-//   sim_fp32           128 x 128 output tile per CTA           sim = q . k^T, fp32 FFMA, k ascending
+//   sim_fp32           128 x 128 output tile per CTA           sim = q . k^T or sim += q . k^T, fp32 FFMA, k asc.
 //   retrieval_rank     one CTA per query                       rank of the best same-label item, hits (+=)
+//   prob_merge         one CTA per video                       fused = (p1 + p2) / 2 in double, argmax hits (+=)
+// (reference eval/merge_2stream_prob.py: sim2 = two sim_fp32 launches, the second accumulating; prob_merge.)
 #include <cuda_runtime.h>
 
 #include "coclr_b200.h"
@@ -151,8 +153,10 @@ center_normalize_kernel(const float* __restrict__ x, const float* __restrict__ m
 // sim[i, j] = sum_k q[i, k] * k[j, k]: one fma chain per output, k ascending.  Both operands are row-major with the
 // reduction dim contiguous; a 128 x 16 slab of each is read as float4 and stored transposed ([k][row]) in shared
 // memory, two slabs in flight.  Each of the 256 threads owns an 8 x 8 block of outputs split 4 + 4 rows and columns at
-// offset 64, so its shared-memory reads are float4 and conflict-free.
+// offset 64, so its shared-memory reads are float4 and conflict-free.  kAccumulate: sim[i, j] = sim[i, j] + dot, one
+// rounded fp32 add of the finished chain to what sim holds (the two-stream sim1 + sim2 of the reference).
 constexpr int kTM = 128, kTK = 16, kPad = 4;
+template <bool kAccumulate>
 __global__ void __launch_bounds__(kThreads, 2)
 sim_fp32_kernel(const float* __restrict__ q, const float* __restrict__ kf, float* __restrict__ sim, int Nq, int Nk,
                 int D) {
@@ -219,12 +223,19 @@ sim_fp32_kernel(const float* __restrict__ q, const float* __restrict__ kf, float
     for (int h = 0; h < 2; ++h) {
       const int gj = col0 + 64 * h + tx * 4;
       if (vec && gj + 3 < Nk) {
-        *reinterpret_cast<float4*>(out + gj) =
-            make_float4(acc[i][4 * h], acc[i][4 * h + 1], acc[i][4 * h + 2], acc[i][4 * h + 3]);
+        float4 v = make_float4(acc[i][4 * h], acc[i][4 * h + 1], acc[i][4 * h + 2], acc[i][4 * h + 3]);
+        if constexpr (kAccumulate) {
+          const float4 o = *reinterpret_cast<const float4*>(out + gj);
+          v = make_float4(__fadd_rn(o.x, v.x), __fadd_rn(o.y, v.y), __fadd_rn(o.z, v.z), __fadd_rn(o.w, v.w));
+        }
+        *reinterpret_cast<float4*>(out + gj) = v;
       } else {
 #pragma unroll
         for (int c = 0; c < 4; ++c)
-          if (gj + c < Nk) out[gj + c] = acc[i][4 * h + c];
+          if (gj + c < Nk) {
+            if constexpr (kAccumulate) out[gj + c] = __fadd_rn(out[gj + c], acc[i][4 * h + c]);
+            else out[gj + c] = acc[i][4 * h + c];
+          }
       }
     }
   }
@@ -288,6 +299,64 @@ retrieval_rank_kernel(const float* __restrict__ sim, const long* __restrict__ ql
   }
 }
 
+// running argmax: ties go to the lower index, and a NaN ranks above every number (np.argmax)
+struct ArgMax {
+  double v;
+  int i;   // -1: nothing seen yet
+  __device__ __forceinline__ void offer(double ov, int oi) {
+    if (oi < 0) return;
+    const bool on = isnan(ov), mn = isnan(v);
+    const bool better = i < 0 || ((on || mn) ? (on && (!mn || oi < i)) : (ov > v || (ov == v && oi < i)));
+    if (better) {
+      v = ov;
+      i = oi;
+    }
+  }
+};
+
+__device__ __forceinline__ int block_argmax(ArgMax m, double* sv, int* si) {
+  sv[threadIdx.x] = m.v;
+  si[threadIdx.x] = m.i;
+  __syncthreads();
+#pragma unroll
+  for (int h = kThreads / 2; h > 0; h >>= 1) {
+    if (threadIdx.x < h) {
+      ArgMax a{sv[threadIdx.x], si[threadIdx.x]};
+      a.offer(sv[threadIdx.x + h], si[threadIdx.x + h]);
+      sv[threadIdx.x] = a.v;
+      si[threadIdx.x] = a.i;
+    }
+    __syncthreads();
+  }
+  const int best = si[0];
+  __syncthreads();
+  return best;
+}
+
+// grid Nv.  fused = (p1 + p2) / 2; the argmax of p1, p2 and fused each scores a hit when it equals the target.
+__global__ void __launch_bounds__(kThreads)
+prob_merge_kernel(const double* __restrict__ p1, const double* __restrict__ p2, const long* __restrict__ target,
+                  int C, double* __restrict__ fused, int* __restrict__ hits) {
+  __shared__ double sv[kThreads];
+  __shared__ int si[kThreads];
+  const size_t r = (size_t)blockIdx.x * C;
+  ArgMax m1{0.0, -1}, m2{0.0, -1}, mf{0.0, -1};
+  for (int j = threadIdx.x; j < C; j += kThreads) {
+    const double a = p1[r + j], b = p2[r + j], f = (a + b) * 0.5;   // == / 2: both round the same exact value
+    fused[r + j] = f;
+    m1.offer(a, j);
+    m2.offer(b, j);
+    mf.offer(f, j);
+  }
+  const int i1 = block_argmax(m1, sv, si), i2 = block_argmax(m2, sv, si), iff = block_argmax(mf, sv, si);
+  if (threadIdx.x == 0) {
+    const long t = target[blockIdx.x];   // outside [0, C): equals no argmax, a miss
+    if (i1 == t) atomicAdd(&hits[0], 1);
+    if (i2 == t) atomicAdd(&hits[1], 1);
+    if (iff == t) atomicAdd(&hits[2], 1);
+  }
+}
+
 inline cudaStream_t S(coclr_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
 inline int LAUNCH_OK() { return cudaGetLastError() == cudaSuccess ? COCLR_OK : COCLR_E_LAUNCH; }
 
@@ -326,7 +395,28 @@ extern "C" int coclr_sim_fp32(const float* q, const float* k, float* sim, int Nq
   if (!q || !k || !sim || Nq <= 0 || Nk <= 0 || D <= 0 || D % 4) return COCLR_E_ARG;
   if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(sim)) % 16)
     return COCLR_E_ARG;
-  sim_fp32_kernel<<<dim3((Nk + kTM - 1) / kTM, (Nq + kTM - 1) / kTM), kThreads, 0, S(stream)>>>(q, k, sim, Nq, Nk, D);
+  sim_fp32_kernel<false>
+      <<<dim3((Nk + kTM - 1) / kTM, (Nq + kTM - 1) / kTM), kThreads, 0, S(stream)>>>(q, k, sim, Nq, Nk, D);
+  return LAUNCH_OK();
+}
+
+extern "C" int coclr_sim2_fp32(const float* q1, const float* k1, int D1, const float* q2, const float* k2, int D2,
+                               float* sim, int Nq, int Nk, coclr_stream_t stream) {
+  if (!q1 || !k1 || !q2 || !k2 || !sim || Nq <= 0 || Nk <= 0 || D1 <= 0 || D2 <= 0 || D1 % 4 || D2 % 4)
+    return COCLR_E_ARG;
+  if ((reinterpret_cast<uintptr_t>(q1) | reinterpret_cast<uintptr_t>(k1) | reinterpret_cast<uintptr_t>(q2) |
+       reinterpret_cast<uintptr_t>(k2) | reinterpret_cast<uintptr_t>(sim)) % 16)
+    return COCLR_E_ARG;
+  const dim3 grid((Nk + kTM - 1) / kTM, (Nq + kTM - 1) / kTM);
+  sim_fp32_kernel<false><<<grid, kThreads, 0, S(stream)>>>(q1, k1, sim, Nq, Nk, D1);
+  sim_fp32_kernel<true><<<grid, kThreads, 0, S(stream)>>>(q2, k2, sim, Nq, Nk, D2);
+  return LAUNCH_OK();
+}
+
+extern "C" int coclr_prob_merge(const double* p1, const double* p2, const long* target, int Nv, int C, double* fused,
+                                int* hits, coclr_stream_t stream) {
+  if (!p1 || !p2 || !target || !fused || !hits || Nv <= 0 || C <= 0) return COCLR_E_ARG;
+  prob_merge_kernel<<<Nv, kThreads, 0, S(stream)>>>(p1, p2, target, C, fused, hits);
   return LAUNCH_OK();
 }
 

@@ -7,6 +7,11 @@
     scores.top1, scores.top5 accuracies over the videos (rank of the target class in scores.prob < 1, < 5)
     sim, rank, acc = retrieval(test_feature, test_label, train_feature, train_label)          (:686-706)
 
+and the two-stream merge of the reference's eval/merge_2stream_prob.py:
+    fused, (acc1, acc2, acc_fused) = merge_probabilities(prob1, prob2, target)                 (merge_prob :60-101)
+    idx = align_two_stream(train_vname1, test_vname1, train_vname2, test_vname2)               (merge_sim :118-170)
+    sim, rank, acc = two_stream_retrieval(test1, train1, test2, train2, test_label, train_label)   (:178-196)
+
 `videos` is any iterable of (video, label, vname) with video a float [3, T_total, H, W] tensor in [0, 1] (the
 reference's ToTensor output, CPU or CUDA).  A video gives T_total // seq_len consecutive, non-overlapping clips (the
 reference's `tr` view, :444-448); frames left over at the end are dropped.
@@ -24,6 +29,7 @@ order, no float atomics, bit-identical from run to run.
 import ctypes as C
 from dataclasses import dataclass, field
 
+import numpy as np
 import torch
 
 from coclr_b200 import lib as L
@@ -257,3 +263,94 @@ def retrieval(test_feature, test_label, train_feature, train_label, ks=RETRIEVAL
     Nq = sim.shape[0]
     acc = [h / Nq for h in hits.tolist()]
     return sim, rank, acc
+
+
+def similarity2(q1, k1, q2, k2):
+    """q1 . k1^T + q2 . k2^T on fp32 FFMA (coclr_sim2_fp32): each stream has its own width D1, D2 (any values; rows
+    are zero-padded to a multiple of 4 where needed).  Bit-identical to similarity(q1, k1) + similarity(q2, k2)."""
+    assert q1.dim() == k1.dim() == q2.dim() == k2.dim() == 2, (q1.shape, k1.shape, q2.shape, k2.shape)
+    assert q1.shape[1] == k1.shape[1] and q2.shape[1] == k2.shape[1], (q1.shape, k1.shape, q2.shape, k2.shape)
+    assert q1.shape[0] == q2.shape[0] and k1.shape[0] == k2.shape[0], (q1.shape, k1.shape, q2.shape, k2.shape)
+    D1, D2 = (q1.shape[1] + 3) // 4 * 4, (q2.shape[1] + 3) // 4 * 4
+    q1, k1, q2, k2 = _gemm_operand(q1, D1), _gemm_operand(k1, D1), _gemm_operand(q2, D2), _gemm_operand(k2, D2)
+    sim = torch.empty(q1.shape[0], k1.shape[0], dtype=torch.float32, device=q1.device)
+    L.check(L.load().coclr_sim2_fp32(L.dptr(q1), L.dptr(k1), D1, L.dptr(q2), L.dptr(k2), D2, L.dptr(sim),
+                                     q1.shape[0], k1.shape[0], L.stream_ptr()), "coclr_sim2_fp32")
+    return sim
+
+
+def two_stream_retrieval(test1, train1, test2, train2, test_label, train_label, ks=RETRIEVAL_KS):
+    """Two-stream nearest-neighbour retrieval of the reference (merge_sim :172-196): centre each of the four sets by
+    its own mean and l2-normalise it, sim = test1 . train1^T + test2 . train2^T, and a query hits at k when a train
+    item of its label is among its k most similar.  The streams must already be aligned row for row
+    (align_two_stream).  Returns (sim [Nq, Nk], rank [Nq] int32, [acc for each k]) as retrieval() does."""
+    if test1.shape[0] != test2.shape[0] or train1.shape[0] != train2.shape[0]:
+        raise ValueError("the two streams have %d / %d test and %d / %d train rows; align them first"
+                         % (test1.shape[0], test2.shape[0], train1.shape[0], train2.shape[0]))
+    q1, k1 = center_normalize(test1.float()), center_normalize(train1.float())
+    q2, k2 = center_normalize(test2.float()), center_normalize(train2.float())
+    sim = similarity2(q1, k1, q2, k2)
+    rank, hits = retrieval_rank(sim, test_label, train_label, ks)
+    Nq = sim.shape[0]
+    acc = [h / Nq for h in hits.tolist()]
+    return sim, rank, acc
+
+
+def merge_probabilities(prob1, prob2, target):
+    """Probability fusion of the reference (merge_prob :60-101) on the device (coclr_prob_merge): fused = (prob1 +
+    prob2) / 2 in float64 per video, and the accuracies of argmax prob1, argmax prob2 and argmax fused against target
+    (ties to the lowest index, as np.argmax; a target outside [0, C) is a miss).  prob1, prob2: [Nv, C] float64 CUDA
+    tensors (the reference reads the JSON floats as float64); target: [Nv] integers.
+    Returns (fused [Nv, C] float64, (acc1, acc2, acc_fused))."""
+    if prob1.dim() != 2 or prob1.shape != prob2.shape or prob1.shape[0] == 0 or prob1.shape[1] == 0:
+        raise ValueError("prob1 and prob2 must be two [Nv, C] matrices of the same non-empty shape, got %s and %s"
+                         % (list(prob1.shape), list(prob2.shape)))
+    if prob1.device.type != "cuda":
+        raise L.CoclrError("coclr_b200 runs on CUDA (sm_90a) only; there is no CPU path")
+    Nv, Cn = prob1.shape
+    p1 = prob1.to(torch.float64).contiguous()
+    p2 = prob2.to(p1.device, torch.float64).contiguous()
+    t = torch.as_tensor(target).to(p1.device, torch.long).contiguous()
+    if t.numel() != Nv:
+        raise ValueError("%d targets for %d videos" % (t.numel(), Nv))
+    fused = torch.empty_like(p1)
+    hits = torch.zeros(3, dtype=torch.int32, device=p1.device)
+    L.check(L.load().coclr_prob_merge(L.dptr(p1), L.dptr(p2), L.dptr(t), Nv, Cn, L.dptr(fused), L.dptr(hits),
+                                      L.stream_ptr()), "coclr_prob_merge")
+    return fused, tuple(h / Nv for h in hits.tolist())
+
+
+def _vname_array(vnames):
+    """The reference's np.squeeze(np.array(vnames)) of a pickled vname list ([[v], ...] as --retrieval writes it, or
+    [v, ...]), kept one-dimensional."""
+    return np.atleast_1d(np.squeeze(np.array(vnames)))
+
+
+def align_two_stream(train_vname1, test_vname1, train_vname2, test_vname2):
+    """The name alignment of the reference's merge_sim (:118-170), on the host: each of the four vname lists is
+    sorted (np.argsort); then, when stream 1 has fewer train videos than stream 2, stream 2's train and test lists
+    keep only the names stream 1 has (np.isin), and after that, when stream 1 has more train videos than stream 2,
+    stream 1's lists keep only the names stream 2 has.  Both steps run when the first one leaves stream 2 shorter.
+    Returns int64 index tensors (train1, test1, train2, test2): row i of the aligned stream s is row idx[i] of its
+    input, and stream 1's labels follow stream 1's indices.  Raises ValueError naming the first position where the
+    aligned names differ (the reference asserts)."""
+    v1tr, v1te = _vname_array(train_vname1), _vname_array(test_vname1)
+    v2tr, v2te = _vname_array(train_vname2), _vname_array(test_vname2)
+    i1tr, i1te, i2tr, i2te = (np.argsort(v) for v in (v1tr, v1te, v2tr, v2te))
+    v1tr, v1te, v2tr, v2te = v1tr[i1tr], v1te[i1te], v2tr[i2tr], v2te[i2te]
+    if len(v1tr) < len(v2tr):
+        keep_tr, keep_te = np.isin(v2tr, v1tr), np.isin(v2te, v1te)
+        v2tr, i2tr, v2te, i2te = v2tr[keep_tr], i2tr[keep_tr], v2te[keep_te], i2te[keep_te]
+    if len(v1tr) > len(v2tr):
+        keep_tr, keep_te = np.isin(v1tr, v2tr), np.isin(v1te, v2te)
+        v1tr, i1tr, v1te, i1te = v1tr[keep_tr], i1tr[keep_tr], v1te[keep_te], i1te[keep_te]
+    for split, a, b in (("train", v1tr, v2tr), ("test", v1te, v2te)):
+        if len(a) != len(b):
+            raise ValueError("after alignment stream 1 has %d %s videos and stream 2 has %d"
+                             % (len(a), split, len(b)))
+        bad = np.flatnonzero(a != b)
+        if len(bad):
+            i = int(bad[0])
+            raise ValueError("%s video %d differs after alignment: %r in stream 1, %r in stream 2"
+                             % (split, i, str(a[i]), str(b[i])))
+    return tuple(torch.from_numpy(np.asarray(i, dtype=np.int64)) for i in (i1tr, i1te, i2tr, i2te))

@@ -421,7 +421,15 @@ int coclr_cls_head_bwd(const coclr_cls_head_t* h, coclr_stream_t stream);
  *   coclr_sim_fp32: sim [Nq, Nk] = q [Nq, D] . k [Nk, D]^T on fp32 FFMA (D % 4 == 0, 16-byte aligned pointers).
  *   coclr_retrieval_rank: rank[i] = position of query i's best same-label item in the order (sim descending, index
  *     ascending), Nk when there is none; hits[m] += rank < ks[m] for the nks (<= COCLR_MAX_KS) values of ks, never for
- *     a query with no same-label item (so a k above Nk counts the queries that have one). */
+ *     a query with no same-label item (so a k above Nk counts the queries that have one).
+ * Two-stream merge (eval/merge_2stream_prob.py of the reference):
+ *   coclr_sim2_fp32: sim [Nq, Nk] = q1 [Nq, D1] . k1 [Nk, D1]^T + q2 [Nq, D2] . k2 [Nk, D2]^T.  Each product is
+ *     coclr_sim_fp32's FFMA chain (k ascending) and the two are joined by one rounded fp32 add, so the result equals
+ *     coclr_sim_fp32(q1, k1) + coclr_sim_fp32(q2, k2) bit for bit without an [Nq, Nk] intermediate (two launches on
+ *     `stream`, the second adding into sim).  D1, D2 % 4 == 0, 16-byte aligned pointers.
+ *   coclr_prob_merge: per video v, fused[v] = (p1[v] + p2[v]) / 2 in double; hits[0] += argmax p1[v] == target[v],
+ *     hits[1] += argmax p2[v] == target[v], hits[2] += argmax fused[v] == target[v] (np.argmax: ties to the lowest
+ *     index, a NaN above every number).  A target outside [0, C) is a miss. */
 #define COCLR_MAX_KS 8
 typedef struct {
   const float* prob_sum; const float* feat_sum; const int* count;   /* [Nv, C], [Nv, D], [Nv] */
@@ -437,6 +445,10 @@ int coclr_center_normalize(const float* x, float* y, float* mean, int N, int D, 
 int coclr_sim_fp32(const float* q, const float* k, float* sim, int Nq, int Nk, int D, coclr_stream_t stream);
 int coclr_retrieval_rank(const float* sim, const long* qlabel, const long* klabel, int Nq, int Nk, const int* ks,
                          int nks, int* rank, int* hits, coclr_stream_t stream);
+int coclr_sim2_fp32(const float* q1, const float* k1, int D1, const float* q2, const float* k2, int D2, float* sim,
+                    int Nq, int Nk, coclr_stream_t stream);
+int coclr_prob_merge(const double* p1, const double* p2, const long* target, int Nv, int C, double* fused, int* hits,
+                     coclr_stream_t stream);   /* [Nv, C] float64 x2, [Nv] int64, [Nv, C] float64, [3] (+=) */
 
 /* ---- Linear probe on extracted features (eval/feature_linear_probe.py of the reference): optional BatchNorm1d
  * (final_bn) + Linear, cross-entropy, SGD (momentum 0.9, coupled weight decay on every parameter), trained for S
