@@ -62,6 +62,7 @@ EXPORTS = {
     "coclr_jpeg_parse": (I, [P, P, I, P, P, I, C.POINTER(I), P, I, C.POINTER(I)]),
     "coclr_jpeg_work_bytes": (C.c_size_t, [P]),
     "coclr_jpeg_decode": (I, [P, P]),
+    "coclr_jpeg_decode_slots": (I, [P, P, P]),
 }
 
 

@@ -610,7 +610,8 @@ __device__ __forceinline__ int chroma(const uint8_t* ws, const coclr_jpeg_frame_
 
 constexpr int kColourX = 32, kColourY = 8;
 
-__global__ void __launch_bounds__(kColourX * kColourY) jpeg_colour_kernel(coclr_jpeg_t p, int f0) {
+__global__ void __launch_bounds__(kColourX * kColourY) jpeg_colour_kernel(coclr_jpeg_t p, coclr_jpeg_slots_t sl,
+                                                                           int f0) {
   const int fi = f0 + blockIdx.z;
   const coclr_jpeg_frame_t& fr = p.frames[fi];
   const int x = blockIdx.x * kColourX + threadIdx.x, y = blockIdx.y * kColourY + threadIdx.y;
@@ -618,21 +619,25 @@ __global__ void __launch_bounds__(kColourX * kColourY) jpeg_colour_kernel(coclr_
   if (x >= w || y >= h) return;
   const coclr_jpeg_frame_t f = fr;
   const uint8_t* ws = reinterpret_cast<const uint8_t*>(p.work) + (f.block0 - p.frames[f0].block0) * 128;
-  uint8_t* out = p.out + fi * p.frame_stride + (int64_t)y * p.row_stride + 3 * x;
   const int Y = sample(ws, f, 0, y, x);
-  if (f.ncomp == 1) {
-    out[0] = out[1] = out[2] = (uint8_t)Y;
-    return;
+  uint8_t r8 = (uint8_t)Y, g8 = r8, b8 = r8;
+  if (f.ncomp != 1) {
+    const int cw = (w + f.hs - 1) / f.hs, ch = (h + f.vs - 1) / f.vs;
+    const int cb = chroma(ws, f, 1, y, x, cw, ch) - 128, cr = chroma(ws, f, 2, y, x, cw, ch) - 128;
+    // jdcolor.c: FIX(1.40200), FIX(1.77200), -FIX(0.71414), -FIX(0.34414) with ONE_HALF, 16-bit shift
+    r8 = (uint8_t)min(max(Y + ((91881 * cr + 32768) >> 16), 0), 255);
+    g8 = (uint8_t)min(max(Y + ((-22554 * cb + 32768 - 46802 * cr) >> 16), 0), 255);
+    b8 = (uint8_t)min(max(Y + ((116130 * cb + 32768) >> 16), 0), 255);
   }
-  const int cw = (w + f.hs - 1) / f.hs, ch = (h + f.vs - 1) / f.vs;
-  const int cb = chroma(ws, f, 1, y, x, cw, ch) - 128, cr = chroma(ws, f, 2, y, x, cw, ch) - 128;
-  // jdcolor.c: FIX(1.40200), FIX(1.77200), -FIX(0.71414), -FIX(0.34414) with ONE_HALF, 16-bit shift
-  const int r = Y + ((91881 * cr + 32768) >> 16);
-  const int g = Y + ((-22554 * cb + 32768 - 46802 * cr) >> 16);
-  const int b = Y + ((116130 * cb + 32768) >> 16);
-  out[0] = (uint8_t)min(max(r, 0), 255);
-  out[1] = (uint8_t)min(max(g, 0), 255);
-  out[2] = (uint8_t)min(max(b, 0), 255);
+  // the output frames this frame was sampled into: one store per slot, no second pass over the output
+  const int s0 = sl.slot_begin ? sl.slot_begin[fi] : fi, s1 = sl.slot_begin ? sl.slot_begin[fi + 1] : fi + 1;
+  const int64_t pix = (int64_t)y * p.row_stride + 3 * x;
+  for (int s = s0; s < s1; ++s) {
+    uint8_t* out = p.out + (sl.slot_begin ? sl.slots[s] : s) * p.frame_stride + pix;
+    out[0] = r8;
+    out[1] = g8;
+    out[2] = b8;
+  }
 }
 
 inline bool args_ok(const coclr_jpeg_t* p) {
@@ -645,6 +650,24 @@ inline bool args_ok(const coclr_jpeg_t* p) {
     if (f.reason != COCLR_JPEG_OK || (size_t)f.blocks * 128 > p->work_bytes) return false;
     if ((int64_t)(f.w * 3) > p->row_stride || (int64_t)(f.h - 1) * p->row_stride + 3 * f.w > p->frame_stride)
       return false;
+  }
+  return true;
+}
+
+// every output frame in [0, n_out) is written by exactly one slot
+inline bool slots_ok(const coclr_jpeg_t* p, const coclr_jpeg_slots_t& s) {
+  if (!s.slot_begin) return true;
+  if (!s.slots || !s.slot_begin_host || !s.slots_host || s.n_out < 0 || s.slot_begin_host[0] != 0 ||
+      s.slot_begin_host[p->n] != s.n_out || (s.n_out && p->frame_stride > INT64_MAX / s.n_out))
+    return false;
+  std::vector<char> seen(s.n_out, 0);
+  for (int i = 0; i < p->n; ++i) {
+    if (s.slot_begin_host[i + 1] < s.slot_begin_host[i]) return false;
+    for (int k = s.slot_begin_host[i]; k < s.slot_begin_host[i + 1]; ++k) {
+      const int o = s.slots_host[k];
+      if (o < 0 || o >= s.n_out || seen[o]) return false;
+      seen[o] = 1;
+    }
   }
   return true;
 }
@@ -689,8 +712,14 @@ extern "C" size_t coclr_jpeg_work_bytes(const coclr_jpeg_t* p) {
 }
 
 extern "C" int coclr_jpeg_decode(const coclr_jpeg_t* p, coclr_stream_t stream) {
+  return coclr_jpeg_decode_slots(p, nullptr, stream);
+}
+
+extern "C" int coclr_jpeg_decode_slots(const coclr_jpeg_t* p, const coclr_jpeg_slots_t* s, coclr_stream_t stream) {
   using namespace coclr;
-  if (!args_ok(p)) return COCLR_E_ARG;
+  coclr_jpeg_slots_t sl{};
+  if (s) sl = *s;
+  if (!args_ok(p) || !slots_ok(p, sl)) return COCLR_E_ARG;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const coclr_jpeg_frame_t* F = p->frames_host;
   const int kMaxPassFrames = 65535;               // the IDCT and colour grids put the pass's frames in y and z
@@ -710,7 +739,7 @@ extern "C" int coclr_jpeg_decode(const coclr_jpeg_t* p, coclr_stream_t stream) {
     jpeg_idct_kernel<<<dim3((unsigned)((max_blocks + kIdctBlocks - 1) / kIdctBlocks), nf), 8 * kIdctBlocks, 0, st>>>(
         *p, f0);
     jpeg_colour_kernel<<<dim3((max_w + kColourX - 1) / kColourX, (max_h + kColourY - 1) / kColourY, nf),
-                         dim3(kColourX, kColourY), 0, st>>>(*p, f0);
+                         dim3(kColourX, kColourY), 0, st>>>(*p, sl, f0);
     if (cudaGetLastError() != cudaSuccess) return COCLR_E_LAUNCH;
     f0 = f1;
   }

@@ -33,6 +33,14 @@ HUFF = np.dtype([("look", np.uint16, 512), ("maxcode", I4, 18), ("valoff", I4, 1
                  ("bits", np.uint8, 16), ("nval", I4), ("pad", I4, 3)])                   # coclr_jpeg_huff_t
 
 
+class JpegFrameError(ValueError):
+    """`parse`'s error: `frame` is the index of the first frame that cannot be decoded, `reason` why."""
+
+    def __init__(self, frame, reason, more=""):
+        super().__init__("frame %d: %s%s" % (frame, reason, more))
+        self.frame, self.reason = frame, reason
+
+
 def _ptr(a):
     return C.c_void_p(a.ctypes.data)
 
@@ -56,17 +64,42 @@ class JpegBatch:
         """Workspace a single pass over the whole batch needs: 128 bytes per 8 x 8 block."""
         return int(self.frames["blocks"].sum()) * 128
 
-    def sample_sizes(self, B):
-        """[(h, w)] of B samples of N / B consecutive frames each; ValueError when a sample's frames differ."""
-        n = len(self)
+    def sample_sizes(self, B, slots=None):
+        """[(h, w)] of B samples of N / B consecutive frames each; ValueError when a sample's frames differ.  With
+        `slots` (as given to JpegDecoder), of the output frames that decode writes."""
+        sizes = self.sizes if slots is None else self.output_sizes(slots)
+        n = len(sizes)
         if B < 1 or n % B:
             raise ValueError("%d frames do not split into %d samples" % (n, B))
-        F, sizes = n // B, self.sizes
+        F = n // B
         for b in range(B):
             s = set(sizes[b * F:(b + 1) * F])
             if len(s) != 1:
                 raise ValueError("sample %d: its frames have different sizes %s" % (b, sorted(s)))
         return [sizes[b * F] for b in range(B)]
+
+    def output_sizes(self, slots):
+        """[(h, w)] of every output frame when frame i is written to output frames slots[i] (JpegDecoder's
+        `slots=`), for `sample_sizes`-style checks on the expanded batch."""
+        begin, flat = slot_arrays(slots, len(self))
+        out = [None] * len(flat)
+        for i, hw in enumerate(self.sizes):
+            for o in flat[begin[i]:begin[i + 1]]:
+                out[o] = hw
+        return out
+
+
+def slot_arrays(slots, n):
+    """`slots` (one list of output frame indices per parsed frame) as the int32 (slot_begin [n + 1], slots) of
+    coclr_jpeg_t; ValueError unless every output frame 0 .. len - 1 is written exactly once."""
+    if len(slots) != n:
+        raise ValueError("slots has %d entries for %d frames" % (len(slots), n))
+    begin = np.zeros(n + 1, np.int32)
+    begin[1:] = np.cumsum([len(s) for s in slots])
+    flat = np.array([o for s in slots for o in s], np.int32).reshape(-1)
+    if not np.array_equal(np.sort(flat), np.arange(len(flat))):
+        raise ValueError("slots must write every output frame 0 .. %d exactly once" % (len(flat) - 1))
+    return begin, flat
 
 
 def parse(jpegs):
@@ -93,7 +126,7 @@ def parse(jpegs):
     if len(bad):
         i = int(bad[0])
         more = " (and %d more)" % (len(bad) - 1) if len(bad) > 1 else ""
-        raise ValueError("frame %d: %s%s" % (i, REASONS[frames["reason"][i]], more))
+        raise JpegFrameError(i, REASONS[frames["reason"][i]], more)
     return JpegBatch(data, offsets, frames, quant[:nq.value], huff[:nh.value])
 
 
@@ -128,29 +161,41 @@ class JpegDecoder:
 
     parse = staticmethod(parse)
 
-    def __call__(self, batch, out=None, check=True):
+    def __call__(self, batch, out=None, check=True, slots=None):
         """Decode `batch` into out (uint8 [N, >= Hmax, >= Wmax, 3] on the GPU, rows and frames strided; only each
         frame's top-left h x w x 3 bytes are written) or a new [N, Hmax, Wmax, 3] tensor.  check=True reads the
         status back (one synchronisation) and raises ValueError naming the frames with invalid entropy-coded data;
-        check=False leaves it in `self.status` on the device."""
+        check=False leaves it in `self.status` on the device.
+
+        slots: one list of output frame indices per parsed frame; frame i is decoded once and written to each of
+        slots[i], so N becomes the number of output frames (every one written exactly once)."""
         if not isinstance(batch, JpegBatch):
             raise ValueError("decode takes the JpegBatch of JpegDecoder.parse")
         n = len(batch)
+        if slots is not None:
+            slot_begin, slot_list = slot_arrays(slots, n)
+            n_out = len(slot_list)
+        else:
+            slot_begin = slot_list = None
+            n_out = n
         dev = torch.device("cuda", torch.cuda.current_device())
         hm = max((h for h, _ in batch.sizes), default=1)
         wm = max((w for _, w in batch.sizes), default=1)
         if out is None:
-            out = torch.empty(n, hm, wm, 3, dtype=torch.uint8, device=dev)
+            out = torch.empty(n_out, hm, wm, 3, dtype=torch.uint8, device=dev)
         elif (not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or not out.is_cuda or out.dim() != 4 or
-              out.shape[0] != n or out.shape[1] < hm or out.shape[2] < wm or out.shape[3] != 3 or
+              out.shape[0] != n_out or out.shape[1] < hm or out.shape[2] < wm or out.shape[3] != 3 or
               out.stride(3) != 1 or out.stride(2) != 3):
-            raise ValueError("out must be a CUDA uint8 [%d, >= %d, >= %d, 3] tensor with packed pixels" % (n, hm, wm))
+            raise ValueError("out must be a CUDA uint8 [%d, >= %d, >= %d, 3] tensor with packed pixels"
+                             % (n_out, hm, wm))
         if n == 0:
             return out
 
-        # one staging image: bytes | records | quant tables | Huffman tables, each 256-aligned
+        # one staging image: bytes | records | quant tables | Huffman tables [| slot_begin | slots], each 256-aligned
         parts = [batch.data.view(np.uint8), batch.frames.view(np.uint8), batch.quant.view(np.uint8),
                  batch.huff.view(np.uint8)]
+        if slots is not None:
+            parts += [slot_begin.view(np.uint8), slot_list.view(np.uint8)]
         offs, total = [], 0
         for a in parts:
             offs.append(total)
@@ -200,13 +245,21 @@ class JpegDecoder:
         base = dbuf.data_ptr()
         p = L.Jpeg()
         p.n = n
-        p.data, p.frames, p.quant, p.huff = (base + o for o in offs)
+        p.data, p.frames, p.quant, p.huff = (base + o for o in offs[:4])
         p.frames_host = _ptr(batch.frames)
         p.out = L.dptr(out)
         p.frame_stride, p.row_stride = out.stride(0), out.stride(1)
         p.status = L.dptr(status)
         p.work, p.work_bytes = L.dptr(work), work.numel()
-        L.check(L.load().coclr_jpeg_decode(C.byref(p), L.stream_ptr()), "coclr_jpeg_decode")
+        if slots is None:
+            L.check(L.load().coclr_jpeg_decode(C.byref(p), L.stream_ptr()), "coclr_jpeg_decode")
+        else:
+            sl = L.JpegSlots()
+            sl.slot_begin, sl.slots = base + offs[4], base + offs[5]
+            sl.slot_begin_host, sl.slots_host = _ptr(slot_begin), _ptr(slot_list)
+            sl.n_out = n_out
+            L.check(L.load().coclr_jpeg_decode_slots(C.byref(p), C.byref(sl), L.stream_ptr()),
+                    "coclr_jpeg_decode_slots")
         if check:
             st = status.cpu().numpy()
             bad = np.nonzero(st)[0]

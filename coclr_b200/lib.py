@@ -160,6 +160,11 @@ class Jpeg(C.Structure):
                 ("work", C.c_void_p), ("work_bytes", C.c_size_t)]
 
 
+class JpegSlots(C.Structure):
+    _fields_ = [("slot_begin", C.c_void_p), ("slots", C.c_void_p), ("slot_begin_host", C.c_void_p),
+                ("slots_host", C.c_void_p), ("n_out", C.c_int)]
+
+
 def library_path():
     return _LIB_PATH
 
@@ -184,7 +189,8 @@ LAUNCHES = 0  # kernels of this library launched so far in this process (bench.p
 KERNELS_PER_CALL = {"coclr_bn_bwd": 2, "coclr_l2norm_bwd": 2, "coclr_conv_packed_bytes": 0, "coclr_gate_fc_bwd": 2, "coclr_wgrad_ws_floats": 0, "coclr_wgrad_tma_plan": 0,
                     "coclr_center_normalize": 2,
                     "coclr_augment_smem_bytes": 0, "coclr_augment_clf_smem_bytes": 0,
-                    "coclr_jpeg_parse": 0, "coclr_jpeg_work_bytes": 0, "coclr_jpeg_decode": 3}
+                    "coclr_jpeg_parse": 0, "coclr_jpeg_work_bytes": 0, "coclr_jpeg_decode": 3,
+                    "coclr_jpeg_decode_slots": 3}
 
 
 def kernels_of(fn, args):

@@ -22,9 +22,15 @@ it), so setting it changes nothing here.
 
 --test CKPT with --retrieval (nearest-neighbour retrieval, R@1/5/10/20/50) or --center_crop / --five_crop / --ten_crop
 (per-video test accuracy over the crops) runs the reference's test paths (:170-208, :425-718) on the engine
-(coclr_b200.evaluate) and writes the reference's output files.  The per-video LMDB datasets are not part of this
-repository, so these paths run with --synthetic only (the PIL crop / scale / jitter transforms run on the GPU with
---gpu-augment):
+(coclr_b200.evaluate) and writes the reference's output files, with --data-root or --synthetic (the PIL crop /
+scale / jitter transforms run on the GPU with --data-root and with --gpu-augment):
+
+  --data-root DIR        the reference's LMDB databases in its relative layout (UCF101/ucf101_frame.lmdb,
+  --split-root DIR       UCF101/ucf101_tvl1_frame.lmdb, HMDB51/hmdb51_{frame,tvl1_frame}.lmdb) and its split files
+                         (ucf101/, hmdb51/ as in process_data/data/): ucf101, ucf101-f, hmdb51 and hmdb51-f with
+                         --which_split are read with coclr_b200.datasets, each batch's distinct frames decoded once
+                         on the GPU and augmented there (coclr_b200.loaders); the test and retrieval outputs are keyed
+                         by the split CSV's path column, as the reference's
 
   --synthetic-videos N   videos per split: seeded, 1-4 clips each, a per-class pattern so that the accuracies are well
                          above chance; every (crop, flip) view of a video has its own deterministic content
@@ -39,7 +45,8 @@ repository, so these paths run with --synthetic only (the PIL crop / scale / jit
                          videos as lists of JPEG bytes (the reference LMDB's value format, encoded once by Pillow at
                          --source-size), decoded on the GPU (coclr_b200.jpeg) in front of the augmentation
 
---optim sgd and a --gpu list are available for training with --synthetic only; the --test paths run one replica with
+--optim sgd and a --gpu list are available for training with --synthetic or --data-root; the --test paths run one
+replica with
 Adam's options and raise for either.
 """
 import argparse
@@ -112,18 +119,20 @@ def parse_args(argv=None):
     p.add_argument('--jpeg', action='store_true',
                    help='with --synthetic --gpu-augment: decode a pool of JPEG-encoded videos on the GPU in front of '
                         'the train / val augmentation')
+    p.add_argument('--data-root', default=None, help='directory of the reference\'s LMDB databases (UCF101/, HMDB51/)')
+    p.add_argument('--split-root', default=None, help='directory of the reference\'s split files (ucf101/, hmdb51/)')
     return p.parse_args(argv)
 
 
 def check_supported(args):
     """Raise for what this driver does not run (see the module docstring)."""
     for flag in ('test', 'retrieval', 'center_crop', 'five_crop', 'ten_crop'):
-        if getattr(args, flag) and not args.synthetic:
+        if getattr(args, flag) and not (args.synthetic or args.data_root):
             raise NotImplementedError("--%s needs the per-video LMDB test datasets of the reference (dataset/), which are "
                                       "not part of this repository; run it with --synthetic" % flag)
     if args.jpeg and not (args.synthetic and args.gpu_augment):
         raise NotImplementedError("--jpeg decodes the synthetic JPEG pool of --synthetic --gpu-augment")
-    synthetic_training = args.synthetic and not args.test
+    synthetic_training = (args.synthetic or bool(args.data_root)) and not args.test
     if args.optim not in ('adam', 'sgd'):
         raise NotImplementedError("--optim %s: Adam (--optim adam) and SGD (--optim sgd) are available" % args.optim)
     if args.optim == 'sgd' and not synthetic_training:
@@ -137,6 +146,8 @@ def check_supported(args):
                                   "--synthetic only (not with --test)" % args.gpu)
     if args.dataset not in NUM_CLASS:
         raise NotImplementedError("dataset %r" % args.dataset)
+    if args.data_root and not args.synthetic and args.dataset not in LMDB_DATASETS:
+        raise NotImplementedError("dataset %r has no LMDB loader in the reference's get_data" % args.dataset)
 
 
 def gpu_list(args):
@@ -228,7 +239,28 @@ class SyntheticClips:
         return self.args.steps_per_epoch
 
 
+LMDB_DATASETS = {'ucf101': ('UCF101LMDB', 'ucf101', 'UCF101/ucf101_frame.lmdb'),
+                 'ucf101-f': ('UCF101Flow_LMDB', 'ucf101', 'UCF101/ucf101_tvl1_frame.lmdb'),
+                 'hmdb51': ('HMDB51LMDB', 'hmdb51', 'HMDB51/hmdb51_frame.lmdb'),
+                 'hmdb51-f': ('HMDB51Flow_LMDB', 'hmdb51', 'HMDB51/hmdb51_tvl1_frame.lmdb')}
+
+
+def lmdb_dataset(args, mode, which_split=None):
+    """get_data of the reference (:747-770) over --data-root / --split-root; which_split defaults to --which_split."""
+    from coclr_b200 import datasets as D
+    if not args.split_root:
+        raise ValueError("--data-root needs --split-root (the reference's process_data/data directory)")
+    cls, split, db = LMDB_DATASETS[args.dataset]
+    return getattr(D, cls)(root=os.path.join(args.split_root, split), db_path=os.path.join(args.data_root, db),
+                           mode=mode, num_frames=args.seq_len * args.num_seq, ds=args.ds,
+                           which_split=args.which_split if which_split is None else which_split, return_label=True)
+
+
 def get_data(args, device, mode):
+    if args.data_root and not args.synthetic:
+        from coclr_b200.loaders import ClassifierBatches
+        return ClassifierBatches(lmdb_dataset(args, mode), args.batch_size, args.seq_len, args.img_dim, device,
+                                 seed=args.seed_base + (0 if mode == 'train' else 1), mode=mode, num_seq=args.num_seq)
     if not args.synthetic:
         raise NotImplementedError(
             "dataset %r: the LMDB loaders and PIL augmentations of the reference (dataset/, utils/augmentation.py) are "
@@ -365,6 +397,14 @@ class SyntheticSourceVideos(SyntheticVideos):
 
 
 def test_videos(args, split, device, view=(5, 0), mode='test'):
+    if args.data_root and not args.synthetic:
+        # the reference's test datasets: mode 'test' (half-overlap windows) for the test split, 'train' (one random
+        # clip per video) for retrieval's train split; vname is the CSV's path column.  test_retrieval (:574-589)
+        # reads split 1 whatever --which_split says; test_10crop reads --which_split
+        from coclr_b200.loaders import TestVideos
+        ds = lmdb_dataset(args, 'test' if split == 'test' else 'train', which_split=1 if mode == 'retrieval' else None)
+        seed = (1 if split == 'test' else 2) * 1000 + (500 if mode == 'retrieval' else 0) + 10 * view[0] + view[1]
+        return TestVideos(ds, args.seq_len, args.img_dim, device, seed, view=view, mode=mode)
     if args.gpu_augment:
         return SyntheticSourceVideos(args, split, device, view, mode)
     return SyntheticVideos(args, split, device, view)
@@ -572,6 +612,8 @@ def main(args):
         if not args.synthetic:
             raise NotImplementedError("--gpu-augment reads the synthetic source frames of --synthetic")
         model.set_input_transform(mean=[0.485, 0.456, 0.406], std=[0.229, 0.224, 0.225])   # :216-220
+    elif args.data_root and not args.synthetic:
+        model.set_input_transform(mean=[0.485, 0.456, 0.406], std=[0.229, 0.224, 0.225])
     if args.test:
         return run_test(model, args, device)
     optimizer = build_optimizer(model, args)
@@ -598,6 +640,17 @@ def main(args):
     args.seed_base = args.start_epoch * 2
     train_loader = get_data(args, device, 'train')
     val_loader = get_data(args, device, 'val')
+    try:
+        train_epochs(args, model, optimizer, criterion, train_loader, val_loader, model_path, best_acc)
+    finally:
+        for loader in (train_loader, val_loader):
+            if hasattr(loader, 'close'):
+                loader.close()
+    print('Training from ep %d to ep %d finished' % (args.start_epoch, args.epochs))
+    return model
+
+
+def train_epochs(args, model, optimizer, criterion, train_loader, val_loader, model_path, best_acc):
     for epoch in range(args.start_epoch, args.epochs):
         np.random.seed(epoch)
         random.seed(epoch)
@@ -615,8 +668,6 @@ def main(args):
                 os.remove(prev)
             if is_best:
                 torch.save(state, os.path.join(model_path, 'model_best.pth.tar'))
-    print('Training from ep %d to ep %d finished' % (args.start_epoch, args.epochs))
-    return model
 
 
 if __name__ == '__main__':

@@ -669,6 +669,18 @@ typedef struct {
 } coclr_jpeg_t;
 size_t coclr_jpeg_work_bytes(const coclr_jpeg_t* p);
 int coclr_jpeg_decode(const coclr_jpeg_t* p, coclr_stream_t stream);
+/* Repeated frames: coclr_jpeg_decode_slots writes parsed frame i to output frames slots[slot_begin[i] ..
+ * slot_begin[i + 1]) -- each pixel computed once and stored once per slot -- so a frame sampled several times is
+ * decoded once.  The host copies are validated before any launch: every output frame in [0, n_out) is written exactly
+ * once.  slot_begin == NULL (or s == NULL) is coclr_jpeg_decode: frame i goes to output frame i. */
+typedef struct {
+  const int* slot_begin;                  /* device [n + 1], or NULL */
+  const int* slots;                       /* device [slot_begin[n]] */
+  const int* slot_begin_host;             /* host copies of the two */
+  const int* slots_host;
+  int n_out;
+} coclr_jpeg_slots_t;
+int coclr_jpeg_decode_slots(const coclr_jpeg_t* p, const coclr_jpeg_slots_t* s, coclr_stream_t stream);
 
 #ifdef __cplusplus
 }

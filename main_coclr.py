@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """CoCLR co-training driver -- command line of the reference's main_coclr.py (:38-95) for the accelerated hot
-path, with --synthetic / --gpu-augment / --jpeg / --precision / --steps-per-epoch as in main_nce.py.
+path, with --synthetic / --gpu-augment / --jpeg / --precision / --steps-per-epoch / --data-root / --split-root as in
+main_nce.py.
 
 Loop semantics kept from the reference (main_coclr.py:348-435): the sampler stays in eval mode (:363); the
 self-positive column is masked out with probability 0.9 for rows that have other positives (:382-388, Python
@@ -183,28 +184,37 @@ def main_worker(args):
         load_two_checkpoints(model, args.pretrain2)
     if args.test:
         return model
-    if not args.synthetic:
+    if args.data_root and not args.synthetic:
+        base.check_jpeg_flag(args)
+        model.set_input_transform(mean=[0.485, 0.456, 0.406], std=[0.229, 0.224, 0.225])
+        loader = base.lmdb_loader(args, device, two_stream=True)
+    elif not args.synthetic:
         raise NotImplementedError("the 2-stream LMDB datasets are outside the accelerated hot path; use --synthetic")
-    base.check_jpeg_flag(args)
-    if args.gpu_augment:
+    else:
+        base.check_jpeg_flag(args)
+    if args.synthetic and args.gpu_augment:
         model.set_input_transform(mean=[0.485, 0.456, 0.406], std=[0.229, 0.224, 0.225])
         loader = base.SyntheticSourceFrames(args, device, two_stream=True)
-    else:
+    elif args.synthetic:
         loader = SyntheticTwoStream(args, device)
     model_path = base.set_path(args)
-    for epoch in range(args.start_epoch, args.epochs):
-        np.random.seed(epoch)                                      # reference main_coclr.py:314-315: the 90 % self-mask
-        random.seed(epoch)                                         # draws restart per epoch (reproducible across resume)
-        base.adjust_learning_rate(optimizer, epoch, args)
-        loss, acc = train_one_epoch(loader, model, optimizer, epoch, args)
-        if args.rank == 0 and ((epoch % args.save_freq == 0) or (epoch == args.epochs - 1)):
-            is_best = acc > best_acc
-            best_acc = max(acc, best_acc)
-            base.save_checkpoint({'epoch': epoch, 'state_dict': model.state_dict(), 'best_acc': best_acc,
-                                  'optimizer': optimizer.state_dict(), 'iteration': args.iteration},
-                                 is_best, gap=args.save_freq,
-                                 filename=os.path.join(model_path, 'epoch%d.pth.tar' % epoch),
-                                 keep_all='k400' in args.dataset)
+    try:
+        for epoch in range(args.start_epoch, args.epochs):
+            np.random.seed(epoch)                                  # reference main_coclr.py:314-315: the 90 % self-mask
+            random.seed(epoch)                                     # draws restart per epoch (reproducible across resume)
+            base.adjust_learning_rate(optimizer, epoch, args)
+            loss, acc = train_one_epoch(loader, model, optimizer, epoch, args)
+            if args.rank == 0 and ((epoch % args.save_freq == 0) or (epoch == args.epochs - 1)):
+                is_best = acc > best_acc
+                best_acc = max(acc, best_acc)
+                base.save_checkpoint({'epoch': epoch, 'state_dict': model.state_dict(), 'best_acc': best_acc,
+                                      'optimizer': optimizer.state_dict(), 'iteration': args.iteration},
+                                     is_best, gap=args.save_freq,
+                                     filename=os.path.join(model_path, 'epoch%d.pth.tar' % epoch),
+                                     keep_all='k400' in args.dataset)
+    finally:
+        if hasattr(loader, 'close'):
+            loader.close()
     print('Training from ep %d to ep %d finished' % (args.start_epoch, args.epochs))
     if args.distributed:
         dist.destroy_process_group()

@@ -2,9 +2,8 @@
 """InfoNCE / UberNCE pre-training driver -- same command line as the reference's main_nce.py (:38-93) for the
 hot path this repository accelerates, plus:
 
-  --synthetic            random clips of the dataset's shape instead of the LMDB loaders (the reference's dataset/
-                         readers are outside the accelerated path; without --synthetic a dataset name raises, because
-                         lmdb/msgpack are not part of this repository)
+  --synthetic            random clips of the dataset's shape instead of the LMDB loaders (without --synthetic or
+                         --data-root a dataset name raises)
   --precision MODE       parity | mixed | fast (see DESIGN.md)
   --steps-per-epoch N    length of a synthetic epoch
   --gpu-augment          with --synthetic: the loader yields seeded uint8 source frames (--source-size H W, 240 320 by
@@ -13,6 +12,10 @@ hot path this repository accelerates, plus:
   --jpeg                 with --synthetic --gpu-augment: the loader holds a seeded pool of videos as lists of JPEG
                          bytes (the reference LMDB's value format, encoded once by Pillow at --source-size); each
                          batch's frames are decoded on the GPU (coclr_b200.jpeg) in front of the augmentation
+  --data-root DIR        the reference's LMDB databases in its relative layout (UCF101/ucf101_frame.lmdb, ...,
+  --split-root DIR       kinetics400-256/frame_full/lmdb/k400_frame_train.lmdb) and its split files (ucf101/, k400/
+                         as in process_data/data/): the dataset is read with coclr_b200.datasets, each batch's
+                         distinct frames are decoded once on the GPU and augmented there (coclr_b200.loaders)
 
 Launch like the reference: `python -m torch.distributed.run --nproc_per_node=N main_nce.py ...` (one process per
 GPU; --local_rank, --local-rank and the LOCAL_RANK env variable are all accepted).
@@ -88,6 +91,8 @@ def parse_args(argv=None):
     p.add_argument('--jpeg', action='store_true',
                    help='with --synthetic --gpu-augment: decode a pool of JPEG-encoded videos on the GPU in front of '
                         'the augmentation')
+    p.add_argument('--data-root', default=None, help='directory of the reference\'s LMDB databases')
+    p.add_argument('--split-root', default=None, help='directory of the reference\'s split files (ucf101/, k400/)')
     p.add_argument('--precision', default='parity', choices=['parity', 'mixed', 'fast'])
     p.add_argument('--steps-per-epoch', default=20, type=int)
     p.add_argument('--num-classes', default=101, type=int, help='label range of the synthetic UberNCE labels')
@@ -182,7 +187,53 @@ def check_jpeg_flag(args):
         raise NotImplementedError("--jpeg decodes the synthetic JPEG pool of --synthetic --gpu-augment")
 
 
+def lmdb_dataset(args, mode='train'):
+    """get_data of the reference's main_nce.py / main_coclr.py over --data-root / --split-root."""
+    from coclr_b200 import datasets as D
+    if not args.split_root:
+        raise ValueError("--data-root needs --split-root (the reference's process_data/data directory)")
+    data, split = args.data_root, args.split_root
+    kw = dict(mode=mode, num_frames=args.seq_len, ds=args.ds, return_label=True)
+    k400 = os.path.join(data, 'kinetics400-256')
+    if args.dataset == 'ucf101-2clip':
+        return D.UCF101LMDB_2CLIP(root=os.path.join(split, 'ucf101'),
+                                  db_path=os.path.join(data, 'UCF101', 'ucf101_frame.lmdb'), **kw)
+    if args.dataset == 'ucf101-f-2clip':
+        return D.UCF101Flow_LMDB_2CLIP(root=os.path.join(split, 'ucf101'),
+                                       db_path=os.path.join(data, 'UCF101', 'ucf101_tvl1_frame.lmdb'), **kw)
+    if args.dataset == 'k400-2clip':
+        return D.K400_LMDB_2CLIP(root=os.path.join(split, 'k400'),
+                                 db_path=os.path.join(k400, 'frame_full', 'lmdb'), **kw)
+    if args.dataset == 'k400-f-2clip':
+        return D.K400_Flow_LMDB_2CLIP(root=os.path.join(split, 'k400'),
+                                      db_path=os.path.join(k400, 'tvl1_flow', 'lmdb'), **kw)
+    if args.dataset == 'ucf101-2stream-2clip':
+        return D.UCF101_2STREAM_LMDB_2CLIP(root=os.path.join(split, 'ucf101'),
+                                           db_path_flow=os.path.join(data, 'UCF101', 'ucf101_tvl1_frame.lmdb'),
+                                           db_path_rgb=os.path.join(data, 'UCF101', 'ucf101_frame.lmdb'),
+                                           return_source=True, **kw)
+    if args.dataset == 'k400-2stream-2clip':
+        return D.K400_2STREAM_LMDB_2CLIP(root=os.path.join(split, 'k400'),
+                                         db_path_flow=os.path.join(k400, 'tvl1_flow', 'lmdb'),
+                                         db_path_rgb=os.path.join(k400, 'frame_full', 'lmdb'),
+                                         return_source=True, **kw)
+    raise NotImplementedError("dataset %r" % args.dataset)
+
+
+def lmdb_loader(args, device, two_stream=False):
+    """Pre-training batches of --data-root: what SyntheticSourceFrames yields, from the dataset's frames."""
+    from coclr_b200.loaders import PretrainBatches
+    if two_stream != args.dataset.endswith('2stream-2clip'):
+        raise NotImplementedError("dataset %r" % args.dataset)
+    return PretrainBatches(lmdb_dataset(args), args.batch_size, args.seq_len, args.img_dim, device,
+                           seed=args.seed * 1000 + args.rank, rank=args.rank, world_size=args.world_size,
+                           two_stream=two_stream)
+
+
 def get_data(args, device):
+    if getattr(args, 'data_root', None) and not args.synthetic:
+        check_jpeg_flag(args)
+        return lmdb_loader(args, device)
     if not args.synthetic:
         raise NotImplementedError(
             "dataset %r: the LMDB/JPEG loaders of the reference (dataset/) are outside the accelerated hot path; run "
@@ -315,7 +366,7 @@ def main_worker(args):
     random.seed(args.seed)
     cls = {'infonce': InfoNCE, 'ubernce': UberNCE}[args.model]
     model = cls(args.net, args.moco_dim, args.moco_k, args.moco_m, args.moco_t, precision=args.precision).to(device)
-    if args.raw_input or args.gpu_augment:
+    if args.raw_input or args.gpu_augment or (args.data_root and not args.synthetic):
         model.set_input_transform(mean=[0.485, 0.456, 0.406], std=[0.229, 0.224, 0.225])   # reference main_nce.py:207-209
     optimizer = moco.FlatAdam(model.encoder_q, lr=args.lr, weight_decay=args.wd)
     args.iteration = 1
@@ -335,19 +386,23 @@ def main_worker(args):
         return model
     loader = get_data(args, device)
     model_path = set_path(args)
-    for epoch in range(args.start_epoch, args.epochs):
-        np.random.seed(epoch)
-        random.seed(epoch)
-        adjust_learning_rate(optimizer, epoch, args)
-        loss, acc = train_one_epoch(loader, model, optimizer, epoch, args)
-        if args.rank == 0 and ((epoch % args.save_freq == 0) or (epoch == args.epochs - 1)):
-            is_best = acc > best_acc
-            best_acc = max(acc, best_acc)
-            save_checkpoint({'epoch': epoch, 'state_dict': model.state_dict(), 'best_acc': best_acc,
-                             'optimizer': optimizer.state_dict(), 'iteration': args.iteration},
-                            is_best, gap=args.save_freq,
-                            filename=os.path.join(model_path, 'epoch%d.pth.tar' % epoch),
-                            keep_all='k400' in args.dataset)
+    try:
+        for epoch in range(args.start_epoch, args.epochs):
+            np.random.seed(epoch)
+            random.seed(epoch)
+            adjust_learning_rate(optimizer, epoch, args)
+            loss, acc = train_one_epoch(loader, model, optimizer, epoch, args)
+            if args.rank == 0 and ((epoch % args.save_freq == 0) or (epoch == args.epochs - 1)):
+                is_best = acc > best_acc
+                best_acc = max(acc, best_acc)
+                save_checkpoint({'epoch': epoch, 'state_dict': model.state_dict(), 'best_acc': best_acc,
+                                 'optimizer': optimizer.state_dict(), 'iteration': args.iteration},
+                                is_best, gap=args.save_freq,
+                                filename=os.path.join(model_path, 'epoch%d.pth.tar' % epoch),
+                                keep_all='k400' in args.dataset)
+    finally:
+        if hasattr(loader, 'close'):
+            loader.close()
     print('Training from ep %d to ep %d finished' % (args.start_epoch, args.epochs))
     if args.distributed:
         dist.destroy_process_group()
