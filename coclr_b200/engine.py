@@ -12,6 +12,7 @@ gradient buffer).  Parameters live in ONE flat fp32 buffer per encoder (nn.Param
 EMA / Adam / all-reduce are single launches over it.
 """
 import ctypes as C
+from collections import namedtuple
 
 import torch
 
@@ -36,6 +37,26 @@ def _round8(c):
     return (c + 7) // 8 * 8
 
 
+class Launch(namedtuple("Launch", "fn args")):
+    """One launch of a plan, fn(*args, stream), which unpacks as (fn, args).  It runs on stream lane `lane` (0: the
+    caller's current stream, 1..3: the engine's own streams) once that lane has waited for `wait`, and it is `kernels`
+    kernels of the library (L.kernels_of, set by the plan once the launch's workspace is known)."""
+
+    def __new__(cls, fn, args, lane=0, wait=None):
+        r = super().__new__(cls, fn, args)
+        r.lane, r.wait, r.kernels = lane, wait, None
+        return r
+
+
+# Launch.wait.  The Inception branches of a Mixed block run on lanes 1..3 from the block's fork point, an event that
+# lane 0 records before the block's first launch.
+FORK = "fork"          # lane 0 records the fork point, the launch's lane waits for it
+AT_FORK = "at fork"    # the fork point (not lane 0's current point: work queued there since must not delay the branch)
+AFTER1 = "after 1"     # the fork point, then the work lane 1 has been given so far
+AFTER0 = "after 0"     # the work lane 0 has been given so far
+JOIN = "join"          # on lane 0: every lane that waited for something since the last JOIN
+
+
 # ---------------------------------------------------------------------------------------------
 # symbolic graph
 # ---------------------------------------------------------------------------------------------
@@ -46,6 +67,7 @@ class TensorSpec:
         self.relu = 1 if pending else 0
         self.residual = None   # TensorSpec added before the ReLU (ResNet bottleneck output)
         self.gates = []        # S3D-G: (SelfGating module name, coff, C) per branch slice of a SepInception output
+        self.lane, self.wait = 0, None   # as a BatchNorm item: lane of its launches, wait of the first (Launch)
 
 
 class ConvSpec:
@@ -60,12 +82,14 @@ class ConvSpec:
         self.src_coff, self.src_C = 0, src.C
         # parameter names whose (adjacent) [cout_i, cin, 1, 1, 1] weights this conv uses as one [sum cout_i, cin] matrix
         self.weight_names = [name]
+        self.lane, self.wait = 0, None
 
 
 class PoolSpec:
     def __init__(self, name, src, dst, k, s, p):
         self.name, self.src, self.dst, self.k, self.s, self.p = name, src, dst, k, s, p
         self.fused = False   # pools straight from its source's conv output (see Graph._fuse_pools)
+        self.lane, self.wait = 0, None
 
 
 # (kernel, stride) of the pools coclr_maxpool_fwd can run from a conv output (coclr_pool_t.y)
@@ -74,24 +98,6 @@ FUSED_POOL_WINDOWS = {((1, 3, 3), (1, 2, 2)), ((3, 3, 3), (2, 2, 2)), ((2, 2, 2)
 
 def _conv_out(d, k, s, p):
     return (d + 2 * p - k) // s + 1
-
-
-FORK, JOIN, AFTER1 = 1, 2, 3   # AFTER1: the item's lane first waits for what lane 1 has been given so far
-
-
-class _LaneList(list):
-    """items list that records the current lane / pending flag of the graph builder for every appended item."""
-
-    def __init__(self, graph):
-        super().__init__()
-        self.graph = graph
-
-    def append(self, item):
-        g = self.graph
-        g.item_lane.append(g.cur_lane)
-        g.item_flag.append(g.next_flag)
-        g.next_flag = 0
-        super().append(item)
 
 
 class Graph:
@@ -103,9 +109,7 @@ class Graph:
         backward starts from that feature's gradient (LinearClassifier's backbone)."""
         assert not (pooled and head_dim is not None)
         self.pooled = pooled
-        self.tensors, self.items = [], _LaneList(self)   # items: ("conv", ConvSpec) | ("pool", PoolSpec) | ("bn", TensorSpec)
-        self.item_lane, self.item_flag = [], []   # per item: stream lane (Inception branches run concurrently) and FORK/JOIN
-        self.cur_lane, self.next_flag = 0, 0
+        self.tensors, self.items = [], []   # items: ("conv", ConvSpec) | ("pool", PoolSpec) | ("bn", TensorSpec)
         self.first_channel = first_channel
         self.head_dim, self.feature_size = head_dim, feature_size
         pre = bb_prefix
@@ -244,28 +248,37 @@ class Graph:
         # the 1x1x1 convs that open branches 1 and 2 read the same input: they run as ONE conv (N = o1a + o2a instead
         # of e.g. 96 and 16 output channels) into one buffer that the two branches slice
         t12 = self._tensor(name + ".b12a", o1a + o2a, self._same(x))
-        self.cur_lane, self.next_flag = 1, FORK     # lane 1: fused 1x1 conv + its BN, then branch 1
+        n = len(self.items)   # lane 1: fused 1x1 conv + its BN, then branch 1
         cv = self._conv(name + ".branch1.0.conv", x, t12, 0, cin, o1a + o2a, *one)
         cv.weight_names, cv.couts = [name + ".branch1.0.conv", name + ".branch2.0.conv"], [o1a, o2a]
         t12.bn_members += [(name + ".branch1.0.bn", 0, o1a), (name + ".branch2.0.bn", o1a, o2a)]
         self.items.append(("bn", t12))
-        self.cur_lane, self.next_flag = 2, AFTER1   # lane 2: branch 2 starts once the shared buffer is ready
+        self._on_lane(n, 1, FORK)
+        n = len(self.items)   # lane 2: branch 2 starts once the shared buffer is ready
         self._st(name + ".branch2.1", t12, cat, o0 + o1b, o2a, o2b, 3, 1, 1, 1, src_coff=o1a)
-        self.cur_lane = 1
+        self._on_lane(n, 2, AFTER1)
+        n = len(self.items)
         self._st(name + ".branch1.1", t12, cat, o0, o1a, o1b, 3, 1, 1, 1, src_coff=0)
-        self.cur_lane = 0
+        self._on_lane(n, 1, None)
         self._conv(name + ".branch0.0.conv", x, cat, 0, cin, o0, *one)
         cat.bn_members.append((name + ".branch0.0.bn", 0, o0))
-        self.cur_lane = 3
+        n = len(self.items)
         tp = self._pool(name + ".branch3.0", x, (3, 3, 3), (1, 1, 1), (1, 1, 1))
         self._conv(name + ".branch3.1.conv", tp, cat, o0 + o1b + o2b, cin, o3b, *one)
         cat.bn_members.append((name + ".branch3.1.bn", o0 + o1b + o2b, o3b))
+        self._on_lane(n, 3, AT_FORK)
         # the branches were issued out of channel order; the per-tensor BatchNorm needs its members' parameters laid
         # out in channel order (one gamma / beta vector for the whole concat buffer)
         cat.bn_members.sort(key=lambda m: m[1])
-        self.cur_lane, self.next_flag = 0, JOIN
+        cat.wait = JOIN
         self.items.append(("bn", cat))
         return cat
+
+    def _on_lane(self, start, lane, wait):
+        """Put the items appended since items[start] on stream lane `lane`, the first of them waiting for `wait`."""
+        for _, spec in self.items[start:]:
+            spec.lane = lane
+        self.items[start][1].wait = wait
 
     def _bottleneck(self, name, x, inplanes, planes, stride, is3d, has_ds):
         """Bottleneck2d / Bottleneck3d (backbone/resnet_2d3d.py:46-131): conv1 (1x1x1 or (3,1,1)) -> conv2 (1,3,3) with
@@ -464,6 +477,13 @@ class _PoolInputView:
         return pl.value()
 
 
+def _count_kernels(records):
+    """Set each record's kernel count (L.kernels_of); returns their total."""
+    for r in records:
+        r.kernels = L.kernels_of(r.fn, r.args)
+    return sum(r.kernels for r in records)
+
+
 class Plan:
     """Buffers + launch lists for one (B, T, H, W, training) configuration."""
 
@@ -472,9 +492,8 @@ class Plan:
         g, dev = eng.graph, eng.store.device
         lib = L.load()
         self.keep = []          # keeps ctypes structs / tensors alive
-        self.fwd, self.bwd = [], []
-        self.fwd_lane = {}      # index into self.fwd -> (lane, FORK/JOIN flag)
-        self.graphs = {}        # captured CUDA graphs of the launch lists
+        self.fwd, self.bwd = [], []   # Launch records
+        self.graphs = {}      # captured CUDA graphs of the launch lists
         nsm = L.num_sms(dev)
         fnp, fbf, bnp = PRECISIONS[eng.precision]
         # gradient planes: with fp16 forward planes dY is stored as fp16 hi/lo of dY * 2^k (k per tensor and step, chosen
@@ -551,7 +570,7 @@ class Plan:
                 return None, None
             return L.dptr(plw.hi), L.dptr(plw.lo)
 
-        def split_op(x, planes, M, Cc, scale, shift, relu, twin=None, bn=None, res=None):
+        def split_op(x, planes, M, Cc, scale, shift, relu, twin=None, bn=None, res=None, lane=0):
             t_hi, t_lo = twin_ptrs(planes, twin)
             sp = L.Split(L.dptr(x), x.shape[-1], 0, Cc, M, L.dptr(scale), L.dptr(shift), int(bool(relu)),
                          L.dptr(planes.hi), L.dptr(planes.lo), planes.ld, 0, planes.bf16, t_hi, t_lo,
@@ -559,10 +578,10 @@ class Plan:
                          L.dptr(res.hi) if res is not None else None, L.dptr(res.lo) if res is not None else None,
                          res.ld if res is not None else 0, 0)
             self.keep.append(sp)
-            return (lib.coclr_affine_split, (C.byref(sp), nsm))
+            return Launch(lib.coclr_affine_split, (C.byref(sp), nsm), lane)
 
         # ---- forward ----
-        for item_i, (kind, it) in enumerate(g.items):
+        for kind, it in g.items:
             n_before = len(self.fwd)
             if kind == "conv":
                 sa, da = acts[it.src.index], acts[it.dst.index]
@@ -572,7 +591,7 @@ class Plan:
                                    stats_sum=da.ssum[it.dst_coff:] if training else None,
                                    stats_sq=da.ssq[it.dst_coff:] if training else None, npass=fnp)
                 self.keep.append(cv)
-                self.fwd.append((lib.coclr_conv_igemm, (C.byref(cv), nsm)))
+                self.fwd.append(Launch(lib.coclr_conv_igemm, (C.byref(cv), nsm), it.lane))
             elif kind == "pool":
                 sa, da = acts[it.src.index], acts[it.dst.index]
                 geom = ops.Geometry(it.k, it.s, it.p)
@@ -586,7 +605,7 @@ class Plan:
                 if fused:   # BatchNorm + ReLU applied while loading the conv output
                     pl.y, pl.scale, pl.shift, pl.relu = L.dptr(sa.data), L.dptr(sa.scale), L.dptr(sa.shift), it.src.relu
                 self.keep.append(pl)
-                self.fwd.append((lib.coclr_maxpool_fwd, (C.byref(pl),)))
+                self.fwd.append(Launch(lib.coclr_maxpool_fwd, (C.byref(pl),), it.lane))
             elif kind == "bn":
                 a = acts[it.index]
                 first = it.bn_members[0][0]
@@ -603,27 +622,26 @@ class Plan:
                     sp = L.Split(L.dptr(a.data), it.C, 0, it.C, a.M, None, None, it.relu, None, None, it.C, 0, 0,
                                  None, None, bf)
                     self.keep.append(sp)
-                    self.fwd.append((lib.coclr_affine_split, (C.byref(sp), nsm)))
+                    self.fwd.append(Launch(lib.coclr_affine_split, (C.byref(sp), nsm), it.lane))
                 else:
                     # BatchNorm finalize is fused into the apply+split launch
                     res = acts[it.residual.index].pl if it.residual is not None else None
-                    self.fwd.append(split_op(a.data, a.pl, a.M, it.C, None, None, it.relu, bn=bf, res=res))
+                    self.fwd.append(split_op(a.data, a.pl, a.M, it.C, None, None, it.relu, bn=bf, res=res, lane=it.lane))
                 if it.gates:
                     # S3D-G feature gating of the block output: the planes written above are scaled in place by
                     # sigmoid(fc(mean_thw)) per clip and channel (csrc/gating.cu)
                     Pn = a.dims[0] * a.dims[1] * a.dims[2]
                     a.gmean = torch.empty(B, it.C, dtype=torch.float32, device=dev)
                     a.gate = torch.empty(B, it.C, dtype=torch.float32, device=dev)
-                    self.fwd.append((lib.coclr_gate_mean, (L.dptr(a.pl.hi), L.dptr(a.pl.lo), a.pl.bf16, a.pl.ld, B, Pn,
-                                                           it.C, L.dptr(a.gmean))))
+                    self.fwd.append(Launch(lib.coclr_gate_mean, (L.dptr(a.pl.hi), L.dptr(a.pl.lo), a.pl.bf16, a.pl.ld, B,
+                                                              Pn, it.C, L.dptr(a.gmean)), it.lane))
                     for nm, coff, c in it.gates:
-                        self.fwd.append((lib.coclr_gate_fc, (L.dptr(a.gmean), L.dptr(st.view(nm + ".fc.weight")),
-                                                             L.dptr(st.view(nm + ".fc.bias")), L.dptr(a.gate), B, it.C,
-                                                             coff, c)))
-                    self.fwd.append((lib.coclr_gate_apply, (L.dptr(a.pl.hi), L.dptr(a.pl.lo), a.pl.bf16, a.pl.ld, B, Pn,
-                                                            it.C, L.dptr(a.gate))))
-            for j in range(n_before, len(self.fwd)):     # tag the launches of this item with its lane / fork / join
-                self.fwd_lane[j] = (g.item_lane[item_i], g.item_flag[item_i] if j == n_before else 0)
+                        self.fwd.append(Launch(lib.coclr_gate_fc, (L.dptr(a.gmean), L.dptr(st.view(nm + ".fc.weight")),
+                                                                L.dptr(st.view(nm + ".fc.bias")), L.dptr(a.gate), B, it.C,
+                                                                coff, c), it.lane))
+                    self.fwd.append(Launch(lib.coclr_gate_apply, (L.dptr(a.pl.hi), L.dptr(a.pl.lo), a.pl.bf16, a.pl.ld, B,
+                                                               Pn, it.C, L.dptr(a.gate)), it.lane))
+            self.fwd[n_before].wait = it.wait   # the item's first launch waits
         # ---- head ----
         out = acts[g.backbone_out.index]
         self.backbone_out = out
@@ -642,8 +660,8 @@ class Plan:
             mk_twin = with_backward and not fbf
             self.feat_plw = ops.Planes((B, 1, 1, 1, fs), 1, dev, lo=bnp > 1) if mk_twin else self.feat_pl
             self.h1_plw = ops.Planes((B, 1, 1, 1, fs), 1, dev, lo=bnp > 1) if mk_twin else self.h1_pl
-            self.fwd.append((lib.coclr_avgpool_fwd, (L.dptr(out.pl.hi), L.dptr(out.pl.lo), out.pl.bf16, out.spec.C, 0,
-                                                     L.dptr(self.feat), B, Pn, fs)))
+            self.fwd.append(Launch(lib.coclr_avgpool_fwd, (L.dptr(out.pl.hi), L.dptr(out.pl.lo), out.pl.bf16, out.spec.C,
+                                                        0, L.dptr(self.feat), B, Pn, fs)))
             self.fwd.append(split_op(self.feat, self.feat_pl, B, fs, None, None, False, self.feat_plw))
             one = ops.Geometry((1, 1, 1))
             b2, b4 = st.view("2.bias"), st.view("4.bias")
@@ -652,20 +670,25 @@ class Plan:
             c1 = ops.make_conv(s_feat, fbf, one.c(0), B, (1, 1, 1), eng.packed_fwd["2"], self.h1, npass=fnp)
             c2 = ops.make_conv(s_h1, fbf, one.c(0), B, (1, 1, 1), eng.packed_fwd["4"], self.h2, npass=fnp)
             self.keep += [c1, c2, s_feat, s_h1]
-            self.fwd.append((lib.coclr_conv_igemm, (C.byref(c1), nsm)))
+            self.fwd.append(Launch(lib.coclr_conv_igemm, (C.byref(c1), nsm)))
             self.fwd.append(split_op(self.h1, self.h1_pl, B, fs, self.ones, b2, True, self.h1_plw))   # bias + ReLU
-            self.fwd.append((lib.coclr_conv_igemm, (C.byref(c2), nsm)))
-            self.fwd.append((lib.coclr_l2norm_fwd, (L.dptr(self.h2), L.dptr(b4), L.dptr(self.q), L.dptr(self.inv_norm), B, hd)))
+            self.fwd.append(Launch(lib.coclr_conv_igemm, (C.byref(c2), nsm)))
+            self.fwd.append(Launch(lib.coclr_l2norm_fwd, (L.dptr(self.h2), L.dptr(b4), L.dptr(self.q), L.dptr(self.inv_norm),
+                                                       B, hd)))
         elif g.pooled:
             fs, Pn = g.feature_size, out.dims[0] * out.dims[1] * out.dims[2]
             self.feat = torch.empty(B, fs, dtype=torch.float32, device=dev)
-            self.fwd.append((lib.coclr_avgpool_fwd, (L.dptr(out.pl.hi), L.dptr(out.pl.lo), out.pl.bf16, out.spec.C, 0,
-                                                     L.dptr(self.feat), B, Pn, fs)))
+            self.fwd.append(Launch(lib.coclr_avgpool_fwd, (L.dptr(out.pl.hi), L.dptr(out.pl.lo), out.pl.bf16, out.spec.C,
+                                                        0, L.dptr(self.feat), B, Pn, fs)))
+        self.fwd_kernels, self.bwd_kernels = _count_kernels(self.fwd), 0
         if not with_backward:
             return
         # ---- backward ----
         bw = self.bwd
-        self.wgrads, self.s2d_wgrads = [], []   # coclr_wgrad_t structs of the plan (workspaces: end of this method)
+        # The weight gradients that share the workspace wg_ws (sized at the end) run one after another on lane 1, each
+        # once lane 0 has produced its dY: nothing later in the pass reads dW, and small layers leave most SMs idle, so
+        # the two chains overlap.
+        self.wgrads, self.s2d_wgrads = [], []   # coclr_wgrad_t structs of the shared and the own-workspace launches
         if g.head_dim is not None:
             self.dq = torch.empty(B, hd, **f32)
             self.dh2 = torch.empty(B, 1, 1, 1, hd, **f32)
@@ -673,8 +696,8 @@ class Plan:
             self.dfeat = torch.empty(B, 1, 1, 1, fs, **f32)
             self.dh2_pl = ops.Planes((B, 1, 1, 1, hd), 1, dev, lo=bnp > 1)
             self.dh1_pl = ops.Planes((B, 1, 1, 1, fs), 1, dev, lo=bnp > 1)
-            bw.append((lib.coclr_l2norm_bwd, (L.dptr(self.q), L.dptr(self.dq), L.dptr(self.inv_norm), L.dptr(self.dh2),
-                                              L.dptr(st.view("4.bias", grad=True)), B, hd)))
+            bw.append(Launch(lib.coclr_l2norm_bwd, (L.dptr(self.q), L.dptr(self.dq), L.dptr(self.inv_norm), L.dptr(self.dh2),
+                                                 L.dptr(st.view("4.bias", grad=True)), B, hd)))
             bw.append(split_op(self.dh2, self.dh2_pl, B, hd, None, None, False))
             s_dh2 = self.dh2_pl.src(0, hd, 1, 1, 1)
             s_dh1 = self.dh1_pl.src(0, fs, 1, 1, 1)
@@ -686,18 +709,18 @@ class Plan:
             dg1 = ops.make_conv(s_dh1, 1, one.c(1), B, (1, 1, 1), eng.packed_bwd["2"], self.dfeat, npass=bnp)
             self.keep += [s_dh2, wg2, dg2, s_dh1, wg1, dg1]
             self.wgrads += [wg2, wg1]
-            bw.append((lib.coclr_conv_wgrad, (C.byref(wg2),)))
-            bw.append((lib.coclr_conv_igemm, (C.byref(dg2), nsm)))
-            bw.append((lib.coclr_bias_relu_bwd, (L.dptr(self.h1), L.dptr(b2), L.dptr(self.dh1),
-                                                 L.dptr(st.view("2.bias", grad=True)), B, fs)))
+            bw.append(Launch(lib.coclr_conv_wgrad, (C.byref(wg2),), 1, AFTER0))
+            bw.append(Launch(lib.coclr_conv_igemm, (C.byref(dg2), nsm)))
+            bw.append(Launch(lib.coclr_bias_relu_bwd, (L.dptr(self.h1), L.dptr(b2), L.dptr(self.dh1),
+                                                    L.dptr(st.view("2.bias", grad=True)), B, fs)))
             bw.append(split_op(self.dh1, self.dh1_pl, B, fs, None, None, False))
-            bw.append((lib.coclr_conv_wgrad, (C.byref(wg1),)))
-            bw.append((lib.coclr_conv_igemm, (C.byref(dg1), nsm)))
-            bw.append((lib.coclr_avgpool_bwd, (L.dptr(self.dfeat), L.dptr(out.grad), out.spec.C, 0, B, Pn, fs)))
+            bw.append(Launch(lib.coclr_conv_wgrad, (C.byref(wg1),), 1, AFTER0))
+            bw.append(Launch(lib.coclr_conv_igemm, (C.byref(dg1), nsm)))
+            bw.append(Launch(lib.coclr_avgpool_bwd, (L.dptr(self.dfeat), L.dptr(out.grad), out.spec.C, 0, B, Pn, fs)))
             grad_seen(out)
         elif g.pooled:
             self.dfeat = torch.empty(B, fs, dtype=torch.float32, device=dev)
-            bw.append((lib.coclr_avgpool_bwd, (L.dptr(self.dfeat), L.dptr(out.grad), out.spec.C, 0, B, Pn, fs)))
+            bw.append(Launch(lib.coclr_avgpool_bwd, (L.dptr(self.dfeat), L.dptr(out.grad), out.spec.C, 0, B, Pn, fs)))
             grad_seen(out)
         convs_into, pool_into = {}, {}
         for kind, it in g.items:
@@ -719,15 +742,16 @@ class Plan:
                     Pn = a.dims[0] * a.dims[1] * a.dims[2]
                     a.dgate = torch.empty(B, t.C, dtype=torch.float32, device=dev)
                     a.dmean = torch.empty(B, t.C, dtype=torch.float32, device=dev)
-                    bw.append((lib.coclr_gate_bwd_reduce, (L.dptr(a.data), t.C, L.dptr(a.scale), L.dptr(a.shift), t.relu,
-                                                           L.dptr(a.grad), t.C, B, Pn, t.C, L.dptr(a.dgate))))
+                    bw.append(Launch(lib.coclr_gate_bwd_reduce, (L.dptr(a.data), t.C, L.dptr(a.scale), L.dptr(a.shift),
+                                                              t.relu, L.dptr(a.grad), t.C, B, Pn, t.C, L.dptr(a.dgate))))
                     for nm, coff, c in t.gates:
-                        bw.append((lib.coclr_gate_fc_bwd, (L.dptr(a.dgate), L.dptr(a.gate), L.dptr(a.gmean),
-                                                           L.dptr(st.view(nm + ".fc.weight")),
-                                                           L.dptr(st.view(nm + ".fc.weight", grad=True)),
-                                                           L.dptr(st.view(nm + ".fc.bias", grad=True)), L.dptr(a.dmean),
-                                                           B, t.C, coff, c)))
-                    bw.append((lib.coclr_gate_bwd_apply, (L.dptr(a.grad), t.C, L.dptr(a.gate), L.dptr(a.dmean), B, Pn, t.C)))
+                        bw.append(Launch(lib.coclr_gate_fc_bwd, (L.dptr(a.dgate), L.dptr(a.gate), L.dptr(a.gmean),
+                                                              L.dptr(st.view(nm + ".fc.weight")),
+                                                              L.dptr(st.view(nm + ".fc.weight", grad=True)),
+                                                              L.dptr(st.view(nm + ".fc.bias", grad=True)), L.dptr(a.dmean),
+                                                              B, t.C, coff, c)))
+                    bw.append(Launch(lib.coclr_gate_bwd_apply, (L.dptr(a.grad), t.C, L.dptr(a.gate), L.dptr(a.dmean), B, Pn,
+                                                             t.C)))
                 a.bsums = torch.zeros(2 * t.C, dtype=torch.float64, device=dev)
                 a.bamax = torch.zeros(2 * t.C, dtype=torch.float32, device=dev)
                 first = t.bn_members[0][0]
@@ -745,7 +769,7 @@ class Plan:
                              0 if gbf else 1, L.dptr(a.bamax), L.dptr(a.dy_scale))
                 oscale = None if gbf else a.dy_scale[1:]
                 self.keep.append(bb)
-                bw.append((lib.coclr_bn_bwd, (C.byref(bb), nsm)))
+                bw.append(Launch(lib.coclr_bn_bwd, (C.byref(bb), nsm)))
                 for it in convs_into[t.index]:
                     sa = acts[it.src.index]
                     geom = ops.Geometry(it.k_eff, it.s_eff, it.p_eff)
@@ -760,19 +784,20 @@ class Plan:
                                      L.dptr(dw_eff), bnp, gbf, gbf, splits, L.dptr(oscale))
                         self.keep += [wg, dy]
                         self.s2d_wgrads.append(wg)
-                        bw.append((eng._s2d_wgrad_op(it.name, wg), ()))
+                        # lane 0, where its torch zeroing and scatter run, so not wg_ws (lane 1 may be using it)
+                        bw.append(Launch(eng._s2d_wgrad_op(it.name), (C.byref(wg),)))
                     else:
                         wg = L.Wgrad(wsrc, geom.c(0), dy, B, a.dims[0], a.dims[1], a.dims[2], it.cout, it.cin,
                                      L.dptr(st.view_span([n + ".weight" for n in it.weight_names], grad=True)), bnp, gbf, gbf,
                                      splits, L.dptr(oscale))
                         self.keep += [wg, dy]
                         self.wgrads.append(wg)
-                        bw.append((lib.coclr_conv_wgrad, (C.byref(wg),)))
+                        bw.append(Launch(lib.coclr_conv_wgrad, (C.byref(wg),), 1, AFTER0))
                     if it.need_dgrad:
                         dg = ops.make_conv(dy, gbf, geom.c(1), B, sa.dims, eng.packed_bwd[it.name], sa.grad, it.src_coff,
                                            accumulate=grad_seen(sa, it.src_coff, it.src_C), npass=bnp, out_scale=oscale)
                         self.keep.append(dg)
-                        bw.append((lib.coclr_conv_igemm, (C.byref(dg), nsm)))
+                        bw.append(Launch(lib.coclr_conv_igemm, (C.byref(dg), nsm)))
             elif t.index in pool_into:
                 it = pool_into[t.index]
                 sa = acts[it.src.index]
@@ -781,23 +806,22 @@ class Plan:
                             sa.dims[0], sa.dims[1], sa.dims[2], a.dims[0], a.dims[1], a.dims[2], geom.c(0),
                             L.dptr(a.grad), L.dptr(sa.grad), int(grad_seen(sa)))
                 self.keep.append(pl)
-                bw.append((lib.coclr_maxpool_bwd, (C.byref(pl),)))
-        # one workspace for the weight-gradient launches (they run one after the other on the side stream): per-CTA
-        # partial sums are written with plain stores and reduced by a second launch instead of fp32 atomics into dW
+                bw.append(Launch(lib.coclr_maxpool_bwd, (C.byref(pl),)))
+        # one workspace for the weight-gradient launches on lane 1 (they run one after the other): per-CTA partial sums
+        # are written with plain stores and reduced by a second launch instead of fp32 atomics into dW
         need = max([int(lib.coclr_wgrad_ws_floats(C.byref(w))) for w in self.wgrads] + [0])
         self.wg_ws = None
         if need > 0:
             self.wg_ws = torch.empty(need, dtype=torch.float32, device=dev)
             for w in self.wgrads:
                 w.ws, w.ws_floats = L.dptr(self.wg_ws).value, need
-            # the space-to-depth stem's weight gradient runs on the main stream (it is followed by a scatter into the
-            # real weight layout) while the others may still be busy on the side stream: its own workspace
             for w in self.s2d_wgrads:
                 n_own = int(lib.coclr_wgrad_ws_floats(C.byref(w)))
                 if n_own > 0:
                     own = torch.empty(n_own, dtype=torch.float32, device=dev)
                     self.keep.append(own)
                     w.ws, w.ws_floats = L.dptr(own).value, n_own
+        self.bwd_kernels = _count_kernels(bw)   # a weight gradient's count depends on the workspace it was given
 
 
 class EncoderEngine:
@@ -810,6 +834,7 @@ class EncoderEngine:
             raise ValueError("precision must be one of %s" % list(PRECISIONS))
         self.store, self.graph, self.precision = store, graph, precision
         self.plans = {}
+        self.lanes = None   # the streams of lanes 1..3 (created at the first launch)
         dev = store.device
         # input of the modules' autograd nodes, so that their outputs require a gradient whatever the caller passes in
         self.anchor = torch.zeros(1, device=dev, requires_grad=True)
@@ -869,13 +894,14 @@ class EncoderEngine:
         for d in getattr(self, "s2d", {}).values():
             torch.mul(d["w"].reshape(-1)[d["idx"]], d["mask"], out=d["w_eff"].view(-1))
 
-    def _s2d_wgrad_op(self, name, wg):
+    def _s2d_wgrad_op(self, name):
+        """op(wg, stream): the weight gradient of the space-to-depth stem `name`; wg: byref of its coclr_wgrad_t."""
         d = self.s2d[name]
         lib = L.load()
 
-        def op(stream):
+        def op(wg, stream):
             d["dw_eff"].zero_()
-            rc = lib.coclr_conv_wgrad(C.byref(wg), stream)
+            rc = lib.coclr_conv_wgrad(wg, stream)
             # W' -> W is one-to-one on the valid entries (masked entries point at index 0 with a zero factor)
             d["dw"].view(-1).index_add_(0, d["idx"], d["dw_eff"].view(-1) * d["mask"])
             return rc
@@ -923,68 +949,46 @@ class EncoderEngine:
             self.plans[key] = p
         return p
 
-    def _run_lanes(self, oplist, lanes):
-        """Forward launch list with fork/join: ops tagged lane 1..3 run on side streams that wait for the fork
-        point (an event on the main stream recorded before the block's first op); the JOIN op first waits for them."""
+    def _launch(self, records, kernels):
+        """Launch a plan's Launch records and add their `kernels` to L.LAUNCHES.  Lane 0 is the current stream; before
+        a launch, its lane waits for what the record's `wait` names, and lane 0 waits for every lane still open at the
+        end.  Under `profile` every launch runs on lane 0 between two timing events."""
         main = torch.cuda.current_stream()
-        if getattr(self, "_lane_streams", None) is None:
-            self._lane_streams = [None] + [torch.cuda.Stream() for _ in range(3)]
-        ptrs = [C.c_void_p(main.cuda_stream)] + [C.c_void_p(s.cuda_stream) for s in self._lane_streams[1:]]
-        fork_ev, active = None, set()
-        for i, (fn, args) in enumerate(oplist):
-            lane, flag = lanes.get(i, (0, 0))
-            if flag == FORK:
-                fork_ev = torch.cuda.Event()
-                fork_ev.record(main)
-                active = set()
-            elif flag == JOIN:
-                for ln in active:
-                    main.wait_stream(self._lane_streams[ln])
-                active = set()
-            if lane != 0 and lane not in active:
-                self._lane_streams[lane].wait_event(fork_ev)
-                active.add(lane)
-            if flag == AFTER1:
-                (self._lane_streams[lane] if lane else main).wait_stream(self._lane_streams[1])
-            rc = fn(*args, ptrs[lane])
-            if rc != 0:
-                raise L.CoclrError("%s failed with code %d" % (fn.__name__, rc))
-        for ln in active:
-            main.wait_stream(self._lane_streams[ln])
-        L.LAUNCHES += sum(L.kernels_of(fn, args) for fn, args in oplist)
-
-    def _run(self, oplist, side_fn=None):
-        """Launch the list on the current stream. Ops whose function is `side_fn` (the weight-gradient GEMMs, which
-        nothing downstream in the list depends on) go to a side stream that waits for the producer of their inputs
-        and is joined at the end: small layers leave most SMs idle, so the two chains overlap."""
-        main = torch.cuda.current_stream()
-        stream = C.c_void_p(main.cuda_stream)
+        if self.lanes is None:
+            self.lanes = [torch.cuda.Stream() for _ in range(3)]
+        lanes = [main] + self.lanes
+        ptrs = [C.c_void_p(s.cuda_stream) for s in lanes]
         prof = EncoderEngine.profile
-        use_side = side_fn is not None and prof is None
-        if use_side:
-            if getattr(self, "_side", None) is None:
-                self._side = torch.cuda.Stream()
-            side = self._side
-            side_ptr = C.c_void_p(side.cuda_stream)
-            side_used = False
-        for fn, args in oplist:
-            if use_side and fn is side_fn:
-                side.wait_stream(main)           # inputs (dY planes) were produced by ops already queued on main
-                rc = fn(*args, side_ptr)
-                side_used = True
-            else:
-                if prof is not None:
-                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    e0.record()
-                rc = fn(*args, stream)
-                if prof is not None:
-                    e1.record()
-                    prof.append((fn.__name__, args, e0, e1))
+        fork, open_lanes = None, set()
+        for r in records:
+            lane = r.lane if prof is None else 0
+            if prof is None and r.wait is not None:
+                s = lanes[lane]
+                if r.wait == FORK:
+                    fork = torch.cuda.Event()
+                    fork.record(main)
+                if r.wait in (FORK, AT_FORK, AFTER1):
+                    s.wait_event(fork)
+                if r.wait in (AFTER1, AFTER0):
+                    s.wait_stream(lanes[1 if r.wait == AFTER1 else 0])
+                if r.wait == JOIN:
+                    for ln in open_lanes:
+                        main.wait_stream(lanes[ln])
+                    open_lanes = set()
+                else:
+                    open_lanes.add(lane)
+            if prof is not None:
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+            rc = r.fn(*r.args, ptrs[lane])
+            if prof is not None:
+                e1.record()
+                prof.append((r.fn.__name__, r.args, e0, e1))
             if rc != 0:
-                raise L.CoclrError("%s failed with code %d" % (fn.__name__, rc))
-        if use_side and side_used:
-            main.wait_stream(side)
-        L.LAUNCHES += sum(L.kernels_of(fn, args) for fn, args in oplist)
+                raise L.CoclrError("%s failed with code %d" % (r.fn.__name__, rc))
+        for ln in open_lanes:
+            main.wait_stream(lanes[ln])
+        L.LAUNCHES += kernels
 
     def forward(self, x, training=True, with_backward=False, repack=True, batch_index=None, batch=None, peers=None,
                 norm=None, replica=0):
@@ -1029,21 +1033,19 @@ class EncoderEngine:
             if training:
                 p.stats.zero_()
                 self.store.nbt += 1
-            if EncoderEngine.profile is None:
-                self._run_lanes(p.fwd, p.fwd_lane)
-            else:
-                self._run(p.fwd)
-        self._graphed(p, "fwd" + ("_repack" if repack else ""), body)
+            self._launch(p.fwd, p.fwd_kernels)
+        self._graphed(p, "fwd" + ("_repack" if repack else ""), body, p.fwd_kernels + int(repack))   # + pack_weights
         if with_backward:
             p.generation += 1
         return p
 
     use_graphs = True   # capture every launch list into a CUDA graph after its first eager run
 
-    def _graphed(self, p, key, body):
+    def _graphed(self, p, key, body, kernels):
         """Every launch of `body` has fixed pointers and shapes: after one eager run (which also performs the
         one-time cudaFuncSetAttribute calls) capture it -- stream forks/joins included -- into a CUDA graph and
-        replay that; the host then enqueues an encoder pass with one call instead of ~400."""
+        replay that; the host then enqueues an encoder pass with one call instead of ~400.  kernels: the library
+        kernels body launches, which a replay adds to L.LAUNCHES (an eager or captured run of body counts them)."""
         if not EncoderEngine.use_graphs or EncoderEngine.profile is not None:
             body()
             return
@@ -1052,15 +1054,13 @@ class EncoderEngine:
             body()
             p.graphs[key] = "warm"
         elif state == "warm":
-            g = torch.cuda.CUDAGraph()
-            before = L.LAUNCHES
+            g = p.graphs[key] = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 body()
-            p.graphs[key] = (g, L.LAUNCHES - before)
             g.replay()
         else:
-            state[0].replay()
-            L.LAUNCHES += state[1]
+            state.replay()
+            L.LAUNCHES += kernels
 
     def backward(self, p, grad, generation):
         """grad: gradient w.r.t. the pass's output -- the normalised features [B, dim] with a head, the pooled feature
@@ -1071,8 +1071,7 @@ class EncoderEngine:
             raise L.CoclrError("backward of an engine pass whose saved activations were overwritten by a later forward "
                                "of the same shape (one outstanding training forward per module and input shape)")
         (p.dq if self.graph.head_dim is not None else p.dfeat).copy_(grad)
-        wg = L.load().coclr_conv_wgrad
-        self._graphed(p, "bwd", lambda: self._run(p.bwd, side_fn=wg))
+        self._graphed(p, "bwd", lambda: self._launch(p.bwd, p.bwd_kernels), p.bwd_kernels)
 
     def backbone_output_ncdhw(self, p):
         return p.backbone_out.pl.value().permute(0, 4, 1, 2, 3).contiguous()

@@ -193,24 +193,23 @@ KERNELS_PER_CALL = {"coclr_bn_bwd": 2, "coclr_l2norm_bwd": 2, "coclr_conv_packed
                     "coclr_jpeg_decode_slots": 3}
 
 
-def kernels_of(fn, args):
-    """Kernels one call of `fn` launches (bench.py reports the per-step total).  A weight gradient on the TMA-staged
-    kernel (a shape it takes, with a large enough workspace) is two launches: partial sums, then the reduction over
-    the pixel splits."""
-    name = fn.__name__
-    if name == "coclr_conv_wgrad" and args and hasattr(args[0], "_obj"):
+def kernels_of(fn, args=()):
+    """Kernels fn(*args) launches (bench.py reports the per-step total); fn: a library function or its name.  A weight
+    gradient (args[0]: its coclr_wgrad_t) on the TMA-staged kernel (a shape it takes, with a large enough workspace) is
+    two launches: partial sums, then the reduction over the pixel splits; so is the engine's space-to-depth stem op."""
+    name = fn if isinstance(fn, str) else fn.__name__
+    if name in ("coclr_conv_wgrad", "coclr_conv_wgrad_s2d") and args:
         wg = args[0]._obj
-        need = load().coclr_wgrad_ws_floats(args[0]) if wg.ws else 0
-        if need > 0 and wg.ws_floats >= need:
+        if wg.ws and 0 < load().coclr_wgrad_ws_floats(args[0]) <= wg.ws_floats:
             return 2
     return KERNELS_PER_CALL.get(name, 1)
 
 
-def check(rc, what):
+def check(rc, what, args=()):
     global LAUNCHES
     if rc != 0:
         raise CoclrError("%s failed with code %d" % (what, rc))
-    LAUNCHES += KERNELS_PER_CALL.get(what, 1)
+    LAUNCHES += kernels_of(what, args)
 
 
 def stream_ptr():

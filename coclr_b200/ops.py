@@ -117,5 +117,5 @@ def conv_wgrad(src, src_bf16, geom_c, dy_src, dy_bf16, B, dst_dims, Cout, Cin_re
         workspace = torch.empty(max(need, 4), dtype=torch.float32, device=dw.device)
     if workspace is not None:
         p.ws, p.ws_floats = L.dptr(workspace).value, workspace.numel()
-    L.check(L.load().coclr_conv_wgrad(C.byref(p), L.stream_ptr()), "coclr_conv_wgrad")
+    L.check(L.load().coclr_conv_wgrad(C.byref(p), L.stream_ptr()), "coclr_conv_wgrad", (C.byref(p),))
     return workspace

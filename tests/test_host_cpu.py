@@ -489,5 +489,8 @@ def test_weight_gradient_workspaces_dry_run():
         # launch accounting: a weight gradient with a workspace is two kernels
         wl = [(fn, a) for fn, a in p.bwd if fn.__name__ == "coclr_conv_wgrad"]
         assert sum(L.kernels_of(fn, a) for fn, a in wl) == len(wl) + sum(1 for n in need if n > 0)
+        # the plan records each launch's count; the space-to-depth stem's launch has a workspace too: two kernels
+        assert all(r.kernels == L.kernels_of(r.fn, r.args) for r in p.bwd)
+        assert [r.kernels for r in p.bwd if r.fn.__name__ == "coclr_conv_wgrad_s2d"] == [2]
     finally:
         L.DRY_RUN = False
