@@ -63,6 +63,16 @@ EXPORTS = {
     "coclr_jpeg_work_bytes": (C.c_size_t, [P]),
     "coclr_jpeg_decode": (I, [P, P]),
     "coclr_jpeg_decode_slots": (I, [P, P, P]),
+    "coclr_tvl1_scales": (I, [I, I]),
+    "coclr_tvl1_work_bytes": (C.c_size_t, [I, I, I]),
+    "coclr_tvl1": (I, [P, P]),
+    "coclr_flow_grey": (I, [P, I, I, I, C.c_int64, C.c_int64, P, P]),
+    "coclr_flow_quantise": (I, [P, I, I, I, P, P]),
+    "coclr_flow_zoom_out": (I, [P, I, I, I, P, P, I, I, P]),
+    "coclr_flow_zoom_in": (I, [P, I, I, I, P, I, I, P]),
+    "coclr_flow_warp": (I, [P, P, P, I, I, I, P, P]),
+    "coclr_flow_iterate_work_bytes": (C.c_size_t, [I, I, I]),
+    "coclr_flow_iterate": (I, [P, P, P, I, I, I, I, P, P, P]),
 }
 
 

@@ -682,6 +682,66 @@ typedef struct {
 } coclr_jpeg_slots_t;
 int coclr_jpeg_decode_slots(const coclr_jpeg_t* p, const coclr_jpeg_slots_t* s, coclr_stream_t stream);
 
+/* TV-L1 optical flow, batched over P frame pairs of one size H x W: the duality-based TV-L1 of Zach, Pock and
+ * Bischof as Sanchez Perez, Meinhardt-Llopis and Facciolo give it (IPOL 2013), with fixed parameters: a pyramid of
+ * zoom factor 0.5 (at most COCLR_TVL1_MAX_SCALES levels, the coarsest short side >= 16; one level down is a separable
+ * Gaussian of sigma 0.6 sqrt(3), radius 4, clamp-to-edge, then bicubic sampling), Keys bicubic (a = -0.5) with
+ * clamped neighbours for the pyramid, the flow upsampling and the warp, COCLR_TVL1_WARPS warps per scale, and per
+ * warp primal-dual iterations (lambda 0.15, theta 0.3, tau 0.25) until the pair's mean |u' - u|^2 <= 0.01^2 or
+ * COCLR_TVL1_MAX_ITERS.
+ *
+ * Convergence is per pair: each pair's error is summed in a fixed order (per-CTA partials, then a second pass), and a
+ * converged pair is frozen on the device, so a pair's flow and iteration counts are bit-identical whether it is
+ * solved alone or in any batch.  Each iteration is two kernels over the whole batch; the host reads the flags back
+ * every COCLR_TVL1_CHECK_EVERY iterations and stops the warp when every pair has converged.
+ *
+ * i0, i1: device [P, H, W] grey frames (0..255); flow: device [P, 2, H, W] (u1 horizontal, u2 vertical, in pixels,
+ * I1(x + u) ~ I0(x)); iterations: device int [P, scales, COCLR_TVL1_WARPS]; work: device, 256-byte aligned, at least
+ * coclr_tvl1_work_bytes.  coclr_tvl1_scales gives the pyramid's level count for H x W.  P is at most
+ * COCLR_FLOW_MAX_BATCH; a larger batch is solved as consecutive calls, with the same result. */
+#define COCLR_FLOW_MAX_BATCH 65535  /* pairs (frames for grey) per call of every coclr_flow_* / coclr_tvl1 function */
+#define COCLR_TVL1_MAX_SCALES 5
+#define COCLR_TVL1_WARPS 5
+#define COCLR_TVL1_MAX_ITERS 300
+#define COCLR_TVL1_CHECK_EVERY 10
+typedef struct {
+  int P, H, W;
+  const float* i0;
+  const float* i1;
+  float* flow;
+  int* iterations;
+  void* work;
+  size_t work_bytes;
+} coclr_tvl1_t;
+int coclr_tvl1_scales(int H, int W);
+size_t coclr_tvl1_work_bytes(int P, int H, int W);
+int coclr_tvl1(const coclr_tvl1_t* t, coclr_stream_t stream);
+
+/* Flow frames.  coclr_flow_grey: uint8 RGB frames (frame n, row y, pixel x at rgb[n * frame_stride + y * row_stride
+ * + 3 x]) to float [N, H, W], Pillow's convert('L'): (19595 R + 38470 G + 7471 B + 0x8000) >> 16.
+ * coclr_flow_quantise: flow [P, 2, H, W] to uint8 [P, H, W, 3], R = q(u1), G = q(u2), B = q(0) = 128 with
+ * q(f) = clamp(floor((f + COCLR_FLOW_BOUND) * 255 / (2 COCLR_FLOW_BOUND) + 0.5), 0, 255) in float32 without
+ * contraction. */
+#define COCLR_FLOW_BOUND 20.0f
+int coclr_flow_grey(const uint8_t* rgb, int N, int H, int W, int64_t frame_stride, int64_t row_stride, float* out,
+                    coclr_stream_t stream);
+int coclr_flow_quantise(const float* flow, int P, int H, int W, uint8_t* out, coclr_stream_t stream);
+
+/* The solver's stages, for testing them one by one.  zoom_out: one pyramid level down, [P, H, W] to [P, Hc, Wc]
+ * (tmp: 2 P H W floats).  zoom_in: coarse flow [P, 2, Hc, Wc] to [P, 2, H, W], u1 scaled by W / Wc and u2 by H / Hc.
+ * warp: out [6, P, H, W] = centred gradients I1x, I1y of i1, then I1x and I1y warped at x + flow, g and rho_c.
+ * iterate: n primal-dual iterations from the warp's planes, updating flow [P, 2, H, W] and dual [P, 4, H, W] (p11,
+ * p12, p21, p22) in place with the convergence test and freezing of the solver; iters: int [P] iterations run;
+ * work: coclr_flow_iterate_work_bytes. */
+int coclr_flow_zoom_out(const float* in, int P, int H, int W, float* tmp, float* out, int Hc, int Wc,
+                        coclr_stream_t stream);
+int coclr_flow_zoom_in(const float* flow, int P, int Hc, int Wc, float* out, int H, int W, coclr_stream_t stream);
+int coclr_flow_warp(const float* i0, const float* i1, const float* flow, int P, int H, int W, float* out,
+                    coclr_stream_t stream);
+size_t coclr_flow_iterate_work_bytes(int P, int H, int W);
+int coclr_flow_iterate(const float* warped, float* flow, float* dual, int P, int H, int W, int n, int* iters,
+                       void* work, coclr_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
