@@ -25,6 +25,7 @@ EXPORTS = {
     "coclr_bias_relu_bwd": (I, [P, P, P, P, I, I, P]),
     "coclr_maxpool_fwd": (I, [P, P]),
     "coclr_maxpool_bwd": (I, [P, P]),
+    "coclr_maxpool_bwd_path": (I, [P]),
     "coclr_avgpool_fwd": (I, [P, P, I, I, I, P, I, I, I, P]),
     "coclr_avgpool_bwd": (I, [P, P, I, I, I, I, I, P]),
     "coclr_pack_input": (I, [P, LG, LG, I, P, P, P, P, I, LG, P, P, I, P, P, P]),

@@ -908,11 +908,11 @@ __global__ void __launch_bounds__(256) maxpool_bwd_scatter_kernel(const coclr_po
   }
 }
 
-// gather form of the backward: dX[in] (+)= sum over windows whose arg-max is `in` of dY[out]
-template <int KT, int KH, int KW, int ST, int SH, int SW>
+// gather form of the backward: dX[in] (+)= sum over windows whose arg-max is `in` of dY[out], added in ascending tap
+// order starting from +0.0, the old dX last (the staged kernel below keeps this order, so both give the same bits)
 __global__ void __launch_bounds__(256) maxpool_bwd_kernel(const coclr_pool_t P) {
-  const int kt = KT ? KT : P.g.kt, kh = KH ? KH : P.g.kh, kw = KW ? KW : P.g.kw;
-  const int st = ST ? ST : P.g.st, sh = SH ? SH : P.g.sh, sw = SW ? SW : P.g.sw;
+  const int kt = P.g.kt, kh = P.g.kh, kw = P.g.kw;
+  const int st = P.g.st, sh = P.g.sh, sw = P.g.sw;
   const int C4 = P.C >> 2;
   const long total = (long)P.B * P.Ti * P.Hi * P.Wi * C4;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -961,6 +961,132 @@ __global__ void __launch_bounds__(256) maxpool_bwd_kernel(const coclr_pool_t P) 
       acc.x += old.x; acc.y += old.y; acc.z += old.z; acc.w += old.w;
     }
     st4(dp, acc);
+  }
+}
+
+// floor and ceiling of a / s for s > 0 and a of either sign
+__host__ __device__ __forceinline__ int floordiv(int a, int s) { return a >= 0 ? a / s : -((s - 1 - a) / s); }
+__host__ __device__ __forceinline__ int ceildiv(int a, int s) { return -floordiv(-a, s); }
+
+// Tile of the staged backward: a CTA owns `ty` input rows (2 threads per input pixel, at most 256 threads); each frame of
+// its ring holds `rows` x `cols` output pixels (the windows of those rows, halo included, starting at output column
+// `ox0`), 16 channels of dY (64 B) then 16 of idx (16 B) per pixel; the ring holds the output frames one input frame
+// reads plus the one in flight.
+struct PoolBwdTile {
+  int ty, rows, cols, ox0, ring;
+  __host__ __device__ uint32_t frame_bytes() const { return (uint32_t)(rows * cols) * 80u; }
+};
+template <int KT, int KH, int KW, int ST, int SH, int SW>
+__host__ __device__ __forceinline__ PoolBwdTile pool_bwd_tile(const coclr_pool_t& P) {
+  PoolBwdTile t;
+  t.ty = P.Hi < 128 / P.Wi ? P.Hi : 128 / P.Wi;
+  t.rows = (t.ty + KH - 2) / SH + 1;
+  t.ox0 = ceildiv(P.g.pw - KW + 1, SW);
+  t.cols = floordiv(P.Wi - 1 + P.g.pw, SW) - t.ox0 + 1;
+  t.ring = (KT - 1) / ST + 2;
+  return t;
+}
+
+// Gather form of the backward through shared memory, for the overlapping windows of S3D: (3,3,3)/1/1 (the Inception
+// branch-3 pools), (1,3,3)/(1,2,2)/(0,1,1) (MaxPool_2a, MaxPool_3a, the ResNet stem pool) and (3,3,3)/2/1 (MaxPool_4a).
+// A CTA owns (clip, a band of input rows, all columns, 16 channels) and walks along t.  The dY and idx tiles of the
+// output pixels whose windows cover the band are staged once per output frame with 16-byte cp.async copies into a ring,
+// the next frame in flight while the current input frame is reduced (the grid-stride kernel above re-reads every window's
+// idx through L1/L2, 27 per input pixel for 3x3x3/s1, in 16-byte requests at most).  A staged pixel outside the output
+// keeps idx 255, which no tap equals (coclr_maxpool_fwd refuses windows of more than 255 taps), so no tap needs a bounds
+// test.  A thread produces 8 channels of one input pixel with maxpool_bwd_kernel's sums: +0.0, the matching windows' dY
+// in ascending tap order (a, then bb, then cc), the old dX last -- so dX is the same bit for bit.
+template <int KT, int KH, int KW, int ST, int SH, int SW>
+__global__ void __launch_bounds__(256) maxpool_bwd_smem_kernel(const coclr_pool_t P) {
+  extern __shared__ __align__(16) uint8_t pool_smem[];
+  const PoolBwdTile tl = pool_bwd_tile<KT, KH, KW, ST, SH, SW>(P);
+  const int W = P.Wi, H = P.Hi, To = P.To, Ho = P.Ho, Wo = P.Wo;
+  const int pt = P.g.pt, ph = P.g.ph, pw = P.g.pw;
+  const int ytiles = (H + tl.ty - 1) / tl.ty;
+  const int cslices = P.C >> 4;
+  int blk = blockIdx.x;
+  const int cs = blk % cslices; blk /= cslices;
+  const int yt = blk % ytiles;
+  const int b = blk / ytiles;
+  const int c0 = cs * 16, yi0 = yt * tl.ty;
+  const int yi_end = yi0 + tl.ty < H ? yi0 + tl.ty : H;
+  const int oy0 = ceildiv(yi0 + ph - KH + 1, SH);                     // first staged output row
+  const int npx = (floordiv(yi_end - 1 + ph, SH) - oy0 + 1) * tl.cols;  // staged pixels per frame
+  const uint32_t fbytes = tl.frame_bytes();
+  const uint32_t idx_off = (uint32_t)(tl.rows * tl.cols) * 64u;         // idx after dY in a frame
+  const int tid = threadIdx.x;
+  const int cq = tid & 1, x = (tid >> 1) % W, y = yi0 + (tid >> 1) / W;  // blockDim = 2 * W * ty
+  const uint32_t sbase = smem_u32(pool_smem);
+  for (uint32_t i = tid; i < (uint32_t)(tl.ring * tl.rows * tl.cols); i += blockDim.x) {
+    const uint32_t f = i / (uint32_t)(tl.rows * tl.cols), px = i % (uint32_t)(tl.rows * tl.cols);
+    *reinterpret_cast<uint4*>(pool_smem + f * fbytes + idx_off + px * 16u) =
+        make_uint4(0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu);
+  }
+  __syncthreads();
+  auto issue_frame = [&](int to) {    // output frame `to` into ring slot to % ring (pixels inside the output only)
+    const uint32_t slot = sbase + (uint32_t)(to % tl.ring) * fbytes;
+    for (int i = tid; i < npx * 5; i += blockDim.x) {
+      const int part = i % 5, px = i / 5;           // 4 x 16 B of dY, then 16 B of idx
+      const int ry = px / tl.cols;
+      const int yo = oy0 + ry, xo = tl.ox0 + px - ry * tl.cols;
+      if ((unsigned)yo >= (unsigned)Ho || (unsigned)xo >= (unsigned)Wo) continue;
+      const size_t o = ((((size_t)b * To + to) * Ho + yo) * Wo + xo) * P.C + c0;
+      if (part < 4) cp_async16(slot + (uint32_t)px * 64u + part * 16u, P.dy + o + part * 4, 16u);
+      else cp_async16(slot + idx_off + (uint32_t)px * 16u, P.idx + o, 16u);
+    }
+    cp_async_commit();
+  };
+  const bool active = y < yi_end;
+  int issued = 0;
+  for (int ti = 0; ti < P.Ti; ++ti) {
+    // the last output frame whose windows reach input frame ti; the one after it is prefetched
+    const int hi = floordiv(ti + pt, ST) < To - 1 ? floordiv(ti + pt, ST) : To - 1;
+    while (issued <= hi + 1 && issued < To) issue_frame(issued++);
+    float* dp = P.dx + ((((size_t)b * P.Ti + ti) * H + y) * W + x) * P.ldx + P.x_coff + c0 + cq * 8;
+    float4 old0 = make_float4(0.f, 0.f, 0.f, 0.f), old1 = old0;
+    if (active && P.accumulate) { old0 = ld4(dp); old1 = ld4(dp + 4); }    // in flight while the tiles land
+    if (issued - 1 > hi) cp_async_wait<1>(); else cp_async_wait<0>();
+    __syncthreads();
+    if (active) {
+      float acc[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) acc[k] = 0.f;
+#pragma unroll
+      for (int a = 0; a < KT; ++a) {
+        const int tn = ti + pt - a;
+        if (tn < 0 || tn % ST != 0 || tn / ST >= To) continue;
+        const uint8_t* slot = pool_smem + (size_t)((tn / ST) % tl.ring) * fbytes;
+#pragma unroll
+        for (int bb = 0; bb < KH; ++bb) {
+          const int yn = y + ph - bb;
+          if (yn % SH != 0) continue;
+          const int ry = yn / SH - oy0;
+#pragma unroll
+          for (int cc = 0; cc < KW; ++cc) {
+            const int xn = x + pw - cc;
+            if (xn % SW != 0) continue;
+            const uint32_t px = (uint32_t)(ry * tl.cols + xn / SW - tl.ox0);
+            const uint2 id = *reinterpret_cast<const uint2*>(slot + idx_off + px * 16u + cq * 8);
+            const uint32_t tap4 = 0x01010101u * (uint32_t)((a * KH + bb) * KW + cc);
+            const uint32_t m0 = __vcmpeq4(id.x, tap4), m1 = __vcmpeq4(id.y, tap4);   // 0xff per matching channel
+            if ((m0 | m1) == 0u) continue;
+            const float4 d0 = *reinterpret_cast<const float4*>(slot + px * 64u + cq * 32);
+            const float4 d1 = *reinterpret_cast<const float4*>(slot + px * 64u + cq * 32 + 16);
+            const float dv[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
+#pragma unroll
+            for (int k = 0; k < 8; ++k)
+              if (((k < 4 ? m0 : m1) >> (8 * (k & 3))) & 1u) acc[k] += dv[k];
+          }
+        }
+      }
+      if (P.accumulate) {
+        acc[0] += old0.x; acc[1] += old0.y; acc[2] += old0.z; acc[3] += old0.w;
+        acc[4] += old1.x; acc[5] += old1.y; acc[6] += old1.z; acc[7] += old1.w;
+      }
+      st4(dp, make_float4(acc[0], acc[1], acc[2], acc[3]));
+      st4(dp + 4, make_float4(acc[4], acc[5], acc[6], acc[7]));
+    }
+    __syncthreads();     // everyone is done with the ring before the next frame's copies land in it
   }
 }
 
@@ -1283,20 +1409,47 @@ extern "C" int coclr_bias_relu_bwd(const float* h, const float* bias, float* dA,
   return LAUNCH_OK();
 }
 
-static void launch_pool_bwd(const coclr_pool_t& p, long total, cudaStream_t s) {
-  const int grid = grid_for(total, 256, 148 * 32);
+// The staged backward takes window (KT,KH,KW)/(ST,SH,SW) when its conditions hold: whole 16-channel slices, dX rows
+// aligned for 16-byte stores, at most 256 threads (2 per input pixel of a band of rows), a ring that fits in shared
+// memory.  Returns the ring's bytes, or 0 when the staged kernel does not take the call.
+template <int KT, int KH, int KW, int ST, int SH, int SW>
+static size_t pool_bwd_smem_bytes(const coclr_pool_t& p) {
   const coclr_geom_t& g = p.g;
-#define POOL_CASE(KT, KH, KW, ST, SH, SW)                                                 \
-  if (g.kt == KT && g.kh == KH && g.kw == KW && g.st == ST && g.sh == SH && g.sw == SW) { \
-    maxpool_bwd_kernel<KT, KH, KW, ST, SH, SW><<<grid, 256, 0, s>>>(p);                   \
-    return;                                                                               \
+  if (g.kt != KT || g.kh != KH || g.kw != KW || g.st != ST || g.sh != SH || g.sw != SW) return 0;
+  if (2 * g.pt > KT || 2 * g.ph > KH || 2 * g.pw > KW) return 0;
+  if (p.C % 16 || p.ldx % 8 || p.x_coff % 8 || p.Wi > 128) return 0;
+  const PoolBwdTile t = pool_bwd_tile<KT, KH, KW, ST, SH, SW>(p);
+  const size_t smem = (size_t)t.ring * t.frame_bytes();
+  return smem <= 227 * 1024 ? smem : 0;
+}
+
+template <int KT, int KH, int KW, int ST, int SH, int SW>
+static bool launch_pool_bwd_smem(const coclr_pool_t& p, cudaStream_t s) {
+  const size_t smem = pool_bwd_smem_bytes<KT, KH, KW, ST, SH, SW>(p);
+  if (smem == 0) return false;
+  // set on every call: the attribute belongs to the current device, and a process may drive more than one
+  auto kernel = maxpool_bwd_smem_kernel<KT, KH, KW, ST, SH, SW>;
+  if (smem > 48 * 1024 && cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+    cudaGetLastError();   // clear it: the grid-stride kernel takes the call instead
+    return false;
   }
-  POOL_CASE(1, 3, 3, 1, 2, 2)
-  POOL_CASE(3, 3, 3, 1, 1, 1)
-  POOL_CASE(3, 3, 3, 2, 2, 2)
-  POOL_CASE(2, 2, 2, 2, 2, 2)
-#undef POOL_CASE
-  maxpool_bwd_kernel<0, 0, 0, 0, 0, 0><<<grid, 256, 0, s>>>(p);
+  const PoolBwdTile t = pool_bwd_tile<KT, KH, KW, ST, SH, SW>(p);
+  const int grid = p.B * ((p.Hi + t.ty - 1) / t.ty) * (p.C / 16);
+  kernel<<<grid, 2 * p.Wi * t.ty, smem, s>>>(p);
+  return true;
+}
+
+// which form of the backward coclr_maxpool_bwd runs (coclr_maxpool_bwd_path)
+enum { kPoolBwdScatter = 0, kPoolBwdGather = 1, kPoolBwdStaged = 2 };
+static int pool_bwd_path(const coclr_pool_t& p) {
+  // scatter form (one add per input element) for disjoint windows and memset-able or accumulated destinations
+  const coclr_geom_t& g = p.g;
+  const bool disjoint = g.st >= g.kt && g.sh >= g.kh && g.sw >= g.kw;
+  if (disjoint && (p.accumulate || (p.ldx == p.C && p.x_coff == 0))) return kPoolBwdScatter;
+  if (pool_bwd_smem_bytes<3, 3, 3, 1, 1, 1>(p) || pool_bwd_smem_bytes<1, 3, 3, 1, 2, 2>(p) ||
+      pool_bwd_smem_bytes<3, 3, 3, 2, 2, 2>(p))
+    return kPoolBwdStaged;
+  return kPoolBwdGather;
 }
 
 // Windows the conv-output form (P.y) is instantiated for: the stage pools of S3D and the ResNet stem pool,
@@ -1362,13 +1515,15 @@ extern "C" int coclr_maxpool_fwd(const coclr_pool_t* p, coclr_stream_t stream) {
   }
   return LAUNCH_OK();
 }
+extern "C" int coclr_maxpool_bwd_path(const coclr_pool_t* p) {
+  if (!p) return COCLR_E_ARG;
+  return pool_bwd_path(*p);
+}
 extern "C" int coclr_maxpool_bwd(const coclr_pool_t* p, coclr_stream_t stream) {
   if (!p || !p->dx || !p->dy || !p->idx || p->C % 4) return COCLR_E_ARG;
-  // scatter form (one add per input element) for disjoint windows and memset-able or accumulated destinations
-  const coclr_geom_t& g = p->g;
-  const bool disjoint = g.st >= g.kt && g.sh >= g.kh && g.sw >= g.kw;
-  if (disjoint && (p->accumulate || (p->ldx == p->C && p->x_coff == 0))) {
-    cudaStream_t s = (cudaStream_t)stream;
+  cudaStream_t s = (cudaStream_t)stream;
+  const int path = pool_bwd_path(*p);
+  if (path == kPoolBwdScatter) {
     if (!p->accumulate) {
       const size_t bytes = (size_t)p->B * p->Ti * p->Hi * p->Wi * p->C * sizeof(float);
       if (cudaMemsetAsync(p->dx, 0, bytes, s) != cudaSuccess) return COCLR_E_LAUNCH;
@@ -1377,8 +1532,12 @@ extern "C" int coclr_maxpool_bwd(const coclr_pool_t* p, coclr_stream_t stream) {
     maxpool_bwd_scatter_kernel<<<grid_for(tot_o, 256, 148 * 32), 256, 0, s>>>(*p);
     return LAUNCH_OK();
   }
+  if (path == kPoolBwdStaged && (launch_pool_bwd_smem<3, 3, 3, 1, 1, 1>(*p, s) ||
+                                 launch_pool_bwd_smem<1, 3, 3, 1, 2, 2>(*p, s) ||
+                                 launch_pool_bwd_smem<3, 3, 3, 2, 2, 2>(*p, s)))
+    return LAUNCH_OK();
   const long total = (long)p->B * p->Ti * p->Hi * p->Wi * (p->C / 4);
-  launch_pool_bwd(*p, total, (cudaStream_t)stream);
+  maxpool_bwd_kernel<<<grid_for(total, 256, 148 * 32), 256, 0, s>>>(*p);
   return LAUNCH_OK();
 }
 

@@ -262,6 +262,9 @@ typedef struct {
 } coclr_pool_t;
 int coclr_maxpool_fwd(const coclr_pool_t* p, coclr_stream_t stream);
 int coclr_maxpool_bwd(const coclr_pool_t* p, coclr_stream_t stream);
+/* which form coclr_maxpool_bwd takes for *p (host only, launches nothing): 0 the scatter form (disjoint windows),
+ * 1 the grid-stride gather, 2 the shared-memory staged gather */
+int coclr_maxpool_bwd_path(const coclr_pool_t* p);
 
 /* ---- nn.AdaptiveAvgPool3d((1,1,1)) (model/pretrain.py:51) ---------------------------------------- */
 int coclr_avgpool_fwd(const void* x_hi, const void* x_lo, int bf16 /* plane format */, int ld, int coff, float* out, int B, int Pn, int C,
