@@ -729,14 +729,7 @@ static int launch_conv(const coclr_conv_t& P, int num_sms, cudaStream_t s) {
   O.BN = P.BN;
   O.N = P.N;
   O.stage_bufs = (int)L.stage_bufs;
-  const uint64_t row_bytes = (uint64_t)P.dst_ld * 4u;
-  MapSpec ms;
-  memset(&ms, 0, sizeof(ms));
-  ms.base[0] = P.dst + P.dst_coff;
-  ms.elem_bytes = 4;
-  ms.dims[0] = (uint64_t)P.N; ms.dims[1] = (uint64_t)M; ms.dims[2] = ms.dims[3] = ms.dims[4] = 1;
-  ms.strides[0] = row_bytes; ms.strides[1] = ms.strides[2] = ms.strides[3] = row_bytes * (uint64_t)M;
-  ms.box[0] = 32; ms.box[1] = 32; ms.box[2] = ms.box[3] = ms.box[4] = 1;
+  const MapSpec ms = plane_map(P.dst, nullptr, P.dst_coff, 4, P.dst_ld, P.N, O.oext, {32, 32, 1, 1, 1});
   if (ms.strides[1] >= (1ull << 40)) return COCLR_E_ARG;   // tensor-map stride limit
   CUtensorMap m_out;
   if (!encode_map(&m_out, ms, 0, 5, /*swizzle=*/true)) return COCLR_E_LAUNCH;

@@ -291,8 +291,110 @@ bool encode_map(CUtensorMap* m, const MapSpec& s, int which, int rank, bool swiz
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-static int ceil_div(int a, int b) { return (a + b - 1) / b; }
-static int pymod(int a, int b) { return ((a % b) + b) % b; }
+bool encode_maps(CUtensorMap* hi, CUtensorMap* lo, const MapSpec& s, int npass) {
+  if (!encode_map(hi, s, 0)) return false;
+  if (npass > 1) return encode_map(lo, s, 1);
+  *lo = *hi;
+  return true;
+}
+
+MapSpec plane_map(const void* hi, const void* lo, int coff, int elem_bytes, int ld, int c, const int (&ext)[4],
+                  const int (&box)[5], int pitch) {
+  MapSpec m;
+  m.base[0] = (void*)((const char*)hi + (long)coff * elem_bytes);
+  m.base[1] = lo ? (void*)((const char*)lo + (long)coff * elem_bytes) : nullptr;
+  m.elem_bytes = elem_bytes;
+  m.dims[0] = (uint64_t)c;
+  uint64_t stride = (uint64_t)ld * (uint64_t)elem_bytes;
+  for (int d = 0; d < 4; ++d) {
+    m.dims[1 + d] = (uint64_t)ext[d];
+    m.strides[d] = stride;
+    stride *= (uint64_t)(d == 0 && pitch > 0 ? pitch : ext[d]);
+  }
+  for (int d = 0; d < 5; ++d) m.box[d] = (uint32_t)box[d];
+  return m;
+}
+
+SlabKind slab_kind(const coclr_geom_t& g, const coclr_src_t& S, int Td, int Hd, int Wd) {
+  if (g.sh != 1 || g.sw != 1) return kSlabNone;
+  if (g.kt == 1 && g.kh == 1 && g.kw == 1) return g.st == 1 ? kSlabFlat : kSlabNone;
+  // The space-to-depth stem: the kw taps of one kernel row are kw CONSECUTIVE pixels of 64/kw channels each, i.e. one
+  // contiguous 128-byte run -- a tensor map whose pixel stride is smaller than its 64-element inner extent (overlapping
+  // rows) turns that run into one K chunk.  Needs the horizontal zero padding materialised in memory (source rows are
+  // W + kw - 1 .. pixels wide, pw == 0) because a window straddles the row edge.
+  if (g.kt == 1 && g.kw > 1 && S.C * g.kw == 64 && S.ld == S.C && S.coff == 0 && g.pw == 0 && !g.transposed &&
+      g.st == 1 && S.W >= Wd + g.kw - 1 && S.H == Hd && S.T == Td)
+    return kSlabWindow;
+  if (g.kt == 1) return g.st == 1 ? kSlabRows : kSlabNone;
+  if (g.kh == 1 && g.kw == 1) return g.st == 1 ? kSlabFrames : (g.st == 2 ? kSlabParity : kSlabNone);
+  return kSlabNone;
+}
+
+int slab_types(SlabKind kind, const coclr_geom_t& g, TmaSlabType (&type)[4]) {
+  memset(type, 0, sizeof(type));
+  int n = 1;
+  if (kind == kSlabFlat) {
+    type[0].nshift = 1;
+  } else if (kind == kSlabWindow || kind == kSlabRows) {
+    // the window's K chunk ya is the kw taps of kernel row ya; else one type per dx, shifts dy
+    n = kind == kSlabRows ? g.kw : 1;
+    for (int xa = 0; xa < n; ++xa) {
+      TmaSlabType& t = type[xa];
+      t.d[0] = xa - g.pw;
+      t.d[1] = -g.ph;
+      t.nshift = g.kh;
+      for (int j = 0; j < g.kh; ++j) t.tap[j] = kind == kSlabRows ? j * g.kw + xa : j;
+    }
+  } else if (kind == kSlabFrames) {
+    type[0].d[2] = -g.pt;
+    type[0].nshift = g.kt;
+    for (int j = 0; j < g.kt; ++j) type[0].tap[j] = j;
+  } else if (kind == kSlabParity) {
+    // input frame 2 t' - pt + dt = 2 (t' + sh) + par: the taps of one parity are consecutive shifts of its frame plane
+    n = 2;
+    for (int par = 0; par < 2; ++par) {
+      TmaSlabType& t = type[par];
+      for (int dt = 0; dt < g.kt; ++dt) {
+        if (pymod(dt - g.pt, 2) != par) continue;
+        if (t.nshift == 0) t.d[2] = (dt - g.pt - par) / 2;   // exact
+        t.tap[t.nshift++] = dt;
+      }
+      t.d[1] = par;
+      if (t.nshift == 0) return 0;
+    }
+  } else {
+    return 0;
+  }
+  if (g.transposed) {
+    // data gradient: the destination pixel reads the source at -offset, so a slab starts at the mirror of the forward
+    // slab's last shift and its taps come in reverse order; the frame parity is the tile's (an output coordinate)
+    const int reuse_dim = kind == kSlabRows ? 1 : 2;
+    for (int i = 0; i < n; ++i) {
+      TmaSlabType& t = type[i];
+      for (int d = 0; d < 4; ++d) t.d[d] = -t.d[d];
+      t.d[reuse_dim] -= t.nshift - 1;
+      if (kind == kSlabParity) t.d[1] = 0;
+      for (int j = 0; j < t.nshift / 2; ++j) {
+        const int tap = t.tap[j];
+        t.tap[j] = t.tap[t.nshift - 1 - j];
+        t.tap[t.nshift - 1 - j] = tap;
+      }
+    }
+  }
+  return n;
+}
+
+MapSpec slab_map(SlabKind kind, const coclr_geom_t& g, const coclr_src_t& S, int B, int Wd, const int (&tile)[4],
+                 int reuse) {
+  int box[5] = {64, tile[0], tile[1], tile[2], tile[3]};
+  box[kind == kSlabWindow || kind == kSlabRows ? 2 : 3] += reuse - 1;
+  const int HW = S.H * S.W;
+  if (kind == kSlabFlat) return plane_map(S.hi, S.lo, S.coff, 2, S.ld, S.C, {(int)((long)B * S.T * HW), 1, 1, 1}, box);
+  if (kind == kSlabWindow) return plane_map(S.hi, S.lo, S.coff, 2, S.ld, 64, {Wd, S.H, S.T, B}, box, S.W);
+  if (kind == kSlabRows) return plane_map(S.hi, S.lo, S.coff, 2, S.ld, S.C, {S.W, S.H, S.T, B}, box);
+  if (kind == kSlabParity && !g.transposed) return plane_map(S.hi, S.lo, S.coff, 2, S.ld, S.C, {HW, 2, S.T / 2, B}, box);
+  return plane_map(S.hi, S.lo, S.coff, 2, S.ld, S.C, {HW, 1, S.T, B}, box);
+}
 
 // Fills the plan and the two map specs; returns false when this launch shape stays on the cp.async kernel.
 static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L, MapSpec& A, MapSpec& O) {
@@ -300,202 +402,75 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
   const coclr_src_t& S = P.src;
   memset(&L, 0, sizeof(L));
   if (P.npass != 1 && P.npass != 3) return false;
+  const SlabKind kind = slab_kind(g, S, P.Td, P.Hd, P.Wd);
+  const bool window = kind == kSlabWindow;
   const int taps = g.kt * g.kh * g.kw;
   // K = tap * C + channel is cut into 64-wide chunks: chunks must not straddle taps (single-tap convs may end with a
-  // partial chunk: the TMA unit zero-fills channels past C and the packed weights are zero past Kreal)
-  // window kind (space-to-depth stem): the kw taps of one kernel row are kw CONSECUTIVE pixels of 64/kw channels each,
-  // i.e. one contiguous 128-byte run -- a tensor map whose pixel stride is smaller than its 64-element inner extent
-  // (overlapping rows) turns that run into one K chunk.  Needs the horizontal zero padding materialised in memory
-  // (source rows are W + kw - 1 .. pixels wide, pw == 0) because a window straddles the row edge.
-  const bool window = g.kt == 1 && g.kw > 1 && S.C * g.kw == 64 && S.ld == S.C && S.coff == 0 && g.pw == 0 &&
-                      !g.transposed && g.st == 1 && S.W >= P.Wd + g.kw - 1 && S.H == P.Hd && S.T == P.Td;
+  // partial chunk: the TMA unit zero-fills channels past C and the packed weights are zero past Kreal); a window
+  // chunk is the kw taps of one kernel row
   if (S.C % 8 != 0 || (taps > 1 && S.C % 64 != 0 && !window)) return false;
   if (P.BN % 32 != 0 || P.BN < 32 || P.BN > kTmaMaxBN || P.n_tiles < 1) return false;
-  if (P.Kreal != g.kt * g.kh * g.kw * S.C) return false;
-  if (g.sh != 1 || g.sw != 1) return false;
+  if (P.Kreal != taps * S.C) return false;
   const int planes = P.npass > 1 ? 2 : 1;
-  const long ld2 = (long)S.ld * 2;
   L.out.BN = P.BN;
   L.out.N = P.N;
   L.out.n_tiles_n = P.n_tiles;
   L.nc = window ? 1 : (S.C + 63) / 64;
   L.nkc = window ? g.kh : taps * L.nc;
   L.sel_dim = -1;
-  L.a_c0_step = 64;
-  A.elem_bytes = 2;
-  A.base[0] = (void*)((const uint16_t*)S.hi + S.coff);
-  A.base[1] = S.lo ? (void*)((const uint16_t*)S.lo + S.coff) : nullptr;
-  O.elem_bytes = 4;
-  O.base[0] = (void*)(P.dst + P.dst_coff);
-  O.base[1] = nullptr;
-  const long old4 = (long)P.dst_ld * 4;
+  L.a_c0_step = window ? 0 : 64;
   int box[4] = {1, 1, 1, 1};     // tile extent per logical dim
   for (int d = 0; d < 4; ++d) L.ntiles[d] = 1;
+  int* oext = L.out.oext;
   const bool tr = g.transposed != 0;
+  const bool same = S.T == P.Td && S.H == P.Hd && S.W == P.Wd;
 
-  if (g.kt == 1 && g.kh == 1 && g.kw == 1) {
-    // ---- 1x1x1: a plain GEMM over the flattened pixels ----
-    if (g.st != 1 || variant > 0) return false;
-    if (S.T != P.Td || S.H != P.Hd || S.W != P.Wd) return false;
+  if (kind == kSlabFlat) {
+    // a plain GEMM over the flattened pixels
+    if (variant > 0 || !same) return false;
     const long M = (long)P.B * P.Td * P.Hd * P.Wd;
     if (M >= (1l << 31)) return false;
     box[0] = 128;
     L.ntiles[0] = ceil_div((int)M, 128);
-    A.dims[0] = S.C; A.dims[1] = M; A.dims[2] = A.dims[3] = A.dims[4] = 1;
-    A.strides[0] = ld2; A.strides[1] = A.strides[2] = A.strides[3] = (uint64_t)ld2 * M;
-    A.box[0] = 64; A.box[1] = 128; A.box[2] = A.box[3] = A.box[4] = 1;
-    O.dims[0] = P.N; O.dims[1] = M; O.dims[2] = O.dims[3] = O.dims[4] = 1;
-    O.strides[0] = old4; O.strides[1] = O.strides[2] = O.strides[3] = (uint64_t)old4 * M;
-    L.out.oext[0] = (int)M; L.out.oext[1] = L.out.oext[2] = L.out.oext[3] = 1;
-    L.n_types = 1;
-    L.type[0].nshift = 1;
-    L.type[0].tap[0] = 0;
-    L.slab_bytes = 128 * 128;
-    L.shift_bytes = 0;
-  } else if (window) {
-    // ---- space-to-depth stem: (1, kh, kw) over 64/kw-channel pixels, one slab serves all kh*kw taps ----
-    static const int kNw[2] = {16, 8}, kNh[2] = {8, 16};
-    if (variant > 1 || g.kh > 8) return false;
+    oext[0] = (int)M; oext[1] = oext[2] = oext[3] = 1;
+  } else if (kind == kSlabWindow || kind == kSlabRows) {
+    static const int kNw[3] = {16, 8, 32}, kNh[3] = {8, 16, 4};
+    if (variant > (window ? 1 : 2) || g.kh > 8 || (!window && (g.kw > 4 || !same))) return false;
     const int nw = kNw[variant], nh = kNh[variant];
     if (P.Wd % nw != 0 || P.Hd < nh) return false;
     box[0] = nw; box[1] = nh;
-    L.ntiles[0] = ceil_div(P.Wd, nw); L.ntiles[1] = ceil_div(P.Hd, nh); L.ntiles[2] = S.T; L.ntiles[3] = P.B;
-    A.dims[0] = 64; A.dims[1] = P.Wd; A.dims[2] = S.H; A.dims[3] = S.T; A.dims[4] = P.B;
-    A.strides[0] = ld2; A.strides[1] = ld2 * S.W; A.strides[2] = ld2 * S.W * S.H; A.strides[3] = ld2 * S.W * S.H * S.T;
-    A.box[0] = 64; A.box[1] = nw; A.box[2] = nh + g.kh - 1; A.box[3] = 1; A.box[4] = 1;
-    O.dims[0] = P.N; O.dims[1] = P.Wd; O.dims[2] = P.Hd; O.dims[3] = P.Td; O.dims[4] = P.B;
-    O.strides[0] = old4; O.strides[1] = old4 * P.Wd; O.strides[2] = old4 * P.Wd * P.Hd;
-    O.strides[3] = old4 * P.Wd * P.Hd * P.Td;
-    L.out.oext[0] = P.Wd; L.out.oext[1] = P.Hd; L.out.oext[2] = P.Td; L.out.oext[3] = P.B;
-    L.n_types = 1;
-    L.a_c0_step = 0;
-    L.type[0].d[1] = -g.ph;
-    L.type[0].nshift = g.kh;
-    for (int j = 0; j < g.kh; ++j) L.type[0].tap[j] = j;     // K chunk ya = the kw taps of kernel row ya
-    L.slab_bytes = nw * (nh + g.kh - 1) * 128;
-    L.shift_bytes = nw * 128;
-  } else if (g.kt == 1) {
-    // ---- (1, kh, kw), stride 1: dy taps share one slab, one slab type per dx ----
-    if (g.st != 1 || g.kw > 4 || g.kh > 8) return false;
-    if (S.T != P.Td || S.H != P.Hd || S.W != P.Wd) return false;
-    static const int kNw[3] = {16, 8, 32}, kNh[3] = {8, 16, 4};
-    if (variant > 2) return false;
-    const int nw = kNw[variant], nh = kNh[variant];
-    if (S.W % nw != 0 || S.H < nh) return false;
-    box[0] = nw; box[1] = nh;
-    L.ntiles[0] = ceil_div(S.W, nw); L.ntiles[1] = ceil_div(S.H, nh); L.ntiles[2] = S.T; L.ntiles[3] = P.B;
-    A.dims[0] = S.C; A.dims[1] = S.W; A.dims[2] = S.H; A.dims[3] = S.T; A.dims[4] = P.B;
-    A.strides[0] = ld2; A.strides[1] = ld2 * S.W; A.strides[2] = ld2 * S.W * S.H; A.strides[3] = ld2 * S.W * S.H * S.T;
-    A.box[0] = 64; A.box[1] = nw; A.box[2] = nh + g.kh - 1; A.box[3] = 1; A.box[4] = 1;
-    O.dims[0] = P.N; O.dims[1] = P.Wd; O.dims[2] = P.Hd; O.dims[3] = P.Td; O.dims[4] = P.B;
-    O.strides[0] = old4; O.strides[1] = old4 * P.Wd; O.strides[2] = old4 * P.Wd * P.Hd;
-    O.strides[3] = old4 * P.Wd * P.Hd * P.Td;
-    L.out.oext[0] = P.Wd; L.out.oext[1] = P.Hd; L.out.oext[2] = P.Td; L.out.oext[3] = P.B;
-    L.n_types = g.kw;
-    for (int xa = 0; xa < g.kw; ++xa) {
-      TmaSlabType& t = L.type[xa];
-      t.d[0] = tr ? g.pw - xa : xa - g.pw;
-      t.d[1] = tr ? g.ph - (g.kh - 1) : -g.ph;
-      t.nshift = g.kh;
-      for (int j = 0; j < g.kh; ++j) {
-        const int ya = tr ? g.kh - 1 - j : j;
-        t.tap[j] = ya * g.kw + xa;
-      }
-    }
-    L.slab_bytes = nw * (nh + g.kh - 1) * 128;
-    L.shift_bytes = nw * 128;
-  } else if (g.kh == 1 && g.kw == 1) {
-    // ---- (kt, 1, 1): pixels of a frame are one flat dimension, dt taps share one slab ----
-    if (g.kt > 8) return false;
-    if (S.H != P.Hd || S.W != P.Wd) return false;
-    const int HW = S.H * S.W;
+    L.ntiles[0] = ceil_div(P.Wd, nw); L.ntiles[1] = ceil_div(P.Hd, nh); L.ntiles[2] = P.Td; L.ntiles[3] = P.B;
+    oext[0] = P.Wd; oext[1] = P.Hd; oext[2] = P.Td; oext[3] = P.B;
+  } else if (kind == kSlabFrames || kind == kSlabParity) {
     static const int kNpx[3] = {16, 8, 32}, kNt[3] = {8, 16, 4};
-    if (variant > 2) return false;
+    if (variant > 2 || g.kt > 8 || S.H != P.Hd || S.W != P.Wd) return false;
+    const int HW = P.Hd * P.Wd;
     const int npx = kNpx[variant], nt = kNt[variant];
-    const int t_tiles_over = (g.st == 1) ? P.Td : (tr ? P.Td / 2 : P.Td);
-    if (HW % npx != 0 || 2 * t_tiles_over < nt + 1) return false;   // at most half a tile of temporal overhang
-    box[0] = npx; box[2] = nt;
-    const long oHW = (long)P.Hd * P.Wd;
-    if (g.st == 1) {
-      if (S.T != P.Td) return false;
-      L.ntiles[0] = ceil_div(HW, npx); L.ntiles[2] = ceil_div(P.Td, nt); L.ntiles[3] = P.B;
-      A.dims[0] = S.C; A.dims[1] = HW; A.dims[2] = 1; A.dims[3] = S.T; A.dims[4] = P.B;
-      A.strides[0] = ld2; A.strides[1] = ld2 * HW; A.strides[2] = ld2 * HW; A.strides[3] = ld2 * HW * S.T;
-      A.box[0] = 64; A.box[1] = npx; A.box[2] = 1; A.box[3] = nt + g.kt - 1; A.box[4] = 1;
-      O.dims[0] = P.N; O.dims[1] = oHW; O.dims[2] = 1; O.dims[3] = P.Td; O.dims[4] = P.B;
-      O.strides[0] = old4; O.strides[1] = old4 * oHW; O.strides[2] = old4 * oHW; O.strides[3] = old4 * oHW * P.Td;
-      L.out.oext[0] = (int)oHW; L.out.oext[1] = 1; L.out.oext[2] = P.Td; L.out.oext[3] = P.B;
-      L.n_types = 1;
-      TmaSlabType& t = L.type[0];
-      t.d[2] = tr ? g.pt - (g.kt - 1) : -g.pt;
-      t.nshift = g.kt;
-      for (int j = 0; j < g.kt; ++j) t.tap[j] = tr ? g.kt - 1 - j : j;
-      L.slab_bytes = npx * (nt + g.kt - 1) * 128;
-    } else if (g.st == 2 && !tr) {
-      // forward, temporal stride 2: input frame 2*t' - pt + dt = 2*(t' + sh) + par; one slab type per frame parity
-      if (S.T % 2 != 0 || (S.T + 2 * g.pt - g.kt) / 2 + 1 != P.Td) return false;
-      L.ntiles[0] = ceil_div(HW, npx); L.ntiles[2] = ceil_div(P.Td, nt); L.ntiles[3] = P.B;
-      int maxshift = 0;
-      L.n_types = 2;
-      for (int par = 0; par < 2; ++par) {
-        TmaSlabType& t = L.type[par];
-        t.nshift = 0;
-        int sh_min = 0;
-        for (int dt = 0; dt < g.kt; ++dt) {
-          if (pymod(dt - g.pt, 2) != par) continue;
-          const int sh = (dt - g.pt - par) / 2;   // exact
-          if (t.nshift == 0) sh_min = sh;
-          t.tap[t.nshift++] = dt;
-        }
-        if (t.nshift == 0) return false;
-        t.d[1] = par;
-        t.d[2] = sh_min;
-        maxshift = t.nshift > maxshift ? t.nshift : maxshift;
-      }
-      A.dims[0] = S.C; A.dims[1] = HW; A.dims[2] = 2; A.dims[3] = S.T / 2; A.dims[4] = P.B;
-      A.strides[0] = ld2; A.strides[1] = ld2 * HW; A.strides[2] = ld2 * HW * 2; A.strides[3] = ld2 * HW * S.T;
-      A.box[0] = 64; A.box[1] = npx; A.box[2] = 1; A.box[3] = nt + maxshift - 1; A.box[4] = 1;
-      O.dims[0] = P.N; O.dims[1] = oHW; O.dims[2] = 1; O.dims[3] = P.Td; O.dims[4] = P.B;
-      O.strides[0] = old4; O.strides[1] = old4 * oHW; O.strides[2] = old4 * oHW; O.strides[3] = old4 * oHW * P.Td;
-      L.out.oext[0] = (int)oHW; L.out.oext[1] = 1; L.out.oext[2] = P.Td; L.out.oext[3] = P.B;
-      L.slab_bytes = npx * (nt + maxshift - 1) * 128;
-    } else if (g.st == 2 && tr) {
-      // data gradient of the temporally strided conv: output frame t = 2*th + par receives dY[th + sh] * W[dt] with
-      // dt = par + pt - 2*sh; the frame parity of a tile selects its slab type
+    // the data gradient of the strided conv tiles the output frames of one parity: Td / 2 of them
+    const int TH = kind == kSlabParity && tr ? P.Td / 2 : P.Td;
+    if (HW % npx != 0 || 2 * TH < nt + 1) return false;   // at most half a tile of temporal overhang
+    if (kind == kSlabFrames && S.T != P.Td) return false;
+    if (kind == kSlabParity && !tr && (S.T % 2 != 0 || (S.T + 2 * g.pt - g.kt) / 2 + 1 != P.Td)) return false;
+    if (kind == kSlabParity && tr) {
+      // output frame t = 2 th + par receives dY[th + sh] * W[dt] with dt = par + pt - 2 sh; the frame parity of a tile
+      // selects its slab type
       if (P.Td % 2 != 0 || (P.Td + 2 * g.pt - g.kt) / 2 + 1 != S.T) return false;
-      const int TH = P.Td / 2;
-      L.ntiles[0] = ceil_div(HW, npx); L.ntiles[1] = 2; L.ntiles[2] = ceil_div(TH, nt); L.ntiles[3] = P.B;
+      L.ntiles[1] = 2;
       L.sel_dim = 1;
-      L.n_types = 2;
-      int maxshift = 0;
-      for (int par = 0; par < 2; ++par) {
-        TmaSlabType& t = L.type[par];
-        t.nshift = 0;
-        int sh_min = 0;
-        for (int dt = g.kt - 1; dt >= 0; --dt) {    // descending dt = ascending sh
-          if (pymod(par + g.pt - dt, 2) != 0) continue;
-          const int sh = (par + g.pt - dt) / 2;     // may be negative: C division of an even number is exact
-          if (t.nshift == 0) sh_min = sh;
-          t.tap[t.nshift++] = dt;
-        }
-        if (t.nshift == 0) return false;
-        t.d[2] = sh_min;
-        maxshift = t.nshift > maxshift ? t.nshift : maxshift;
-      }
-      A.dims[0] = S.C; A.dims[1] = HW; A.dims[2] = 1; A.dims[3] = S.T; A.dims[4] = P.B;
-      A.strides[0] = ld2; A.strides[1] = ld2 * HW; A.strides[2] = ld2 * HW; A.strides[3] = ld2 * HW * S.T;
-      A.box[0] = 64; A.box[1] = npx; A.box[2] = 1; A.box[3] = nt + maxshift - 1; A.box[4] = 1;
-      O.dims[0] = P.N; O.dims[1] = oHW; O.dims[2] = 2; O.dims[3] = TH; O.dims[4] = P.B;
-      O.strides[0] = old4; O.strides[1] = old4 * oHW; O.strides[2] = old4 * oHW * 2; O.strides[3] = old4 * oHW * P.Td;
-      L.out.oext[0] = (int)oHW; L.out.oext[1] = 2; L.out.oext[2] = TH; L.out.oext[3] = P.B;
-      L.slab_bytes = npx * (nt + maxshift - 1) * 128;
-    } else {
-      return false;
     }
-    L.shift_bytes = npx * 128;
+    box[0] = npx; box[2] = nt;
+    L.ntiles[0] = ceil_div(HW, npx); L.ntiles[2] = ceil_div(TH, nt); L.ntiles[3] = P.B;
+    oext[0] = HW; oext[1] = L.ntiles[1]; oext[2] = TH; oext[3] = P.B;
   } else {
     return false;
   }
+  L.n_types = slab_types(kind, g, L.type);
+  if (L.n_types == 0) return false;
+  int reuse = 0;
+  for (int i = 0; i < L.n_types; ++i) reuse = L.type[i].nshift > reuse ? L.type[i].nshift : reuse;
+  A = slab_map(kind, g, S, P.B, P.Wd, box, reuse);
+  L.slab_bytes = 128 * (int)(A.box[1] * A.box[2] * A.box[3] * A.box[4]);
+  L.shift_bytes = kind == kSlabFlat ? 0 : 128 * box[0];   // one row of the reuse dimension (box[1] = 1 for frames)
   if (L.slab_bytes / 128 > 256 * 4) return false;
   for (int d = 0; d < 4; ++d) {
     L.out.obox[d] = box[d];
@@ -506,7 +481,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
     L.a_mul[L.sel_dim] = 0;
     L.out.o_mul[L.sel_dim] = 1;
   }
-  if (g.st == 2 && !tr && g.kt > 1) L.a_mul[1] = 0, L.out.o_mul[1] = 0;   // A parity coordinate comes from the slab type
+  if (kind == kSlabParity && !tr) L.a_mul[1] = 0, L.out.o_mul[1] = 0;   // A parity coordinate comes from the slab type
   long mt = 1;
   for (int d = 0; d < 4; ++d) mt *= L.ntiles[d];
   if (mt * L.out.n_tiles_n >= (1l << 31)) return false;
@@ -519,8 +494,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
     rem /= sb[d];
   }
   if (rem != 1) return false;
-  O.box[0] = 32;
-  for (int d = 0; d < 4; ++d) O.box[1 + d] = sb[d];
+  O = plane_map(P.dst, nullptr, P.dst_coff, 4, P.dst_ld, P.N, L.out.oext, {32, sb[0], sb[1], sb[2], sb[3]});
   for (int w = 0; w < 4; ++w) {
     int r = 32 * w;
     for (int d = 0; d < 4; ++d) {
@@ -532,7 +506,7 @@ static bool conv_tma_plan_variant(const coclr_conv_t& P, int variant, TmaPlan& L
   for (int i = 0; i < 2; ++i)
     if (A.base[i] && ((uintptr_t)A.base[i] & 15)) return false;
   if (planes == 2 && !A.base[1]) return false;
-  if (((uintptr_t)O.base[0] & 15) || (old4 % 16) != 0 || (ld2 % 16) != 0) return false;
+  if (((uintptr_t)O.base[0] & 15) || O.strides[0] % 16 != 0 || A.strides[0] % 16 != 0) return false;
   for (int d = 0; d < 5; ++d)
     if (A.box[d] > 256 || O.box[d] > 256 || A.dims[d] == 0 || O.dims[d] == 0) return false;
   // ---- shared memory ----
@@ -639,13 +613,7 @@ int coclr::conv_tma_try(const coclr_conv_t& P, int num_sms, cudaStream_t stream)
   MapSpec A, O;
   if (!conv_tma_plan(P, args.plan, A, O)) return 1;
   CUtensorMap m_hi, m_lo, m_out;
-  if (!encode_map(&m_hi, A, 0)) return 1;
-  if (P.npass > 1) {
-    if (!encode_map(&m_lo, A, 1)) return 1;
-  } else {
-    m_lo = m_hi;
-  }
-  if (!encode_map(&m_out, O, 0)) return 1;
+  if (!encode_maps(&m_hi, &m_lo, A, P.npass) || !encode_map(&m_out, O, 0)) return 1;
   const TmaPlan& L = args.plan;
   args.wpk = P.wpk;
   args.wunscale = P.wunscale;

@@ -325,9 +325,10 @@ inline int launch_with_smem(void (*kernel)(Params...), int grid, int threads, ui
   return COCLR_OK;
 }
 
-// One TMA slab load: coordinate offsets (logical dims 1..4 of the tensor map) relative to the tile origin, and the
-// taps it serves -- shift j reads the slab at row offset j * shift_rows and multiplies with packed K chunk
-// tap[j] * nc + channel_chunk.
+// One TMA slab load of the activation planes: its origin relative to the tile origin (logical dims 1..4 of the tensor
+// map), and the taps of the reuse dimension it serves.  Shift j reads the slab j rows of that dimension further on and
+// belongs to tap[j] (kt-major, as in the weight tensor): the convolution multiplies it with packed K chunk
+// tap[j] * nc + channel_chunk, the weight gradient makes it N block j.
 struct TmaSlabType {
   int d[4];
   int nshift;
@@ -376,6 +377,37 @@ struct MapSpec {
 };
 // cuTensorMapEncodeTiled through the runtime's driver entry point (no -lcuda); plane `which`; false when unavailable
 bool encode_map(CUtensorMap* m, const MapSpec& s, int which, int rank = 5, bool swizzle = true);
+// The hi map, and the lo map when there are several passes (else a copy of the hi map, which the kernel never reads).
+bool encode_maps(CUtensorMap* hi, CUtensorMap* lo, const MapSpec& s, int npass);
+// A dense channels-last plane at base(s) + coff elements, pixels ld elements apart, as a 5-D tensor map: dim 0 the c
+// channels, dims 1..4 the logical extents ext (dim 1 fastest, each dim's stride the previous one's times its extent).
+// pitch > 0: dim 2 advances pitch pixels although dim 1 holds only ext[0] of them (the window map's rows).
+MapSpec plane_map(const void* hi, const void* lo, int coff, int elem_bytes, int ld, int c, const int (&ext)[4],
+                  const int (&box)[5], int pitch = 0);
+
+// How the TMA kernels see the activation planes of a launch.  A tile covers a box of destination pixels; its halo slab
+// is that box extended along the kind's reuse dimension (logical dim 1 for the rows, 2 for the frames) by the taps
+// that read it.
+enum SlabKind {
+  kSlabNone,     // not on the TMA kernels
+  kSlabFlat,     // 1x1x1: the pixels as one flat dimension [C, M, 1, 1, 1], one tap
+  kSlabWindow,   // space-to-depth stem (1,kh,kw): [64, W, H, T, B] over 64/kw-channel pixels, see slab_kind
+  kSlabRows,     // (1,kh,kw): [C, W, H, T, B]; one slab type per dx, the kh taps of dy share it
+  kSlabFrames,   // (kt,1,1): [C, H*W, 1, T, B]; the kt taps of dt share one slab
+  kSlabParity,   // (kt,1,1) at temporal stride 2: [C, H*W, 2, T/2, B]; one slab type per frame parity
+};
+// The kind of a spatially unstrided convolution of source S onto a Td x Hd x Wd grid.  Each planner adds its own limits.
+SlabKind slab_kind(const coclr_geom_t& g, const coclr_src_t& S, int Td, int Hd, int Wd);
+// Fills the kind's slab types (the data gradient's, g.transposed, mirrored: taps reversed, origins reflected) and
+// returns how many there are, 0 when a frame parity has no taps.
+int slab_types(SlabKind kind, const coclr_geom_t& g, TmaSlabType (&type)[4]);
+// The source planes of a kind as one tensor map over B clips onto a destination Wd pixels wide, loaded 64 channels x
+// the slab of a tile box whose types serve up to `reuse` taps each.
+MapSpec slab_map(SlabKind kind, const coclr_geom_t& g, const coclr_src_t& S, int B, int Wd, const int (&tile)[4],
+                 int reuse);
+
+inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
+inline int pymod(int a, int b) { return ((a % b) + b) % b; }
 
 // TMA-staged weight gradient (wgrad_tma.cu): 0 = launched, < 0 = error, 1 = shape not covered (caller falls back)
 int wgrad_tma_try(const coclr_wgrad_t& P, cudaStream_t stream);

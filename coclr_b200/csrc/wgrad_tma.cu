@@ -45,12 +45,6 @@ static constexpr int kWgTilePx = 64;                 // pixels per pipeline stag
 static constexpr int kWgBlockBytes = kWgTilePx * 128;  // one [64 px][64 ch] operand block
 static constexpr int kWgMaxStages = 4;
 
-struct WgType {
-  int d[4];        // slab origin relative to the tile origin (logical dims 1..4 of the X map)
-  int nblk;        // N blocks served by this slab (taps of the reuse dimension)
-  int tap[8];      // tap index (kt-major, as in the weight tensor) of each block
-};
-
 struct WgPlan {
   int ntiles[4];     // pixel tiles per logical dim (dim 0 fastest)
   int box[4];        // tile extent per dim
@@ -59,10 +53,10 @@ struct WgPlan {
   int nc;            // 64-channel chunks of the input
   int n_cgroups;     // column groups per type: nc (slab mode) or ceil(nc / nload) (block mode)
   int nload;         // X loads per stage and plane (block mode: up to 4 channel chunks; slab mode: 1)
-  WgType type[4];
+  TmaSlabType type[4];
   int slab_bytes;    // one X load (a multiple of 1024)
   int lbo_bytes;     // distance between consecutive N blocks
-  int N;             // columns of one MMA = 64 * blocks (the widest slab type; a type with fewer taps uses 64 * nblk)
+  int N;             // columns of one MMA = 64 * blocks (the widest slab type; a type with fewer taps uses 64 * nshift)
   int win_c, win_kw; // window mode (space-to-depth stem): a 64-element block is win_kw pixels of win_c channels
   int mb;            // 64-cout blocks per item, one per MMA warpgroup (stacked: 2 = hi / lo plane of the one block)
   int m_groups;      // cout groups
@@ -87,7 +81,7 @@ struct WgArgs {
 struct WgCol {
   int tap, c;
 };
-COCLR_DEVINL WgCol wg_col(const WgPlan& L, const WgType& T, int cg, int col) {
+COCLR_DEVINL WgCol wg_col(const WgPlan& L, const TmaSlabType& T, int cg, int col) {
   const int blk = col >> 6;
   WgCol r;
   if (L.win_c) {                      // window mode: a block is a kernel row, its 64 elements are (dx, channel)
@@ -95,7 +89,7 @@ COCLR_DEVINL WgCol wg_col(const WgPlan& L, const WgType& T, int cg, int col) {
     const int dx = within / L.win_c;
     r.tap = T.tap[blk] * L.win_kw + dx;
     r.c = within - dx * L.win_c;
-  } else if (L.nload > 1 || T.nblk == 1) {   // block mode: a block is a channel chunk of the single tap
+  } else if (L.nload > 1 || T.nshift == 1) {   // block mode: a block is a channel chunk of the single tap
     r.tap = T.tap[0];
     r.c = (cg * L.nload + blk) * 64 + (col & 63);
   } else {                            // slab mode: a block is a tap of the reuse dimension
@@ -161,7 +155,7 @@ wgrad_tma_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid_con
     mbar_fence_init();
   }
   __syncthreads();
-  const WgType& T = L.type[type_i];
+  const TmaSlabType& T = L.type[type_i];
   const uint32_t dy_plane_bytes = (uint32_t)L.mb * kWgBlockBytes;
   const uint32_t x_plane_bytes = (uint32_t)L.nload * (uint32_t)L.slab_bytes;
 
@@ -344,7 +338,7 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const WgArgs P) {
   const int rows = L.stacked ? 64 : L.mb * 64;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   const int col = idx / rows, r = idx - col * rows;
-  if (col >= (L.nload > 1 ? L.N : 64 * L.type[type_i].nblk)) return;
+  if (col >= (L.nload > 1 ? L.N : 64 * L.type[type_i].nshift)) return;
   const int n = L.stacked ? r : mg * L.mb * 64 + r;
   const WgCol k = wg_col(L, L.type[type_i], cg, col);
   if (n >= L.Cout || k.c >= L.Cin_real) return;
@@ -363,8 +357,6 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const WgArgs P) {
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-static int wg_ceil_div(int a, int b) { return (a + b - 1) / b; }
-
 static int wg_num_sms() {
   static int n = 0;
   if (n == 0) {
@@ -380,21 +372,29 @@ static long wg_ws_floats(const WgPlan& L) {
   return (long)L.n_types * L.n_cgroups * L.m_groups * L.splits * L.N * 128 * L.m_tiles;
 }
 
+// Of the tile shapes (w[v], h[v]), the first that pads a W x H grid least; false when even that one would make more
+// than half of every tile padding.
+template <int n>
+static bool least_padding(const int (&w)[n], const int (&h)[n], int W, int H, int& bw, int& bh) {
+  long best_px = 0;
+  for (int v = 0; v < n; ++v) {
+    const long px = (long)ceil_div(W, w[v]) * w[v] * ceil_div(H, h[v]) * h[v];
+    if (v == 0 || px < best_px) { best_px = px; bw = w[v]; bh = h[v]; }
+  }
+  return 2 * (long)W * H >= best_px;
+}
+
 static bool wgrad_tma_plan(const coclr_wgrad_t& P, WgPlan& L, MapSpec& DY, MapSpec& X) {
   const coclr_geom_t& g = P.g;
   const coclr_src_t& S = P.src;
   const coclr_src_t& D = P.dy;
   memset(&L, 0, sizeof(L));
   if (P.npass != 1 && P.npass != 3) return false;
-  if (g.transposed || g.sh != 1 || g.sw != 1 || (g.st != 1 && g.st != 2)) return false;
-  if (D.T != P.Td || D.H != P.Hd || D.W != P.Wd) return false;
-  // window kind (the space-to-depth stem, see conv_tma.cu): the kw taps of a kernel row are kw consecutive pixels of
-  // 64 / kw channels = one 128-byte run, read through a tensor map whose pixel stride is smaller than its inner extent
-  const bool window = g.kt == 1 && g.kw > 1 && S.C * g.kw == 64 && S.ld == S.C && S.coff == 0 && g.pw == 0 &&
-                      g.st == 1 && S.W >= P.Wd + g.kw - 1 && S.H == P.Hd && S.T == P.Td;
-  const bool tstride = g.st == 2 && g.kh == 1 && g.kw == 1 && g.kt > 1;
-  if (g.st == 2 && !tstride) return false;
-  if (!window && !tstride && (S.T != P.Td || S.H != P.Hd || S.W != P.Wd)) return false;   // else "same" convs only
+  if (g.transposed) return false;
+  const SlabKind kind = slab_kind(g, S, P.Td, P.Hd, P.Wd);
+  if (kind == kSlabNone || D.T != P.Td || D.H != P.Hd || D.W != P.Wd) return false;
+  // "same" convolutions only, but for the window's padded rows and the strided conv's input frames
+  if (kind != kSlabWindow && kind != kSlabParity && (S.T != P.Td || S.H != P.Hd || S.W != P.Wd)) return false;
   if (S.C % 8 || D.C % 8 || S.ld % 8 || D.ld % 8 || S.coff % 8 || D.coff % 8) return false;
   if (P.npass > 1 && (!S.lo || !D.lo)) return false;
   if (((uintptr_t)S.hi | (uintptr_t)D.hi | (uintptr_t)S.lo | (uintptr_t)D.lo) & 15) return false;
@@ -406,164 +406,60 @@ static bool wgrad_tma_plan(const coclr_wgrad_t& P, WgPlan& L, MapSpec& DY, MapSp
   L.Cin_real = P.Cin_real;
   L.Cout = P.Cout;
   L.planes = P.npass > 1 ? 2 : 1;
-  L.nc = wg_ceil_div(S.C, 64);
-  const long ldx = (long)S.ld * 2, ldd = (long)D.ld * 2;
-  DY.elem_bytes = X.elem_bytes = 2;
-  DY.base[0] = (void*)((const uint16_t*)D.hi + D.coff);
-  DY.base[1] = D.lo ? (void*)((const uint16_t*)D.lo + D.coff) : nullptr;
-  X.base[0] = (void*)((const uint16_t*)S.hi + S.coff);
-  X.base[1] = S.lo ? (void*)((const uint16_t*)S.lo + S.coff) : nullptr;
+  L.nc = ceil_div(S.C, 64);
+  L.nload = 1;
+  L.n_cgroups = L.nc;
   for (int d = 0; d < 4; ++d) L.ntiles[d] = L.box[d] = 1;
-  int reuse = 1;       // taps served by one slab
-  if (L.taps == 1) {
-    // ---- 1x1x1: flat pixels, up to four channel chunks next to each other ----
+  int ext[4];          // the output grid in the logical dims of the kind
+  if (kind == kSlabFlat) {
+    // flat pixels, up to four channel chunks next to each other
     L.box[0] = kWgTilePx;
-    L.ntiles[0] = wg_ceil_div((int)M, kWgTilePx);
-    for (MapSpec* m : {&DY, &X}) {
-      const long ld = m == &DY ? ldd : ldx;
-      m->dims[0] = m == &DY ? D.C : S.C; m->dims[1] = M; m->dims[2] = m->dims[3] = m->dims[4] = 1;
-      m->strides[0] = ld; m->strides[1] = m->strides[2] = m->strides[3] = (uint64_t)ld * M;
-      m->box[0] = 64; m->box[1] = kWgTilePx; m->box[2] = m->box[3] = m->box[4] = 1;
-    }
-    L.n_types = 1;
-    L.type[0].nblk = 1;
-    L.type[0].tap[0] = 0;
+    L.ntiles[0] = ceil_div((int)M, kWgTilePx);
     L.nload = L.nc < 4 ? L.nc : (L.nc % 4 == 0 ? 4 : (L.nc % 3 == 0 ? 3 : 4));
-    L.n_cgroups = wg_ceil_div(L.nc, L.nload);
-    L.slab_bytes = kWgBlockBytes;
-    L.lbo_bytes = kWgBlockBytes;
-    L.N = 64 * L.nload;
-  } else if (window) {
-    // ---- space-to-depth stem: (1, kh, kw) over 64/kw-channel pixels; ONE slab serves all kh * kw taps: its blocks are
-    // the kernel rows, the 64 elements of a block the kw pixels x channels of that row ----
-    static const int kNw[2] = {8, 16}, kNh[2] = {8, 4};
-    int best = -1;
-    long best_px = 0;
-    for (int v = 0; v < 2; ++v) {
-      const long px = (long)wg_ceil_div(P.Wd, kNw[v]) * kNw[v] * wg_ceil_div(P.Hd, kNh[v]) * kNh[v];
-      if (best < 0 || px < best_px) { best = v; best_px = px; }
-    }
-    const int nw = kNw[best], nh = kNh[best];
-    if (2 * (long)P.Wd * P.Hd < best_px || g.kh > 4) return false;
+    L.n_cgroups = ceil_div(L.nc, L.nload);
+    ext[0] = (int)M; ext[1] = ext[2] = ext[3] = 1;
+  } else if (kind == kSlabWindow || kind == kSlabRows) {
+    // tiles of nw x nh pixels; the window's blocks are the kernel rows, the 64 elements of a block the kw pixels x
+    // channels of that row, so ONE slab serves all kh * kw taps
+    static const int kNw[3] = {16, 8, 32}, kNh[3] = {4, 8, 2};          // least padding first, then the wider rows
+    static const int kWinNw[2] = {8, 16}, kWinNh[2] = {8, 4};
+    int nw, nh;
+    const bool fits = kind == kSlabWindow ? least_padding(kWinNw, kWinNh, P.Wd, P.Hd, nw, nh) && g.kh <= 4
+                                          : least_padding(kNw, kNh, P.Wd, P.Hd, nw, nh);
+    if (!fits) return false;
     L.box[0] = nw; L.box[1] = nh;
-    L.ntiles[0] = wg_ceil_div(P.Wd, nw); L.ntiles[1] = wg_ceil_div(P.Hd, nh); L.ntiles[2] = P.Td; L.ntiles[3] = P.B;
-    DY.dims[0] = D.C; DY.dims[1] = P.Wd; DY.dims[2] = P.Hd; DY.dims[3] = P.Td; DY.dims[4] = P.B;
-    DY.strides[0] = ldd; DY.strides[1] = ldd * P.Wd; DY.strides[2] = ldd * P.Wd * P.Hd;
-    DY.strides[3] = ldd * P.Wd * P.Hd * P.Td;
-    DY.box[0] = 64; DY.box[1] = nw; DY.box[2] = nh; DY.box[3] = DY.box[4] = 1;
-    X.dims[0] = 64; X.dims[1] = P.Wd; X.dims[2] = S.H; X.dims[3] = S.T; X.dims[4] = P.B;
-    X.strides[0] = ldx; X.strides[1] = ldx * S.W; X.strides[2] = ldx * S.W * S.H; X.strides[3] = ldx * S.W * S.H * S.T;
-    X.box[0] = 64; X.box[1] = nw; X.box[2] = nh + g.kh - 1; X.box[3] = X.box[4] = 1;
-    reuse = g.kh;
-    L.n_types = 1;
-    L.type[0].d[1] = -g.ph;
-    L.type[0].nblk = g.kh;
-    for (int j = 0; j < g.kh; ++j) L.type[0].tap[j] = j;
-    L.nc = 1;
-    L.nload = 1;
-    L.n_cgroups = 1;
-    L.win_c = S.C;
-    L.win_kw = g.kw;
-    L.slab_bytes = nw * (nh + g.kh - 1) * 128;
-    L.lbo_bytes = nw * 128;
-    L.N = 64 * g.kh;
-  } else if (g.kt == 1) {
-    // ---- (1, kh, kw): tiles of nw x nh pixels, one slab type per dx, the kh taps of a column share the slab ----
-    static const int kNw[3] = {16, 8, 32}, kNh[3] = {4, 8, 2};
-    int best = -1;
-    long best_px = 0;
-    for (int v = 0; v < 3; ++v) {      // least padding first, then the wider rows
-      const long px = (long)wg_ceil_div(P.Wd, kNw[v]) * kNw[v] * wg_ceil_div(P.Hd, kNh[v]) * kNh[v];
-      if (best < 0 || px < best_px) { best = v; best_px = px; }
+    L.ntiles[0] = ceil_div(P.Wd, nw); L.ntiles[1] = ceil_div(P.Hd, nh); L.ntiles[2] = P.Td; L.ntiles[3] = P.B;
+    if (kind == kSlabWindow) {
+      L.win_c = S.C;
+      L.win_kw = g.kw;
     }
-    const int nw = kNw[best], nh = kNh[best];
-    if (2 * (long)P.Wd * P.Hd < best_px) return false;       // more than half of every tile would be padding
-    L.box[0] = nw; L.box[1] = nh;
-    L.ntiles[0] = wg_ceil_div(P.Wd, nw); L.ntiles[1] = wg_ceil_div(P.Hd, nh); L.ntiles[2] = P.Td; L.ntiles[3] = P.B;
-    for (MapSpec* m : {&DY, &X}) {
-      const long ld = m == &DY ? ldd : ldx;
-      m->dims[0] = m == &DY ? D.C : S.C; m->dims[1] = P.Wd; m->dims[2] = P.Hd; m->dims[3] = P.Td; m->dims[4] = P.B;
-      m->strides[0] = ld; m->strides[1] = ld * P.Wd; m->strides[2] = ld * P.Wd * P.Hd;
-      m->strides[3] = ld * P.Wd * P.Hd * P.Td;
-      m->box[0] = 64; m->box[1] = nw; m->box[2] = nh; m->box[3] = m->box[4] = 1;
-    }
-    X.box[2] = nh + g.kh - 1;
-    reuse = g.kh;
-    L.n_types = g.kw;
-    for (int xa = 0; xa < g.kw; ++xa) {
-      WgType& t = L.type[xa];
-      t.d[0] = xa - g.pw;
-      t.d[1] = -g.ph;
-      t.nblk = g.kh;
-      for (int j = 0; j < g.kh; ++j) t.tap[j] = j * g.kw + xa;
-    }
-    L.nload = 1;
-    L.n_cgroups = L.nc;
-    L.slab_bytes = nw * (nh + g.kh - 1) * 128;
-    L.lbo_bytes = nw * 128;
-    L.N = 64 * g.kh;
-  } else if (g.kh == 1 && g.kw == 1) {
-    // ---- (kt, 1, 1): the pixels of a frame are one flat dimension; tiles of npx pixels x nt frames ----
-    const int HW = P.Hd * P.Wd;
-    static const int kNpx[4] = {16, 8, 32, 64}, kNt[4] = {4, 8, 2, 1};
-    int best = -1;
-    long best_px = 0;
-    for (int v = 0; v < 4; ++v) {
-      const long px = (long)wg_ceil_div(HW, kNpx[v]) * kNpx[v] * wg_ceil_div(P.Td, kNt[v]) * kNt[v];
-      if (best < 0 || px < best_px) { best = v; best_px = px; }
-    }
-    const int npx = kNpx[best], nt = kNt[best];
-    if (2 * (long)HW * P.Td < best_px) return false;
-    L.box[0] = npx; L.box[2] = nt;
-    L.ntiles[0] = wg_ceil_div(HW, npx); L.ntiles[2] = wg_ceil_div(P.Td, nt); L.ntiles[3] = P.B;
-    DY.dims[0] = D.C; DY.dims[1] = HW; DY.dims[2] = 1; DY.dims[3] = P.Td; DY.dims[4] = P.B;
-    DY.strides[0] = ldd; DY.strides[1] = ldd * HW; DY.strides[2] = ldd * HW; DY.strides[3] = ldd * HW * P.Td;
-    DY.box[0] = 64; DY.box[1] = npx; DY.box[2] = 1; DY.box[3] = nt; DY.box[4] = 1;
-    L.nload = 1;
-    L.n_cgroups = L.nc;
-    L.lbo_bytes = npx * 128;
-    if (!tstride) {
-      X.dims[0] = S.C; X.dims[1] = HW; X.dims[2] = 1; X.dims[3] = S.T; X.dims[4] = P.B;
-      X.strides[0] = ldx; X.strides[1] = ldx * HW; X.strides[2] = ldx * HW; X.strides[3] = ldx * HW * S.T;
-      X.box[0] = 64; X.box[1] = npx; X.box[2] = 1; X.box[3] = nt + g.kt - 1; X.box[4] = 1;
-      reuse = g.kt;
-      L.n_types = 1;
-      WgType& t = L.type[0];
-      t.d[2] = -g.pt;
-      t.nblk = g.kt;
-      for (int j = 0; j < g.kt; ++j) t.tap[j] = j;
-    } else {
-      // temporal stride 2 (the stem's (7,1,1) conv): input frame 2 * t' - pt + dt = 2 * (t' + sh) + par; the X map
-      // splits the frames by parity, [C, HW, 2, T / 2, B], and there is one slab type per parity
-      if (S.H != P.Hd || S.W != P.Wd || S.T % 2 != 0 || (S.T + 2 * g.pt - g.kt) / 2 + 1 != P.Td) return false;
-      X.dims[0] = S.C; X.dims[1] = HW; X.dims[2] = 2; X.dims[3] = S.T / 2; X.dims[4] = P.B;
-      X.strides[0] = ldx; X.strides[1] = ldx * HW; X.strides[2] = ldx * HW * 2; X.strides[3] = ldx * HW * S.T;
-      L.n_types = 2;
-      for (int par = 0; par < 2; ++par) {
-        WgType& t = L.type[par];
-        t.nblk = 0;
-        for (int dt = 0; dt < g.kt; ++dt) {
-          const int rel = dt - g.pt;
-          if ((((rel % 2) + 2) % 2) != par) continue;
-          const int sh = (rel - par) / 2;            // exact
-          if (t.nblk == 0) t.d[2] = sh;               // taps of one parity are consecutive shifts
-          t.tap[t.nblk++] = dt;
-        }
-        t.d[1] = par;
-        if (t.nblk == 0) return false;
-        if (t.nblk > reuse) reuse = t.nblk;
-      }
-      X.box[0] = 64; X.box[1] = npx; X.box[2] = 1; X.box[3] = nt + reuse - 1; X.box[4] = 1;
-    }
-    L.slab_bytes = npx * (nt + reuse - 1) * 128;
-    L.N = 64 * reuse;
+    ext[0] = P.Wd; ext[1] = P.Hd; ext[2] = P.Td; ext[3] = P.B;
   } else {
-    return false;
+    // tiles of npx pixels x nt frames; temporal stride 2 (the stem's (7,1,1) conv) reads the input frames by parity
+    static const int kNpx[4] = {16, 8, 32, 64}, kNt[4] = {4, 8, 2, 1};
+    const int HW = P.Hd * P.Wd;
+    int npx, nt;
+    if (!least_padding(kNpx, kNt, HW, P.Td, npx, nt)) return false;
+    if (kind == kSlabParity &&
+        (S.H != P.Hd || S.W != P.Wd || S.T % 2 != 0 || (S.T + 2 * g.pt - g.kt) / 2 + 1 != P.Td))
+      return false;
+    L.box[0] = npx; L.box[2] = nt;
+    L.ntiles[0] = ceil_div(HW, npx); L.ntiles[2] = ceil_div(P.Td, nt); L.ntiles[3] = P.B;
+    ext[0] = HW; ext[1] = 1; ext[2] = P.Td; ext[3] = P.B;
   }
+  L.n_types = slab_types(kind, g, L.type);
+  if (L.n_types == 0) return false;
+  int reuse = 0;       // taps served by one slab
+  for (int i = 0; i < L.n_types; ++i) reuse = L.type[i].nshift > reuse ? L.type[i].nshift : reuse;
+  DY = plane_map(D.hi, D.lo, D.coff, 2, D.ld, D.C, ext, {64, L.box[0], L.box[1], L.box[2], L.box[3]});
+  X = slab_map(kind, g, S, P.B, P.Wd, L.box, reuse);
+  L.slab_bytes = 128 * (int)(X.box[1] * X.box[2] * X.box[3] * X.box[4]);
+  L.lbo_bytes = 128 * L.box[0];
+  L.N = 64 * (kind == kSlabFlat ? L.nload : reuse);
   if (L.N > 256 || reuse > 4) return false;
   L.total_tiles = L.ntiles[0] * L.ntiles[1] * L.ntiles[2] * L.ntiles[3];
   // ---- cout blocks per item: one per MMA warpgroup, as many as shared memory (>= 2 stages) allows ----
-  const int cout_blocks = wg_ceil_div(P.Cout, 64);
+  const int cout_blocks = ceil_div(P.Cout, 64);
   L.stacked = (P.npass > 1 && P.Cout <= 64) ? 1 : 0;
   const uint32_t x_bytes = (uint32_t)L.planes * L.nload * L.slab_bytes;
   const uint32_t budget = 227u * 1024u - 2048u;
@@ -583,7 +479,7 @@ static bool wgrad_tma_plan(const coclr_wgrad_t& P, WgPlan& L, MapSpec& DY, MapSp
     }
     if (L.stacked) return false;
   }
-  L.m_groups = L.stacked ? 1 : wg_ceil_div(cout_blocks, L.mb);
+  L.m_groups = L.stacked ? 1 : ceil_div(cout_blocks, L.mb);
   int st = (int)(budget / L.stage_bytes);
   L.stages = st > kWgMaxStages ? kWgMaxStages : st;
   L.off_bars = (uint32_t)L.stages * L.stage_bytes;
@@ -594,8 +490,8 @@ static bool wgrad_tma_plan(const coclr_wgrad_t& P, WgPlan& L, MapSpec& DY, MapSp
   const int max_splits = L.total_tiles / 4 > 0 ? L.total_tiles / 4 : 1;
   if (splits > max_splits) splits = max_splits;
   if (splits < 1) splits = 1;
-  L.tiles_per_split = wg_ceil_div(L.total_tiles, splits);
-  L.splits = wg_ceil_div(L.total_tiles, L.tiles_per_split);
+  L.tiles_per_split = ceil_div(L.total_tiles, splits);
+  L.splits = ceil_div(L.total_tiles, L.tiles_per_split);
   return true;
 }
 
@@ -608,13 +504,7 @@ int wgrad_tma_try(const coclr_wgrad_t& P, cudaStream_t stream) {
   if (!wgrad_tma_plan(P, args.plan, DY, X) || wg_ws_floats(args.plan) > P.ws_floats) return 1;
   args.ws = P.ws;
   CUtensorMap m_dy_hi, m_dy_lo, m_x_hi, m_x_lo;
-  if (!encode_map(&m_dy_hi, DY, 0) || !encode_map(&m_x_hi, X, 0)) return 1;
-  if (P.npass > 1) {
-    if (!encode_map(&m_dy_lo, DY, 1) || !encode_map(&m_x_lo, X, 1)) return 1;
-  } else {
-    m_dy_lo = m_dy_hi;
-    m_x_lo = m_x_hi;
-  }
+  if (!encode_maps(&m_dy_hi, &m_dy_lo, DY, P.npass) || !encode_maps(&m_x_hi, &m_x_lo, X, P.npass)) return 1;
   const WgPlan& L = args.plan;
   args.dw = P.dw;
   args.out_scale = P.out_scale;
