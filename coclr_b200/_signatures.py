@@ -64,6 +64,10 @@ EXPORTS = {
     "coclr_jpeg_work_bytes": (C.c_size_t, [P]),
     "coclr_jpeg_decode": (I, [P, P]),
     "coclr_jpeg_decode_slots": (I, [P, P, P]),
+    "coclr_jpeg_encode_header": (I, [I, I, I, I, P]),
+    "coclr_jpeg_encode_max_bytes": (C.c_size_t, [I, I, I]),
+    "coclr_jpeg_encode_work_bytes": (C.c_size_t, [I, I, I, I]),
+    "coclr_jpeg_encode": (I, [P, P]),
     "coclr_tvl1_scales": (I, [I, I]),
     "coclr_tvl1_work_bytes": (C.c_size_t, [I, I, I]),
     "coclr_tvl1": (I, [P, P]),

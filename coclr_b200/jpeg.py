@@ -1,5 +1,6 @@
 """JPEG decoding on the GPU: the reference datasets' `pil_from_raw_rgb` (`Image.open(BytesIO(raw)).convert('RGB')`)
-as CUDA kernels (csrc/jpeg.cu), bit-identical to Pillow's libjpeg-turbo decoder.
+as CUDA kernels (csrc/jpeg.cu), bit-identical to Pillow's libjpeg-turbo decoder; and JPEG encoding on the GPU
+(`JpegEncoder`, csrc/jpeg_encode.cu), byte-identical to Pillow's `Image.save(buf, "JPEG", quality=, subsampling=)`.
 
     dec = JpegDecoder()
     batch = dec.parse(jpegs)                  # host only: one bytes object per frame; ValueError names a bad frame
@@ -268,6 +269,83 @@ class JpegDecoder:
                     "frame %d: %s" % (int(i), STATUS[st[i]] if st[i] < len(STATUS) else st[i]) for i in bad[:8]) +
                     (" (and %d more)" % (len(bad) - 8) if len(bad) > 8 else ""))
         return out
+
+
+MAX_SIDE = 65500                                     # COCLR_JPEG_MAX_SIDE
+HEADER_BYTES = 623                                   # COCLR_JPEG_HEADER_BYTES
+
+
+def _settings(quality, subsampling):
+    if isinstance(quality, bool) or not isinstance(quality, (int, np.integer)) or not 1 <= quality <= 100:
+        raise ValueError("quality must be an integer 1 .. 100, got %r" % (quality,))
+    if isinstance(subsampling, bool) or subsampling not in (0, 1, 2):
+        raise ValueError("subsampling must be 0 (4:4:4), 1 (4:2:2) or 2 (4:2:0), got %r" % (subsampling,))
+
+
+def encode_header(h, w, quality=75, subsampling=2):
+    """Host only: the bytes every encoded h x w file starts with (SOI through SOS), as Pillow writes them."""
+    _settings(quality, subsampling)
+    if not (1 <= h <= MAX_SIDE and 1 <= w <= MAX_SIDE):
+        raise ValueError("frame sides must be 1 .. %d, got %d x %d" % (MAX_SIDE, h, w))
+    buf = np.zeros(HEADER_BYTES, np.uint8)
+    n = L.load().coclr_jpeg_encode_header(h, w, int(quality), int(subsampling), _ptr(buf))
+    if n != HEADER_BYTES:
+        raise L.CoclrError("coclr_jpeg_encode_header failed with code %d" % n)
+    return buf.tobytes()
+
+
+class JpegEncoder:
+    """Encodes uint8 RGB frames on the current CUDA device into JPEG files byte-identical to Pillow's
+    `Image.fromarray(frame).save(buf, "JPEG", quality=quality, subsampling=subsampling)` (csrc/jpeg_encode.cu).
+
+        enc = JpegEncoder(quality=95, subsampling=0)
+        files = enc(frames)          # CUDA uint8 [N, H, W, 3] (rows and frames may be strided) -> list of N bytes
+
+    Defaults are Pillow's: quality 75, 4:2:0.  work_limit caps the workspace (bytes): a batch that needs more is
+    encoded in passes of consecutive frames within one call, with the same bytes.  The output buffer holds every
+    file's worst case (coclr_jpeg_encode_max_bytes).  A call reads back the file offsets, then the files' bytes (one
+    copy each, into a pinned buffer).  Device and pinned buffers grow on demand and are reused."""
+
+    def __init__(self, quality=75, subsampling=2, work_limit=1 << 30):
+        _settings(quality, subsampling)
+        self.quality, self.subsampling = int(quality), int(subsampling)
+        self.work_limit = int(work_limit)
+        self._work = self._out = self._offsets = self._host = None
+
+    @staticmethod
+    def _grow(buf, n, **kw):
+        return buf if buf is not None and buf.numel() >= n else torch.empty(max(n, 1), dtype=torch.uint8, **kw)
+
+    def __call__(self, frames):
+        if (not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8 or not frames.is_cuda or
+                frames.dim() != 4 or frames.shape[3] != 3 or frames.stride(3) != 1 or frames.stride(2) != 3):
+            raise ValueError("frames must be a CUDA uint8 [N, H, W, 3] tensor with packed pixels")
+        n, h, w, _ = frames.shape
+        if not (1 <= h <= MAX_SIDE and 1 <= w <= MAX_SIDE):
+            raise ValueError("frame sides must be 1 .. %d, got %d x %d" % (MAX_SIDE, h, w))
+        if n == 0:
+            return []
+        lib = L.load()
+        dev = frames.device
+        q, s = self.quality, self.subsampling
+        max_bytes = lib.coclr_jpeg_encode_max_bytes(h, w, s)
+        work = min(lib.coclr_jpeg_encode_work_bytes(n, h, w, s),
+                   max(self.work_limit, lib.coclr_jpeg_encode_work_bytes(1, h, w, s)))
+        with torch.cuda.device(dev):
+            self._work = self._grow(self._work, work, device=dev)
+            self._out = self._grow(self._out, n * max_bytes, device=dev)
+            if self._offsets is None or self._offsets.numel() < n + 1:
+                self._offsets = torch.empty(max(n + 1, 64), dtype=torch.int64, device=dev)
+            p = L.JpegEncode(n, h, w, q, s, L.dptr(frames), frames.stride(0), frames.stride(1), L.dptr(self._out),
+                             self._out.numel(), L.dptr(self._offsets), L.dptr(self._work), self._work.numel())
+            L.check(lib.coclr_jpeg_encode(C.byref(p), L.stream_ptr()), "coclr_jpeg_encode")
+            offs = self._offsets[:n + 1].cpu().numpy()
+            total = int(offs[-1])
+            self._host = self._grow(self._host, total, pin_memory=True)
+            self._host[:total].copy_(self._out[:total], non_blocking=True)
+            torch.cuda.current_stream().synchronize()
+        data = self._host[:total].numpy().tobytes()
+        return [data[offs[i]:offs[i + 1]] for i in range(n)]
 
 
 class JpegVideoPool:

@@ -160,6 +160,13 @@ class Jpeg(C.Structure):
                 ("work", C.c_void_p), ("work_bytes", C.c_size_t)]
 
 
+class JpegEncode(C.Structure):
+    _fields_ = [("n", C.c_int), ("h", C.c_int), ("w", C.c_int), ("quality", C.c_int), ("subsampling", C.c_int),
+                ("rgb", C.c_void_p), ("frame_stride", C.c_int64), ("row_stride", C.c_int64),
+                ("out", C.c_void_p), ("out_bytes", C.c_size_t), ("offsets", C.c_void_p),
+                ("work", C.c_void_p), ("work_bytes", C.c_size_t)]
+
+
 class Tvl1(C.Structure):
     _fields_ = [("P", C.c_int), ("H", C.c_int), ("W", C.c_int), ("i0", C.c_void_p), ("i1", C.c_void_p),
                 ("flow", C.c_void_p), ("iterations", C.c_void_p), ("work", C.c_void_p), ("work_bytes", C.c_size_t)]
@@ -195,7 +202,10 @@ KERNELS_PER_CALL = {"coclr_bn_bwd": 2, "coclr_l2norm_bwd": 2, "coclr_conv_packed
                     "coclr_center_normalize": 2,
                     "coclr_augment_smem_bytes": 0, "coclr_augment_clf_smem_bytes": 0,
                     "coclr_jpeg_parse": 0, "coclr_jpeg_work_bytes": 0, "coclr_jpeg_decode": 3,
-                    "coclr_jpeg_decode_slots": 3, "coclr_tvl1_scales": 0, "coclr_tvl1_work_bytes": 0,
+                    "coclr_jpeg_decode_slots": 3, "coclr_jpeg_encode_header": 0,
+                    "coclr_jpeg_encode_max_bytes": 0, "coclr_jpeg_encode_work_bytes": 0,
+                    "coclr_jpeg_encode": 8,     # per pass: a batch split by its workspace counts one pass
+                    "coclr_tvl1_scales": 0, "coclr_tvl1_work_bytes": 0,
                     "coclr_flow_zoom_out": 3, "coclr_flow_warp": 2, "coclr_flow_iterate_work_bytes": 0,
                     # data-dependent (two launches per primal-dual iteration until the pairs converge): not counted
                     "coclr_tvl1": 0, "coclr_flow_iterate": 0}

@@ -685,6 +685,49 @@ typedef struct {
 } coclr_jpeg_slots_t;
 int coclr_jpeg_decode_slots(const coclr_jpeg_t* p, const coclr_jpeg_slots_t* s, coclr_stream_t stream);
 
+/* JPEG encoding, byte-identical to Pillow's `Image.fromarray(frame).save(buf, "JPEG", quality=q, subsampling=s)` on
+ * libjpeg(-turbo): baseline sequential Huffman with the Annex K tables, libjpeg's fixed-point RGB -> YCbCr, 2:1
+ * chroma downsampling with its alternating bias, the ISLOW forward DCT and jpeg_set_quality's tables (baseline).
+ * Accepted: quality 1..100, subsampling 0 (4:4:4), 1 (4:2:2), 2 (4:2:0), 1 <= h, w <= COCLR_JPEG_MAX_SIDE.
+ *
+ * coclr_jpeg_encode_header (host only, no CUDA call) writes the COCLR_JPEG_HEADER_BYTES bytes every file starts
+ * with: SOI, JFIF APP0 (1.01, no units, 1:1), DQT 0, DQT 1 (8-bit, zigzag), SOF0 (component ids 1, 2, 3), DHT DC0,
+ * AC0, DC1, AC1, SOS.  Returns COCLR_JPEG_HEADER_BYTES, or COCLR_E_ARG for an unaccepted setting.
+ *
+ * coclr_jpeg_encode encodes n uint8 RGB frames of one size h x w: frame i, row y, column x, channel c is
+ * rgb[i * frame_stride + y * row_stride + 3 * x + c].  Frame i's complete file (header, entropy-coded segment, EOI)
+ * is out[offsets[i], offsets[i + 1]), offsets[0] = 0: the files are packed.  out_bytes must be at least
+ * n * coclr_jpeg_encode_max_bytes(h, w, subsampling), the files' worst case.  It runs in passes of consecutive frames
+ * whose workspace fits work_bytes (at least coclr_jpeg_encode_work_bytes(1, ...); (n, ...) is one pass), a memset
+ * and eight launches per pass, each writing its result in full before the next reads it:
+ *   transform  colour conversion, downsampling, ISLOW DCT and quantisation of 32 blocks per CTA, 8 threads per
+ *              block; int16 coefficients in scan (MCU) order, zigzag within a block, dummy blocks included
+ *   count      one thread per block: its Huffman bits (the DC difference from the component's previous block)
+ *   scan       per frame: the exclusive scan of the block bit counts (64-bit)
+ *   emit       one thread per block ORs its codes in at its bit offset; the last block pads with 1-bits
+ *   stuff      per 1 KB tile: its 0xFF bytes; per frame: the scan of those counts; then the packed file offsets
+ *   scatter    the stuffed bytes (0x00 after each 0xFF), the header before them and EOI after
+ * The bytes are a pure function of each frame and the settings: the same in any batch or pass.  Error codes:
+ * COCLR_E_ARG (a setting, size, stride, pointer or buffer size), COCLR_E_LAUNCH.  No allocation, no
+ * synchronisation. */
+#define COCLR_JPEG_MAX_SIDE 65500
+#define COCLR_JPEG_HEADER_BYTES 623
+typedef struct {
+  int n, h, w;
+  int quality, subsampling;
+  const uint8_t* rgb;                     /* device */
+  int64_t frame_stride, row_stride;       /* bytes */
+  uint8_t* out;                           /* device */
+  size_t out_bytes;
+  int64_t* offsets;                       /* device [n + 1] */
+  void* work;                             /* device, 256-byte aligned */
+  size_t work_bytes;
+} coclr_jpeg_encode_t;
+int coclr_jpeg_encode_header(int h, int w, int quality, int subsampling, uint8_t* out);
+size_t coclr_jpeg_encode_max_bytes(int h, int w, int subsampling);   /* 0 for an unaccepted size or subsampling */
+size_t coclr_jpeg_encode_work_bytes(int n, int h, int w, int subsampling);
+int coclr_jpeg_encode(const coclr_jpeg_encode_t* p, coclr_stream_t stream);
+
 /* TV-L1 optical flow, batched over P frame pairs of one size H x W: the duality-based TV-L1 of Zach, Pock and
  * Bischof as Sanchez Perez, Meinhardt-Llopis and Facciolo give it (IPOL 2013), with fixed parameters: a pyramid of
  * zoom factor 0.5 (at most COCLR_TVL1_MAX_SCALES levels, the coarsest short side >= 16; one level down is a separable

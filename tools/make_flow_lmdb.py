@@ -4,10 +4,10 @@
 
 Every video of the RGB database (keys '%09d', in key order) is decoded on the GPU (coclr_b200.jpeg), converted to
 grey, and its N - 1 consecutive frame pairs are solved with coclr_b200.flow.tvl1 in chunks of at most --pairs pairs.
-The flow is quantised to 8-bit frames on the GPU (coclr_b200.flow.LAYOUT) and each frame is JPEG-encoded with Pillow
-(QUALITY, SUBSAMPLING) in a thread pool, overlapping the next video's solve.  The video's list of JPEGs is stored under
-the same key, then `__keys__`, `__len__` and `__order__` as the RGB database has them and `__vlen__` with the flow
-frame counts (N - 1) in `__keys__` order.  The flow frames use the msgpack family (str or bin) of the RGB database's
+The flow is quantised to 8-bit frames on the GPU (coclr_b200.flow.LAYOUT) and each chunk is JPEG-encoded there too
+(coclr_b200.jpeg.JpegEncoder, QUALITY, SUBSAMPLING), byte-identical to `encode`, Pillow's encoder: only the JPEG bytes
+come back to the host.  The video's list of JPEGs is stored under the same key, then `__keys__`, `__len__` and
+`__order__` as the RGB database has them and `__vlen__` with the flow frame counts (N - 1) in `__keys__` order.  The flow frames use the msgpack family (str or bin) of the RGB database's
 byte strings, `__keys__` and frames, so a reader of the RGB database reads this one.  A one-frame video gets an empty
 list.
 
@@ -20,13 +20,10 @@ import os
 import shutil
 import sys
 import time
-from concurrent.futures import ThreadPoolExecutor
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
-
-import numpy as np  # noqa: E402
 
 QUALITY = 95          # Pillow JPEG quality of a stored flow frame
 SUBSAMPLING = 0       # 4:4:4: the two flow channels are not smoothed by chroma subsampling
@@ -44,13 +41,14 @@ def encode(frame):
     return b.getvalue()
 
 
-def solve_video(dec, jpegs, pairs, name):
-    """uint8 [N - 1, H, W, 3] quantised flow frames (host) of one video's JPEG frames."""
+def solve_video(dec, enc, jpegs, pairs, name, stats):
+    """The JPEG files of one video's N - 1 quantised flow frames; stats["encode_s"] gains the encode time."""
+    import torch
     from coclr_b200 import flow
     from coclr_b200.jpeg import JpegFrameError
     n = len(jpegs)
     if n == 0:
-        return np.zeros((0, 1, 1, 3), np.uint8)
+        return []
     try:
         batch = dec.parse(jpegs)
     except JpegFrameError as e:
@@ -63,14 +61,17 @@ def solve_video(dec, jpegs, pairs, name):
     except ValueError as e:
         raise Refused("video %s: cannot decode %s" % (name, e))
     if n == 1:                                      # decoded all the same: a bad single frame is refused too
-        return np.zeros((0,) + sizes[0] + (3,), np.uint8)
+        return []
     grey = flow.grey(rgb)
-    h, w = sizes[0]
-    out = np.empty((n - 1, h, w, 3), np.uint8)
+    out = []
     for a in range(0, n - 1, pairs):
         b = min(a + pairs, n - 1)
         f, _ = flow.tvl1(grey[a:b], grey[a + 1:b + 1])
-        out[a:b] = flow.quantise(f).cpu().numpy()
+        q = flow.quantise(f)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        out += enc(q)                               # synchronises: the files are on the host when it returns
+        stats["encode_s"] += time.perf_counter() - t0
     return out
 
 
@@ -84,11 +85,11 @@ def frame_family(keys_value):
     return True if bt is None else bt
 
 
-def build(rgb_path, out_path, pairs, threads=None, log=print):
+def build(rgb_path, out_path, pairs, log=print):
     """Write the flow database of rgb_path to out_path (which must not exist); returns the run's figures."""
     import torch
     from coclr_b200 import lmdb_read, lmdb_write
-    from coclr_b200.jpeg import JpegDecoder
+    from coclr_b200.jpeg import JpegDecoder, JpegEncoder
     if os.path.exists(out_path):
         raise Refused("%s exists; remove it or choose another --out" % out_path)
     src = lmdb_read.open(rgb_path)
@@ -102,42 +103,24 @@ def build(rgb_path, out_path, pairs, threads=None, log=print):
     if not torch.cuda.is_available():
         raise Refused("no CUDA device: the flow is computed on the GPU")
     dec = JpegDecoder()
+    enc = JpegEncoder(QUALITY, SUBSAMPLING)
     vlen, stats = {}, {"videos": 0, "pairs": 0, "solve_s": 0.0, "encode_s": 0.0}
     t_start = time.perf_counter()
-
-    def timed_encode(frame):
-        t0 = time.perf_counter()
-        b = encode(frame)
-        return b, time.perf_counter() - t0
-
     writer = lmdb_write.Writer(out_path)
     try:
-        with ThreadPoolExecutor(threads or min(16, os.cpu_count() or 1)) as pool:
-            pending = None
-
-            def store(key, futures):
-                done = [f.result() for f in futures]
-                stats["encode_s"] += sum(t for _, t in done)
-                writer.put(key, lmdb_write.pack([b for b, _ in done], bt))
-                vlen[key] = len(done)
-
-            for key in sorted(set(keys)):
-                raw = src.get(key)
-                if raw is None:
-                    raise Refused("%s: key %s is listed in __keys__ but not stored" % (rgb_path, key.decode()))
-                i = int(key)
-                name = "%s (key %s)" % (order[i] if 0 <= i < len(order) else "?", key.decode())
-                t0 = time.perf_counter()
-                q = solve_video(dec, [bytes(f) for f in lmdb_read.unpack(raw)], pairs, name)
-                stats["solve_s"] += time.perf_counter() - t0
-                futures = [pool.submit(timed_encode, q[j]) for j in range(len(q))]
-                if pending is not None:
-                    store(*pending)
-                pending = (key, futures)
-                stats["videos"] += 1
-                stats["pairs"] += len(q)
-            if pending is not None:
-                store(*pending)
+        for key in sorted(set(keys)):
+            raw = src.get(key)
+            if raw is None:
+                raise Refused("%s: key %s is listed in __keys__ but not stored" % (rgb_path, key.decode()))
+            i = int(key)
+            name = "%s (key %s)" % (order[i] if 0 <= i < len(order) else "?", key.decode())
+            t0, e0 = time.perf_counter(), stats["encode_s"]
+            files = solve_video(dec, enc, [bytes(f) for f in lmdb_read.unpack(raw)], pairs, name, stats)
+            stats["solve_s"] += time.perf_counter() - t0 - (stats["encode_s"] - e0)
+            writer.put(key, lmdb_write.pack(files, bt))
+            vlen[key] = len(files)
+            stats["videos"] += 1
+            stats["pairs"] += len(files)
         writer.put(b"__keys__", special[b"__keys__"])
         writer.put(b"__len__", special[b"__len__"])
         writer.put(b"__order__", special[b"__order__"])
@@ -149,7 +132,7 @@ def build(rgb_path, out_path, pairs, threads=None, log=print):
         raise
     wall = time.perf_counter() - t_start
     stats["pairs_per_s"] = stats["pairs"] / wall if wall > 0 else 0.0
-    log("videos %d  pairs %d  pairs/s %.1f  solve %.1f s  encode %.1f s (thread time)"
+    log("videos %d  pairs %d  pairs/s %.1f  solve %.1f s  encode %.1f s (GPU, synchronised)"
         % (stats["videos"], stats["pairs"], stats["pairs_per_s"], stats["solve_s"], stats["encode_s"]))
     return stats
 
